@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 # -*- coding: utf-8 -*-
-"""bench.py -- the driver's benchmark contract for the WaveNet hot paths on B200.
+"""bench.py -- the benchmark of the WaveNet hot paths on the H100.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload train|decode]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload train|decode] [--dump-outputs DIR]
 
 Default workload = BASELINE.json configs[1]: arctic/sd 16 kHz, 3x10 dilation layers, 64 res / 512 skip,
 mu-law 256, aux 28 + UpSampling(80), batch 8 x 23 040-sample windows (20 000 nominal + receptive field,
@@ -16,9 +16,14 @@ that batch (reference bin/train.py:530-540) through ``pytorchwavenetvocoder_b200
             number of samples per utterance -- stated in the object;
   roofline= fused residual-block FORWARD kernel: algorithmic bytes s*(2R + A + 2S) per sample-layer
             (SURVEY.md 8d; 4 720 B fp32 at 64/512/28) x B*T per launch / mean launch time (CUDA events on
-            the launching stream, inside the timed steps) against MEASURED_PEAKS.json hbm_gbs;
+            the launching stream, inside the timed steps) against MEASURED_PEAKS.json hbm_gbs (else the H100 SXM
+            data-sheet 3.35 TB/s, reported as "fallback");
   cpu_baseline / --impl reference = oracle/torch_port.py (the reference's op sequence on torch CPU, all
             host threads) on a bounded sample (1 window per step).
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step computed as DIR/<name>.npy (float32 /
+float64, <= 64 MB in all): the loss, every parameter after the optimizer step and its gradient, and with the decode
+workload the generated samples.  Inputs and weights are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -36,7 +41,7 @@ import torch  # noqa: E402
 
 CFG = (256, 28, 64, 512, 10, 3, 2, 80)       # BASELINE.json configs[1] / north_star shape
 BATCH, BATCH_LENGTH = 8, 20000
-FALLBACK_HBM_GBS = 6650.0
+FALLBACK_HBM_GBS = 3350.0      # H100 SXM data sheet (HBM3); MEASURED_PEAKS.json overrides
 
 
 def _peaks():
@@ -48,16 +53,16 @@ def _peaks():
 
 
 def _tensor_peak():
-    """Sustained dense bf16 TFLOP/s of MEASURED_PEAKS.json (cuBLAS, back to back); kind::tf32 runs at half that rate."""
+    """Sustained dense bf16 TFLOP/s of MEASURED_PEAKS.json (cuBLAS, back to back); tf32 runs at half that rate."""
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["bf16_tflops_sustained"]), "measured"
     except Exception:
-        return 1443.0, "fallback"
+        return 989.0, "fallback"      # H100 SXM data sheet, dense BF16
 
 
 class ClockSampler(object):
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -213,6 +218,12 @@ def run_ours(args):
         barrier()
         ms = e0.elapsed_time(e1)
         launches = _lib.launch_count() - l0
+        if args.dump_outputs and rank == 0:     # (outside the timed region; the steps after this one do not change it)
+            DUMP["loss"] = loss.detach().double().cpu().numpy().reshape(1)
+            for name, prm in net.named_parameters():
+                DUMP["param." + name] = prm.detach().float().cpu().numpy()
+                if prm.grad is not None:
+                    DUMP["grad." + name] = prm.grad.detach().float().cpu().numpy()
         evs = wn.PROFILE_EVENTS or []
         wn.PROFILE_EVENTS = None
         blk_ms = [a.elapsed_time(b) for a, b in evs]
@@ -363,7 +374,7 @@ def run_ours(args):
         blk = float(np.mean(blk_ms)) if blk_ms else None
         ach = alg_bytes / (blk * 1e-3) / 1e9 if blk else None
         roof = {"kernel": "resblock_fwd (%s)" % args.math, "bound": "hbm", "achieved": ach, "peak": hbm,
-                "unit": "GB/s", "frac": (ach / hbm) if ach else None, "traffic": TRAFFIC_NCU.get(args.math),
+                "unit": "GB/s", "frac": (ach / hbm) if ach else None, "traffic": None,
                 "peak_source": how, "algorithmic_bytes_per_launch": alg_bytes,
                 "mean_launch_ms": blk, "launches_timed": len(blk_ms)}
         if not stack and args.math == "tf32" and R * R >= 256 * 256:
@@ -374,9 +385,9 @@ def run_ours(args):
             flops = 3.0 * fwd * float(Bq) * T
             pk, pk_how = _tensor_peak()
             ach_tf = flops / (per_step * 1e-3) / 1e12
-            roof = {"kernel": "whole step: every GEMM of the composed tcgen05 path (gemm_nt_tc / wgrad_tc kernels)",
+            roof = {"kernel": "whole step: every GEMM of the composed tensor-core path (gemm_nt_tc / wgrad_tc kernels)",
                     "bound": "tensor", "achieved": ach_tf, "peak": pk / 2, "unit": "TFLOP/s", "frac": ach_tf / (pk / 2),
-                    "traffic": None, "peak_source": pk_how + " bf16_tflops_sustained / 2 (kind::tf32 rate)",
+                    "traffic": None, "peak_source": pk_how + " bf16_tflops_sustained / 2 (tf32 rate)",
                     "flops_per_step": flops,
                     "note": "fwd FLOPs/sample = L*[2R^2(2ks+1)+4RA+2SR]+2S^2+2QS (SURVEY 8d), backward = 2x"}
         roof_all = None
@@ -397,9 +408,9 @@ def run_ours(args):
                 a = alg[name] / (mean * 1e-3) / 1e9
                 roof_all.append({"kernel": name, "launches_timed": n, "mean_launch_ms": mean,
                                  "share_of_step": tot / ms_prof, "algorithmic_bytes_per_launch": alg[name],
-                                 "achieved": a, "frac": a / hbm, "traffic": TRAFFIC_NCU_STACK.get(name)})
+                                 "achieved": a, "frac": a / hbm, "traffic": None})
             # the four per-block backward kernels against what ONE fused kernel per block would have to move
-            # (x, dout, dZ_all slice, aux in; dx out = s*(4R+Ap) per sample; DESIGN.md 3.2 says why it is not built)
+            # (x, dout, dZ_all slice, aux in; dx out = s*(4R+Ap) per sample; DESIGN.md 3.1 says why it is not built)
             byk = {r["kernel"]: r for r in roof_all}
             fused_ideal = None
             if all(k in byk for k in ("gate_bwd", "dx_gemm", "dw1", "dw2res")):
@@ -428,7 +439,7 @@ def run_ours(args):
                                    % (str(CFG).replace(" ", ""), BATCH, int(T)),
                        "global_batch": world * BATCH, "seq_len": int(T), "parallelism": "dp%d" % world,
                        "math": args.math, "storage": "fp32 channels-last",
-                       "l2": "per-step working set ~10 GB >> 126 MB L2 (no explicit flush needed)"},
+                       "l2": "per-step working set ~10 GB >> 50 MB L2 (no explicit flush needed)"},
             "e2e": {"value": samples / (ms_e2e / args.steps * 1e-3), "unit": "samples/s",
                     "h2d_bytes_per_step": int(xh.numel() * 8 + th.numel() * 8 + hh.numel() * 4),
                     "d2h_bytes_per_step": 4, "ms_per_step": ms_e2e / args.steps, "last_loss": last,
@@ -462,6 +473,8 @@ def run_ours(args):
         else:
             out["decode"] = dec
     if rank == 0:
+        if args.dump_outputs:
+            write_dump(args.dump_outputs)
         if world == 1 and args.cpu_baseline:
             out["cpu_baseline"] = cpu_baseline(args, out.get("config", {}).get("workload", ""),
                                                decode=(args.workload == "decode"))
@@ -470,17 +483,32 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the ncu --set full captures committed under profiles/
-# (filled in by hand from those captures; None = not captured)
-# per-block fused forward with skip accumulation (wnb_resblock_fwd): profiles/r1_ncu_resblock_fwd_tc_summary.txt
-TRAFFIC_NCU = {"fp32": None, "tf32": 814.14e6}
-# kernel kinds timed by wnb_profile_read (WNB_PROF_* order) and their ncu DRAM bytes per launch, round 2:
-# profiles/r2_ncu_fwdz_summary.txt (block forward: 70.9 MB read + 43.5 MB written -- the x(t-d) halo and part of the
-# z / xout stores live in the 126 MB L2), r2_ncu_nt_summary.txt (launch 0 skip GEMM, 5 dZ_all GEMM, 8 gate backward of a
-# block with a residual input, 9 its dX), r2_ncu_wg_summary.txt (2 dW1, 3 dW2res, 4/5 dWskip)
+# kernel kinds timed by wnb_profile_read (WNB_PROF_* order)
 STACK_KINDS = ["fwd_block", "skip_gemm", "dzall_gemm", "gate_bwd", "dx_gemm", "dw1", "dw2res", "dwskip"]
-TRAFFIC_NCU_STACK = {"fwd_block": 112.8e6, "skip_gemm": 1807.5e6, "dzall_gemm": 1740.2e6, "gate_bwd": 224.3e6,
-                     "dx_gemm": 204.5e6, "dw1": 4896.0e6, "dw2res": 2741.8e6, "dwskip": 1610.2e6}
+
+
+DUMP = {}                       # name -> array: what the last timed step computed (--dump-outputs)
+DUMP_BUDGET = 63 * 1024 * 1024       # (+ the .npy headers: <= 64 MB in all)
+
+
+def write_dump(out_dir):
+    """DUMP -> out_dir/<name>.npy.  If the arrays exceed DUMP_BUDGET in all, the largest ones are replaced by a fixed,
+    seeded sample of their elements (<name>.npy, flattened) with the sampled flat indices in <name>.index.npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = dict(DUMP)
+    total = sum(a.nbytes for a in arrays.values())
+    for name in sorted(arrays, key=lambda k: -arrays[k].nbytes):
+        if total <= DUMP_BUDGET:
+            break
+        a = arrays[name]
+        keep = (DUMP_BUDGET - (total - a.nbytes)) // (a.itemsize + 8)      # sampled values + float64 indices
+        keep = min(a.size, keep if keep > 0 else 1 << 16)                   # (<= 0: the next arrays are sampled too)
+        idx = np.sort(np.random.RandomState(0).choice(a.size, size=keep, replace=False))
+        arrays[name] = a.reshape(-1)[idx]
+        arrays[name + ".index"] = idx.astype(np.float64)
+        total = sum(v.nbytes for v in arrays.values())
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def run_decode(args, dev, rank, world, dist):
@@ -517,10 +545,12 @@ def run_decode(args, dev, rank, world, dist):
         l0 = _lib.launch_count()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        once(False)
+        gen_timed = once(False)
         e1.record()
         torch.cuda.synchronize()
         launches = _lib.launch_count() - l0
+        if args.dump_outputs and rank == 0:
+            DUMP["decode.samples"] = gen_timed.float().cpu().numpy()   # mu-law codes < 2^24: exact in float32
         ms = e0.elapsed_time(e1)
         t0 = time.time()
         once(True)
@@ -534,10 +564,11 @@ def run_decode(args, dev, rank, world, dist):
     wbytes = sum(p.numel() for p in net.parameters()) * 4
     kern = getattr(net, "last_decode_kernel", None)
     cl = int(lib.wnb_decode_warp_cluster(args.decode_utts)) if kern == "warp" else 1
-    nu = 1 if args.decode_utts <= 148 else (2 if args.decode_utts <= 296 else 4)
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    nu = 1 if args.decode_utts <= sms else (2 if args.decode_utts <= 2 * sms else 4)
     ctas = (args.decode_utts + nu - 1) // nu * cl
     us_step = ms * 1e3 / steps_incl_warmup
-    sm_mhz = 1965.0
+    sm_mhz = 1980.0      # H100 SXM boost clock; MEASURED_PEAKS.json sm_max_mhz overrides
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             sm_mhz = float(json.load(f).get("sm_max_mhz", sm_mhz))
@@ -549,7 +580,7 @@ def run_decode(args, dev, rank, world, dist):
     # with the FFMA GEMVs (128 B/clk shared-memory pipe); the HBM traffic per generated sample is < 10 B
     per_cta_bytes = wbytes / cl
     roof = {"bound": "per-sample dependency chain; per-SM L2->smem weight stream",
-            "kernel": "decode_%s_kernel, %d CTA(s) per utterance, %d CTAs on %d SMs" % (kern, cl, ctas, 148),
+            "kernel": "decode_%s_kernel, %d CTA(s) per utterance, %d CTAs on %d SMs" % (kern, cl, ctas, sms),
             "us_per_step": us_step, "sm_cycles_per_step": cyc_step,
             "smem_read_floor_cycles": per_cta_bytes / 128.0,
             "frac_of_smem_floor": (per_cta_bytes / 128.0) / cyc_step,
@@ -557,7 +588,7 @@ def run_decode(args, dev, rank, world, dist):
             "l2_to_sm_weight_stream_GBps": ctas * per_cta_bytes / (us_step * 1e-6) / 1e9,
             "algorithmic_hbm_bytes_per_sample": 4.0 * cfg.n_aux / max(U, 1) + 8.0,
             "flops_per_sample": 4.2e6, "achieved_tflops": n_utt_total * n / (ms * 1e-3) * 4.2e6 / 1e12,
-            "dram_bytes_ncu": DECODE_DRAM_NCU}
+            "dram_bytes_ncu": None}
     return {
         "metric": "autoregressive decode samples/s (persistent fast-generate kernel, sampling mode)",
         "value": n_utt_total * n / (ms * 1e-3), "unit": "samples/s", "n_gpus": world,
@@ -577,128 +608,9 @@ def run_decode(args, dev, rank, world, dist):
     }
 
 
-# ncu dram__bytes_read.sum / dram__bytes_write.sum of ONE decode launch (profiles/r2_ncu_decode_*.txt); None = not captured
-# profiles/r2_ncu_decode_summary.txt: decode_warp_kernel<1,16,1,2>, 64 utterances x (3069 warm-up + 1000) steps, 192 ms
-DECODE_DRAM_NCU = {"dram_read_bytes": 9.99e6, "dram_write_bytes": 59.75e6, "steps": 4069, "utterances": 64,
-                   "bytes_per_utterance_step": (9.99e6 + 59.75e6) / (64 * 4069),
-                   "l2_to_sm_bytes": 36325948200 * 32.0,
-                   "note": "the 786 KB/utterance dilation queues are written back once; weights and queue reads are L2 hits"}
-
-
-def _ref_nets():
-    """The UNMODIFIED reference ``wavenet_vocoder.nets.wavenet`` from git-ignored baseline/_ref (installed by
-    baseline/install_ref.py in the build container; it travels to the GPU box).  None if it is not there."""
-    try:
-        from baseline.install_ref import import_ref
-        return import_ref()
-    except Exception:
-        return None
-
-
-def _ref_model(R, seed=20260924):
-    torch.manual_seed(seed)
-    m = R.WaveNet(*CFG)
-    m.apply(R.initialize)
-    with torch.no_grad():
-        for name, prm in m.named_parameters():
-            if name.endswith("bias"):
-                prm.add_(0.05 * torch.randn_like(prm))
-    return m
-
-
-def _thread_candidates():
-    n = os.cpu_count() or 1
-    return [c for c in (4, 8, 16, 32, 64) if c <= n] or [n]
-
-
 def cpu_baseline(args, workload, decode=False, steps=None):
-    """The reference's own code on the host cores: baseline/_ref (kind "reference") when it travelled with the
-    snapshot, else oracle/torch_port.py (kind "port").  Bounded sample; the thread count is the best of a short
-    sweep (torch's CPU conv path collapses when oversubscribed: 183 s/step with 128 threads on the GPU host vs
-    1.2 s with 16), `cores` reports the threads actually used and `thread_sweep` the sweep."""
-    R = _ref_nets()
-    cfg = _Cfg(CFG)
-    rf = cfg.receptive_field
-    if R is None:
-        return _cpu_baseline_port(args, decode, steps)
-    Q = cfg.n_quantize
-    if decode:
-        m = _ref_model(R).eval()
-        B = 8
-        g = torch.Generator().manual_seed(1)
-        x = torch.full((B, 1), Q // 2, dtype=torch.int64)
-
-        def run(n):
-            h = torch.randn(B, cfg.n_aux, (n + 1 + cfg.upsampling_factor - 1) // cfg.upsampling_factor, generator=g)
-            t0 = time.time()
-            with torch.no_grad():
-                m.batch_fast_generate(x, h, [n] * B, None, "argmax")
-            return time.time() - t0
-        sweep = {}
-        run(4)                         # one-time initialisations out of the way
-        for c in _thread_candidates():
-            torch.set_num_threads(c)
-            run(4)
-            a, b = run(8), run(48)
-            sweep[c] = B * 40 / (b - a) if b - a > 1e-3 else 0.0
-            if c >= 16 and sweep[c] < 0.5 * max(sweep.values()):
-                break
-        cores = max(sweep, key=sweep.get)
-        torch.set_num_threads(cores)
-        a, b = run(20), run(100)      # differencing removes the receptive-field warm-up (BASELINE.md section 2)
-        v = B * 80 / max(b - a, 1e-9)
-        return {"value": v, "unit": "samples/s", "cores": cores, "kind": "reference",
-                "sample": "reference batch_fast_generate B=8 argmax, 100 vs 20 samples differenced, torch CPU fp32",
-                "thread_sweep": {str(k): v_ for k, v_ in sweep.items()}}
-    m = _ref_model(R).train()
-    crit = torch.nn.CrossEntropyLoss()
-    opt = torch.optim.Adam(m.parameters(), lr=1e-4)
-
-    def step(x, h, t):
-        y = m(x, h)
-        loss = crit(y[:, rf:].contiguous().view(-1, Q), t[:, rf:].contiguous().view(-1))   # reference train.py:534-536
-        opt.zero_grad()
-        loss.backward()
-        opt.step()
-        return float(loss.detach())
-
-    # thread sweep on a short window (rf + 130 samples -> 3200), one warm-up + one timed step each
-    U = cfg.upsampling_factor
-    gs = torch.Generator().manual_seed(7)
-    Ts = ((rf + 130 + U - 1) // U) * U
-    xs_ = torch.randint(0, Q, (1, Ts + 1), generator=gs)
-    hs_ = torch.randn(1, cfg.n_aux, Ts // U, generator=gs)
-    sweep = {}
-    for c in _thread_candidates():
-        torch.set_num_threads(c)
-        step(xs_[:, :-1], hs_, xs_[:, 1:])
-        t0 = time.time()
-        step(xs_[:, :-1], hs_, xs_[:, 1:])
-        sweep[c] = time.time() - t0
-        if c >= 16 and sweep[c] > 2.0 * min(sweep.values()):
-            break      # oversubscription cliff: do not go further up
-    cores = min(sweep, key=sweep.get)
-    torch.set_num_threads(cores)
-    x, h, t = synth_batch(cfg, 0, 1, pinned=False)
-    t0 = time.time()
-    step(x, h, t)
-    warm = time.time() - t0
-    k = steps or 2
-    if warm > 15.0:       # keep the whole baseline leg bounded: count the warm-up step itself
-        k, dt = 1, warm
-    else:
-        t0 = time.time()
-        for _ in range(k):
-            step(x, h, t)
-        dt = (time.time() - t0) / k
-    return {"value": BATCH_LENGTH / dt, "unit": "samples/s", "cores": cores, "kind": "reference",
-            "sample": "%d step(s) of 1 x %d-sample window (fwd+CE+bwd+Adam) through the unmodified reference "
-                      "wavenet_vocoder.nets.WaveNet (baseline/_ref), torch CPU fp32, after 1 warm-up" % (k, x.shape[1]),
-            "sec_per_step": dt, "thread_sweep_sec_short_window": {str(k_): v_ for k_, v_ in sweep.items()}}
-
-
-def _cpu_baseline_port(args, decode=False, steps=None):
-    """Fallback when baseline/_ref did not travel: the reference's op sequence restated on torch CPU ops."""
+    """The reference's op sequence restated on torch CPU ops (oracle/torch_port.py, kind "port") on the host cores;
+    bounded sample."""
     from oracle import torch_port as TP
     from oracle import wavenet_oracle as O
     cores = min(os.cpu_count() or 1, 16)
@@ -726,7 +638,7 @@ def _cpu_baseline_port(args, decode=False, steps=None):
     TP.train_step(cfg, p, opt, x, h, t)
     warm = time.time() - t0
     k = steps or 2
-    if warm > 15.0:
+    if warm > 15.0 and steps is None:
         k, dt = 1, warm
     else:
         t0 = time.time()
@@ -744,7 +656,7 @@ def run_reference(args):
         return
     cfg = _Cfg(CFG)
     decode = args.workload == "decode"
-    k = max(1, min(args.steps, 3))
+    k = max(1, args.steps)
     cb = cpu_baseline(args, "", decode=decode, steps=k)
     world = int(os.environ.get("WORLD_SIZE", 1))
     out = {
@@ -766,7 +678,8 @@ def run_reference(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--steps", type=int, default=5,
+                    help="timed training steps (the decode leg always times one full decode of --decode-utts utterances)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="train", choices=["train", "decode"])
@@ -782,6 +695,8 @@ def main():
                     help="samples per utterance (configs[3]: 2000 frames x 80 - 1 = 159 999, reference decode.py:158)")
     ap.add_argument("--batch-length", type=int, default=None, help="override the nominal batch length (default 20000)")
     ap.add_argument("--fp32-line", type=int, default=1, help="also time a few steps of the fp32 FFMA parity mode")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
     global CFG, BATCH, BATCH_LENGTH
     if args.batch_length:

@@ -1,5 +1,5 @@
 /*
- * wnb200.h -- C ABI of libwnb200.so, the B200 (sm_100a) kernels behind the WaveNet vocoder hot paths.
+ * wnb200.h -- C ABI of libwnb200.so, the H100 (sm_90a) kernels behind the WaveNet vocoder hot paths.
  *
  * The reference (kan-bayashi/PytorchWaveNetVocoder v0.1.1) is pure Python on top of torch: it has no
  * FFI layer of its own (SURVEY.md 8b).  This header is therefore OUR drop-in boundary: each entry
@@ -50,7 +50,7 @@ extern "C" {
 #define WNB_ERR_UNSUPPORTED (-3)
 
 #define WNB_MATH_FP32 0        /* SIMT FFMA, fp32 throughout (parity mode) */
-#define WNB_MATH_TF32 1        /* tcgen05 kind::tf32 contractions, fp32 accumulate in TMEM */
+#define WNB_MATH_TF32 1        /* wgmma tf32 contractions, fp32 accumulate */
 
 #define WNB_MODE_ARGMAX 0
 #define WNB_MODE_SAMPLING 1
@@ -96,7 +96,8 @@ WNB_API int wnb_resblock_fwd(const float* xin, const float* haux, const float* w
                      int B, int T, int R, int S, int Ap, int ks, int dilation, int skip_init,
                      int math_mode, void* stream);
 
-/* 1 = fused kernel, 2 = composed tcgen05 path (pass the zsave scratch), 0 = not covered by math_mode */
+/* tf32: 1 = fused per-block kernel (no zsave), 2 = composed tensor-core path (zsave optional), 0 = not covered;
+   fp32: 1 = covered, 0 = not */
 WNB_API int wnb_resblock_fwd_supported(int R, int S, int Ap, int ks, int math_mode);
 
 /* ---- a5 standalone: CausalConv1d.forward (wavenet.py:95-121), channels-last, fp32 FFMA, forward only.

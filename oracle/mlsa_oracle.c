@@ -2,8 +2,8 @@
  * through pysptk (reference wavenet_vocoder/bin/noise_shaping.py:28-43 `pysptk.mc2b`, :57-87
  * `pysptk.synthesis.Synthesizer(pysptk.synthesis.MLSADF(order, alpha), hopsize).synthesis(x, tiled_coef)`).
  *
- * pysptk (requirements: `pysptk>=0.1.17`, reference setup.py) is a Cython wrapper of SPTK 3.11 and is NOT in
- * /root/reference or this image, so this file restates the PUBLISHED algorithm of SPTK's `mc2b` and `mlsadf`
+ * pysptk (requirements: `pysptk>=0.1.17`, reference setup.py) is a Cython wrapper of SPTK 3.11 and is NOT part of
+ * the reference or a dependency here, so this file restates the PUBLISHED algorithm of SPTK's `mc2b` and `mlsadf`
  * (Imai, Sumita, Furuichi: "Mel log spectrum approximation (MLSA) filter for speech synthesis", 1983; SPTK reference
  * manual, commands mc2b / mlsadf): a cascade of two Pade approximants (order pd = 4 or 5) of exp(), the first over the
  * b[1] basic filter, the second over the FIR part b[2..m] on a chain of first-order all-pass sections, and pysptk's

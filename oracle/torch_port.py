@@ -6,8 +6,8 @@ restates the SAME path with the SAME torch CPU operators the reference module is
 (``F.conv1d`` with dilation + trim, one-hot scatter, ``conv_transpose2d``, cat/slice queue updates,
 reference wavenet_vocoder/nets/wavenet.py:78-154, 212-241, 309-395, 397-511, 525-549) so that its
 wall-clock is representative of "the reference's own CPU implementation" on the host cores.  It is
-what ``bench.py`` times for ``cpu_baseline`` and for ``--impl reference`` (kind = "port": the Python
-reference itself cannot travel to the GPU box, see the task's tier rules).  It is checked against
+what ``bench.py`` times for ``cpu_baseline`` and for ``--impl reference`` (kind = "port": the
+repository does not carry the original Python package).  It is checked against
 the numpy oracle / golden vectors in tests/test_torch_port.py.
 
 Parameters: dict keyed by the reference state_dict names -> torch tensors (fp32).

@@ -11,7 +11,7 @@ follows.  Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s cpu_ba
 
 Parity pinning: the reference ships no golden vectors (its tests are unseeded
 self-consistency checks, SURVEY.md section 4), so this oracle is pinned against the reference
-module itself, imported from /root/reference in the build container by
+module itself, imported from a checkout of the original project by
 ``tests/golden/make_golden.py``; the resulting vectors are committed under ``tests/golden/``
 and ``tests/test_oracle_golden.py`` checks the oracle against them on every CPU run.
 

@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""pytorchwavenetvocoder_b200 -- B200 (sm_100a) native WaveNet vocoder hot paths.
+"""pytorchwavenetvocoder_b200 -- H100 (sm_90a) native WaveNet vocoder hot paths.
 
 Drop-in for the two hot paths of kan-bayashi/PytorchWaveNetVocoder (training forward/backward through
 the residual stack, autoregressive fast generation) behind the reference's own module surface

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 # -*- coding: utf-8 -*-
-"""DECODE WITH WAVENET VOCODER -- B200 build of ``wavenet_vocoder/bin/decode.py`` (reference v0.1.1).
+"""DECODE WITH WAVENET VOCODER -- H100 build of ``wavenet_vocoder/bin/decode.py`` (reference v0.1.1).
 
 Same flags (reference decode.py:179-204), same inputs (``model.conf``, ``checkpoint*.pkl`` with key
 ``"model"``, feature ``.h5`` files, ``stats.h5``) and outputs (``{feat_id}.wav`` PCM_16 at ``--fs``).

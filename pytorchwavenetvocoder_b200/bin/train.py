@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 # -*- coding: utf-8 -*-
-"""TRAIN WAVENET VOCODER -- B200 build of ``wavenet_vocoder/bin/train.py`` (reference v0.1.1).
+"""TRAIN WAVENET VOCODER -- H100 build of ``wavenet_vocoder/bin/train.py`` (reference v0.1.1).
 
 Same command line (reference train.py:337-394), same ``model.conf`` / ``checkpoint-*.pkl`` formats
 (:315-332, :429, :564-568), same batching arithmetic (``train_generator`` :67-312), same loop (:530-561).
-What changes underneath: ``WaveNet`` is the sm_100a kernel build, the loss is the fused CE kernel, and
+What changes underneath: ``WaveNet`` is the sm_90a kernel build, the loss is the fused CE kernel, and
 ``--n_gpus N`` means N *processes* (the command re-launches itself under ``torch.distributed.run``; one rank per
 GPU, a single flat NCCL all-reduce of the gradients per step) instead of single-process ``nn.DataParallel``
 (:449-454).  ``--batch_size`` stays the GLOBAL batch: every rank trains on ``batch_size / n_gpus`` windows of it.  Extra, optional flags: ``--math_mode {tf32,fp32}``.
@@ -206,9 +206,9 @@ def get_parser():
     parser.add_argument("--n_gpus", default=1, type=int, help="number of gpus")
     parser.add_argument("--verbose", default=1, type=int, help="log level")
     parser.add_argument("--math_mode", default="tf32", choices=["tf32", "fp32"], type=str,
-                        help="(B200 build) contraction precision of the training kernels")
+                        help="(H100 build) contraction precision of the training kernels")
     parser.add_argument("--host_loader", default=False, type=_strtobool,
-                        help="(B200 build) build the mini-batches on the host like the reference instead of on the GPU")
+                        help="(H100 build) build the mini-batches on the host like the reference instead of on the GPU")
     return parser
 
 
@@ -239,7 +239,7 @@ def main():
     local = int(os.environ.get("LOCAL_RANK", 0))
     if args.n_gpus > 1 and "WORLD_SIZE" not in os.environ:
         # the recipes call `train.py --n_gpus N` as ONE process (reference nn.DataParallel, train.py:449-454); the
-        # B200 build runs one process per GPU, so re-launch this command line under torch.distributed.run
+        # this build runs one process per GPU, so re-launch this command line under torch.distributed.run
         import socket
         with socket.socket() as s_:
             s_.bind(("127.0.0.1", 0))

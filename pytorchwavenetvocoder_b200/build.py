@@ -1,11 +1,11 @@
 # -*- coding: utf-8 -*-
-"""Build libwnb200.so (hand-written sm_100a kernels + C ABI) in-tree with nvcc.
+"""Build libwnb200.so (hand-written sm_90a kernels for the H100 + C ABI) in-tree with nvcc.
 
     python -m pytorchwavenetvocoder_b200.build [--force]
 
 The library is a plain C-ABI shared object (no torch headers); cudart is linked statically and the
 driver API (TMA descriptor encoding) is resolved at run time through cudaGetDriverEntryPoint, so the
-.so loads on a machine without a GPU (CPU test tier) and travels to the GPU box with the snapshot.
+.so loads on a machine without a GPU (CPU test tier).
 """
 import os
 import subprocess
@@ -14,8 +14,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libwnb200.so")
-SOURCES = ["elementwise.cu", "resblock_simt.cu", "resblock_tc.cu", "decode.cu", "decode_stream.cu", "wgrad_tc.cu", "decode_warp.cu", "gemm_nt_tc.cu", "resblock_z.cu", "stack.cu", "pack.cu", "loader.cu", "mlsa.cu", "adam.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+SOURCES = ["elementwise.cu", "resblock_simt.cu", "decode.cu", "decode_stream.cu", "wgrad_tc.cu", "decode_warp.cu", "gemm_nt_tc.cu", "resblock_z.cu", "stack.cu", "pack.cu", "loader.cu", "mlsa.cu", "adam.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--fmad=true", "-cudart", "static"]
 
 

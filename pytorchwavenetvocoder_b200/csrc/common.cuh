@@ -49,6 +49,10 @@ cudaError_t ensure_dynamic_smem(const void* func, size_t bytes);
 // get different words and may run concurrently; launches on one stream are ordered.  A few bytes per stream, allocated
 // on first use and kept for the life of the process (library state, not a caller-visible buffer).
 unsigned int* sched_counters(cudaStream_t st);
+// Device scratch owned by (current device, stream, slot), grown on demand (an outgrown buffer stays allocated, so a
+// pointer handed out earlier remains valid).  Used for the per-CTA partial sums that make the gradient reductions independent of scheduling.
+void* scratch_buffer(cudaStream_t st, int slot, size_t bytes);
+enum { SCRATCH_WGRAD = 0, SCRATCH_EMBED = 1, SCRATCH_AUX = 2, SCRATCH_LOSS = 3, SCRATCH_EMBED_PART = 4 };
 
 #define WNB_REQUIRE(cond, ...)            \
   do {                                    \

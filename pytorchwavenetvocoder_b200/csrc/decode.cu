@@ -9,7 +9,7 @@
 //
 // Per step every matrix-vector product is a K-major GEMV: warp lanes read 512 contiguous bytes of one
 // weight row (float4 per lane) and broadcast the activation from shared memory, so the weight stream
-// (8.6 MB fp32 at 64/512, resident in the 126 MB L2) is perfectly coalesced; K is split over the CTA's
+// (8.6 MB fp32 at 64/512, resident in the 50 MB L2) is perfectly coalesced; K is split over the CTA's
 // warps and reduced through shared memory.  The dilation queues (786 KB fp32 per utterance at 64/512)
 // live in global memory but are L2 resident; all (ks-1)*L taps of a step are prefetched at the top of
 // the step because they only depend on earlier steps.  fp32 FFMA throughout: autoregressive argmax
@@ -394,9 +394,9 @@ WNB_API int wnb_decode(int32_t* xs, const float* h, const float* up_w, const flo
   p.q_per_utt = off;
 
   // utterances per CTA: share the weight stream between utterances once there are more utterances than
-  // SMs; stay at 1 while B <= 148 so that every utterance gets its own SM's L2 port.
+  // SMs; stay at 1 while B <= the SM count so that every utterance gets its own SM's L2 port.
   int NU = 1;
-  if (B > 148 * 2) NU = 4; else if (B > 148) NU = 2;
+  if (B > device_sms() * 2) NU = 4; else if (B > device_sms()) NU = 2;
   size_t smem = 0;
   for (;;) {
     smem = decode_smem_floats(NU, R, S, p.Qp, Ap, ks, L, p.O1, p.O2, p.Sp) * sizeof(float);

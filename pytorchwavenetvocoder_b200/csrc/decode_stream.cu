@@ -407,7 +407,7 @@ int decode_stream_launch(StreamParams& p, cudaStream_t st) {
     if (widths[i] % 4 != 0 || widths[i] / 4 > kConsThreads || widths[i] * 4 > kChunkBytes) return WNB_ERR_UNSUPPORTED;
   if (p.L > kMaxLayersS || p.R % 4 != 0 || p.S % 4 != 0 || p.Ap % 4 != 0) return WNB_ERR_UNSUPPORTED;
   int NU = 1;
-  if (p.B > 148 * 2) NU = 4; else if (p.B > 148) NU = 2;
+  if (p.B > device_sms() * 2) NU = 4; else if (p.B > device_sms()) NU = 2;
   size_t work = 0, smem = 0;
   int nslot = 0;
   for (;;) {

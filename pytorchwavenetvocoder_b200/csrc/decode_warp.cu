@@ -18,7 +18,7 @@
 // stream, whichever is slower; utterances sharing a CTA (NU = 2, 4) reuse both.
 // Numerics identical in kind to v1/v2: fp32 FFMA, precise expf/tanhf, first-max argmax, Philox sampling.
 //
-// CL = 2 (batches of <= 74 utterances): ONE UTTERANCE PER 2-CTA CLUSTER.  The 16 "virtual" consumer warps of the
+// CL = 2 (batches of at most half the SM count): ONE UTTERANCE PER 2-CTA CLUSTER.  The 16 "virtual" consumer warps of the
 // single-CTA form are split over the two CTAs (8 each); each CTA streams only ITS warps' half of every matrix
 // (4.3 MB instead of 8.6 MB per step through its L2 -> shared-memory path, the measured bound), computes its half of
 // every output vector and stores it into BOTH CTAs' shared memory (st.shared::cluster, 64..512 floats per phase);
@@ -35,7 +35,7 @@ namespace dw {
 
 constexpr int kR = 64, kS = 512, kQ = 256, kAp = 32, kK1 = 160;
 // W = consumer warps (8 or 16).  More warps = more latency hiding for the dependent smem->FMA chains
-// (the kernel is issue-latency bound, the weight stream is always ahead: see profiles/r1_decode_notes.md).
+// (the kernel is issue-latency bound, the weight stream is always ahead).
 constexpr int kSlot = 32 * 1024;          // ring slot: 32 KB, or 2 * kSlot when the BIG (64 KB) schedule is used
 constexpr int kMaxL = 64;
 // stream layout per layer (floats), G = 32 / W groups of 4 gate values, H = 16 / W groups of 4 res values:
@@ -448,14 +448,6 @@ __global__ void __launch_bounds__((W / CL) * 32 + 64, 1) decode_warp_kernel(cons
     WNB_T(0);
     cons_sync_w<WP>();     // (CTA-local: the prologue only touches this CTA's shared memory)
     WNB_T(1);
-    // layer 0's input (the front output) goes into its queue only now, after every tap has been read
-    for (int e = tid; e < NU * kR; e += kCons) {
-      const int u = e >> 6, r = e & 63;
-      if (u0 + u < p.B) {   // (CL == 2: both CTAs hold the same values and both write them)
-        float* q0 = p.queues + (size_t)(u0 + u) * p.q_per_utt + p.qoff[0];
-        __stcg(q0 + (size_t)(pos & (p.dil[0] - 1)) * kR + r, cur[e]);
-      }
-    }
 
     float skip_tot[NU][SL];
 #pragma unroll
@@ -548,6 +540,14 @@ __global__ void __launch_bounds__((W / CL) * 32 + 64, 1) decode_warp_kernel(cons
         __syncwarp();
         if (lane < CH * NU) {
           const int u = lane / CH, cc = lane % CH, c = vw * CH + cc;
+          // Layer 0's input (the front output) goes into its queue here, not in the prologue: the slot is the one this step's
+          // taps were read from, and with CL == 2 the peer reads them while picking the previous sample (the next-step
+          // prefetch) -- a peer already in this step's prologue could overwrite the slot under that read.  Past the z
+          // hand-over of layer 0 both CTAs have read all their taps; each writes its own channels, like the other layers.
+          if (l == 0 && u0 + u < p.B) {
+            float* q0 = p.queues + (size_t)(u0 + u) * p.q_per_utt + p.qoff[0];
+            __stcg(q0 + (size_t)(pos & (p.dil[0] - 1)) * kR + c, cur[u * kR + c]);
+          }
           const float v = my_pre[u * CH + cc] + res_b + cur[u * kR + c];
           st_both<CL>(&cur[u * kR + c], v, peer_delta, xs_.peer_bar());
           if (l + 1 < L && u0 + u < p.B) {   // input of layer l+1 at time `pos` -> its dilation queue
@@ -815,14 +815,16 @@ __global__ void __launch_bounds__((W / CL) * 32 + 64, 1) decode_warp_kernel(cons
 }  // namespace dw
 
 // utterances per CTA, consumer warps and cluster size for a batch of B utterances (shared by the packer and the
-// launcher).  Up to 74 utterances (half the SMs): one utterance per 2-CTA cluster, so that 2 B SMs stream the weights.
+// launcher).  Up to half the SM count of utterances: one utterance per 2-CTA cluster, so that 2 B SMs stream the
+// weights and every cluster is resident at once (the kernel runs one CTA per SM: more clusters would run as a second
+// wave and double the decode time).
 static void decode_warp_plan(int B, int* NU, int* W, int* CL) {
   int nu = 1;
-  if (B > 148 * 2) nu = 4; else if (B > 148) nu = 2;
+  if (B > device_sms() * 2) nu = 4; else if (B > device_sms()) nu = 2;
   *NU = nu;
   *W = (nu == 4) ? 8 : 16;   // 16 warps hide the smem->FMA latency; NU = 4 needs the registers of the 8-warp form
   static const int cl_on = [] { const char* e = getenv("WNB_DECODE_CL"); return (e && e[0] == '1') ? 0 : 1; }();
-  *CL = (cl_on && B <= 74) ? 2 : 1;
+  *CL = (cl_on && B <= device_sms() / 2) ? 2 : 1;
 }
 
 int decode_warp_launch(dw::Params& p, int W_packed, int CL_packed, cudaStream_t st) {

@@ -8,6 +8,8 @@
 #include <atomic>
 #include <map>
 #include <mutex>
+#include <tuple>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -36,9 +38,9 @@ static std::mutex g_state_mu;
 int device_sms() {
   static int sms[64] = {};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   std::lock_guard<std::mutex> lk(g_state_mu);
-  if (!sms[dev] && cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms[dev] = 148;
+  if (!sms[dev] && cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms[dev] = 132;
   return sms[dev];
 }
 cudaError_t ensure_dynamic_smem(const void* func, size_t bytes) {
@@ -68,6 +70,27 @@ unsigned int* sched_counters(cudaStream_t st) {
   return p;
 }
 
+void* scratch_buffer(cudaStream_t st, int slot, size_t bytes) {
+  // A buffer that has been outgrown is kept, not freed: work already queued on the stream, or another host thread that
+  // obtained it, may still use it.  Sizes grow geometrically, so what is kept is less than the live buffer.
+  struct Buf { void* p; size_t n; };
+  static std::mutex mu;
+  static std::map<std::tuple<int, cudaStream_t, int>, Buf> bufs;
+  static std::vector<void*> retired;
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
+  std::lock_guard<std::mutex> lk(mu);
+  Buf& b = bufs[std::make_tuple(dev, st, slot)];
+  if (b.n < bytes) {
+    const size_t n = bytes > 2 * b.n ? bytes : 2 * b.n;
+    void* p = nullptr;
+    if (cudaMalloc(&p, n) != cudaSuccess) return nullptr;
+    if (b.p) retired.push_back(b.p);
+    b.p = p; b.n = n;
+  }
+  return b.p;
+}
+
 // ---- per-launch event timing (off by default; bench.py switches it on for the timed region) ----
 struct ProfRec { int kind; cudaEvent_t e0, e1; };
 static bool g_prof_on = false;
@@ -92,7 +115,7 @@ void prof_end(int kind, cudaStream_t st) {
 
 static int grid_for(int64_t work_items, int threads) {
   int64_t blocks = (work_items + threads - 1) / threads;
-  const int64_t cap = 148 * 16;  // 16 resident 256-thread CTAs per SM is plenty for streaming kernels
+  const int64_t cap = (int64_t)device_sms() * 16;  // 16 resident 256-thread CTAs per SM is plenty for streaming kernels
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   return (int)blocks;
@@ -223,69 +246,119 @@ __global__ void __launch_bounds__(256) front_embed_fwd_v4_kernel(const int64_t* 
   }
 }
 
-// dwf[k][q][r] += dout[b][t][r] for q = x[b][t-(ks-1-k)];  dbias[r] += sum dout
-__global__ void front_embed_bwd_kernel(const int64_t* __restrict__ x, const float* __restrict__ dout,
-                                       float* __restrict__ dwf, float* __restrict__ dbias, int B, int T, int Q,
-                                       int R, int ks, int rows_per_block) {
-  // block handles rows [row0, row0+rows_per_block); thread -> channel r (strided), loops over rows
-  const int64_t row0 = (int64_t)blockIdx.x * rows_per_block;
-  const int64_t nrows = (int64_t)B * T;
-  for (int r = threadIdx.x; r < R; r += blockDim.x) {
-    float bsum = 0.f;
-    for (int64_t row = row0; row < row0 + rows_per_block && row < nrows; row++) {
-      const float g = dout[row * R + r];
-      bsum += g;
-      const int t = (int)(row % T);
-      for (int k = 0; k < ks; k++) {
-        const int s = ks - 1 - k;
-        if (t - s >= 0) {
-          int64_t q = x[row - s] % Q;
-          if (q < 0) q += Q;
-          atomicAdd(dwf + ((size_t)k * Q + q) * R + r, g);
-        }
-      }
-    }
-    atomicAdd(dbias + r, bsum);
+// dwf[k][q][r] += sum of dout[b][t][r] over the rows whose tap-k token x[b][t-(ks-1-k)] is q.  A scatter by token:
+// instead of atomics (whose order depends on scheduling), block q scans all rows and owns row q of every tap's table,
+// so each sum is taken in one fixed order.  Threads: `lanes` time lanes x Rv channel groups of V floats; lane l takes the
+// rows l, l + lanes, ... and the lanes are added in lane order.  The tap with no shift sees every row exactly once, so
+// its per-token sums (qpart) add up to the bias gradient.
+// tok[row] = x[row] mod Q in [0, Q): computed once per call instead of in every block of the scan below
+__global__ void token_kernel(const int64_t* __restrict__ x, int* __restrict__ tok, int64_t n, int Q) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    int64_t q = x[i] % Q;
+    tok[i] = (int)(q < 0 ? q + Q : q);
   }
 }
-// One thread per (row, 4 channels): a 16-byte load of dout and ONE 16-byte vector reduction per tap into the
-// (ks, Q, R) table (a quarter of the L2 atomic operations of the scalar kernel above: 96 -> ~30 us at the bench shape);
-// the bias gradient is summed in registers over the rows a thread owns and reduced once per block.
-// (A shared-memory private table per CTA was tried: float atomics in shared memory are CAS loops -- 435 us.)
-__global__ void __launch_bounds__(256) front_embed_bwd_v4_kernel(const int64_t* __restrict__ x, const float4* __restrict__ dout,
-                                                                 float* __restrict__ dwf, float* __restrict__ dbias, int B,
-                                                                 int T, int Q, int R4, int ks) {
-  const int rows_per_blk = blockDim.x / R4;                 // host guarantees blockDim.x % R4 == 0, R4 <= 64
-  const int lr = threadIdx.x / R4, r4 = threadIdx.x - lr * R4;
+template <int V>
+__global__ void __launch_bounds__(512) front_embed_bwd_kernel(const int* __restrict__ tok, const float* __restrict__ dout,
+                                                              float* __restrict__ dwf, float* __restrict__ qpart, int B, int T,
+                                                              int Q, int Rv, int ks) {
+  typedef typename std::conditional<V == 4, float4, float>::type vec;
+  constexpr int kMaxKs = 4;
+  const int q = blockIdx.x;
+  const int lanes = blockDim.x / Rv;
+  const int lr = threadIdx.x / Rv, rv = threadIdx.x - lr * Rv;
+  const vec* dv = reinterpret_cast<const vec*>(dout);
+  float acc[kMaxKs][V];
+#pragma unroll
+  for (int k = 0; k < kMaxKs; k++)
+#pragma unroll
+    for (int i = 0; i < V; i++) acc[k][i] = 0.f;
+  for (int b = 0; b < B; b++)
+  for (int t = lr; t < T; t += lanes) {
+    const int64_t row = (int64_t)b * T + t;
+#pragma unroll
+    for (int k = 0; k < kMaxKs; k++) {
+      if (k >= ks) break;
+      const int s_ = ks - 1 - k;
+      if (t - s_ < 0 || __ldg(tok + row - s_) != q) continue;
+      const vec g = __ldg(dv + row * Rv + rv);
+      const float* gf = reinterpret_cast<const float*>(&g);
+#pragma unroll
+      for (int i = 0; i < V; i++) acc[k][i] += gf[i];
+    }
+  }
+  __shared__ float red[512 * V];
+  for (int k = 0; k < ks && k < kMaxKs; k++) {
+#pragma unroll
+    for (int i = 0; i < V; i++) red[threadIdx.x * V + i] = acc[k][i];
+    __syncthreads();
+    if (lr == 0) {
+      float sum[V];
+#pragma unroll
+      for (int i = 0; i < V; i++) sum[i] = 0.f;
+      for (int l = 0; l < lanes; l++)
+#pragma unroll
+        for (int i = 0; i < V; i++) sum[i] += red[(l * Rv + rv) * V + i];
+      float* dst = dwf + ((size_t)k * Q + q) * Rv * V + (size_t)rv * V;
+#pragma unroll
+      for (int i = 0; i < V; i++) dst[i] += sum[i];
+      if (k == ks - 1)
+#pragma unroll
+        for (int i = 0; i < V; i++) qpart[((size_t)q * Rv + rv) * V + i] = sum[i];
+    }
+    __syncthreads();
+  }
+}
+// Chunked form of the same sums, for tables that fit in shared memory: block c owns rows [c * chunk, (c + 1) * chunk)
+// and builds its own (ks, Q, R) table there.  Thread (qg, rv) owns the entries of the tokens q with q % QG == qg and
+// channel group rv, and walks the block's rows in order, so every entry is summed in one fixed order without atomics;
+// the per-chunk tables are then added in chunk order (front_embed_reduce_kernel).
+__global__ void __launch_bounds__(256) front_embed_bwd_chunk_kernel(const int* __restrict__ tok, const float4* __restrict__ dout,
+                                                                    float* __restrict__ part, int B, int T, int Q, int R4, int ks,
+                                                                    int64_t chunk) {
+  extern __shared__ float4 tab[];                    // [ks][Q][R4]
+  const int QG = blockDim.x / R4;
+  const int qg = threadIdx.x / R4, rv = threadIdx.x - qg * R4;
+  const int n4 = ks * Q * R4;
+  for (int i = threadIdx.x; i < n4; i += blockDim.x) tab[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  __syncthreads();
   const int64_t nrows = (int64_t)B * T;
-  float4 bs = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int64_t row = (int64_t)blockIdx.x * rows_per_blk + lr; row < nrows; row += (int64_t)gridDim.x * rows_per_blk) {
-    const float4 g = __ldg(dout + row * R4 + r4);
-    bs.x += g.x; bs.y += g.y; bs.z += g.z; bs.w += g.w;
-    const int t = (int)(row % T);
+  const int64_t row0 = (int64_t)blockIdx.x * chunk;
+  const int64_t row1 = row0 + chunk < nrows ? row0 + chunk : nrows;
+  int t = (int)(row0 % T);
+  for (int64_t row = row0; row < row1; row++) {
     for (int k = 0; k < ks; k++) {
       const int s_ = ks - 1 - k;
-      if (t - s_ >= 0) {
-        int64_t q = x[row - s_] % Q;
-        if (q < 0) q += Q;
-        float* dst = dwf + (((size_t)k * Q + q) * R4 + r4) * 4;
-        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(g.x), "f"(g.y), "f"(g.z), "f"(g.w)
-                     : "memory");
-      }
+      if (t - s_ < 0) continue;
+      const int q = __ldg(tok + row - s_);
+      if (q % QG != qg) continue;
+      const float4 g = __ldg(dout + row * R4 + rv);
+      float4& e = tab[((size_t)k * Q + q) * R4 + rv];
+      e.x += g.x; e.y += g.y; e.z += g.z; e.w += g.w;
     }
+    if (++t == T) t = 0;
   }
-  __shared__ float4 sbs[256];
-  sbs[threadIdx.x] = bs;
   __syncthreads();
-  if (threadIdx.x < R4) {
-    float4 t4 = sbs[threadIdx.x];
-    for (int j = 1; j < rows_per_blk; j++) {
-      const float4 o = sbs[j * R4 + threadIdx.x];
-      t4.x += o.x; t4.y += o.y; t4.z += o.z; t4.w += o.w;
-    }
-    atomicAdd(dbias + 4 * threadIdx.x, t4.x); atomicAdd(dbias + 4 * threadIdx.x + 1, t4.y);
-    atomicAdd(dbias + 4 * threadIdx.x + 2, t4.z); atomicAdd(dbias + 4 * threadIdx.x + 3, t4.w);
+  float4* dst = reinterpret_cast<float4*>(part) + (size_t)blockIdx.x * n4;
+  for (int i = threadIdx.x; i < n4; i += blockDim.x) dst[i] = tab[i];
+}
+// dwf[i] += sum over chunks c (in order) of part[c][i]; the last tap's sums also go to qpart (for the bias gradient)
+__global__ void front_embed_reduce_kernel(const float* __restrict__ part, float* __restrict__ dwf, float* __restrict__ qpart,
+                                          int nchunks, int n, int last0) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    float s = 0.f;
+    for (int c = 0; c < nchunks; c++) s += part[(size_t)c * n + i];
+    dwf[i] += s;
+    if (i >= last0) qpart[i - last0] = s;
   }
+}
+// out[r] += sum over rows j = 0 .. n-1 (in that order) of part[j * ld + r], r < R
+__global__ void sum_rows_kernel(const float* __restrict__ part, int ld, float* __restrict__ out, int n, int R) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= R) return;
+  float s = 0.f;
+  for (int j = 0; j < n; j++) s += part[(size_t)j * ld + r];
+  out[r] += s;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -344,11 +417,11 @@ __global__ void __launch_bounds__(256) aux_upsample_fwd_v4_kernel(const float* _
 // dw[j] += sum_{b,a,tf} h[b][a][tf] * dhaux[b][tf*U+j][a] ; dbias += sum_{b,t,a<A} dhaux
 // block = one (b, tf); warp-strided over j, lanes over a.
 __global__ void aux_upsample_bwd_kernel(const float* __restrict__ h, const float* __restrict__ dhaux,
-                                        float* __restrict__ dw, float* __restrict__ dbias, int B, int A, int Ap,
-                                        int Tf, int U) {
+                                        float* __restrict__ part, int B, int A, int Ap, int Tf, int U) {
   // Warp w of a block owns the sub-sample offsets j = w, w + nwarps, ... and keeps their partial sums in REGISTERS over
-  // all the (b, tf) items of the block (lanes = aux channels); one atomic per (block, j) at the end.  (One atomic per
-  // dhaux row onto the U addresses of dw -- 184 320 atomics onto 80 words at the bench shape -- took 129 us.)
+  // all the (b, tf) items of the block (lanes = aux channels); the block writes its partials part[block][0 .. U-1] (dw)
+  // and part[block][U] (dbias), which sum_rows_kernel adds up in block order (no atomics: the result does not depend on
+  // scheduling).
   constexpr int kMaxJ = 16;                                   // j values per warp and pass (128 per pass with 8 warps)
   constexpr int kAC = 8;                                      // aux channels per lane: A <= 256
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
@@ -388,7 +461,7 @@ __global__ void aux_upsample_bwd_kernel(const float* __restrict__ h, const float
     for (int i = 0; i < kMaxJ; i++) {
       const int j = jbase + warp + i * nwarps;
       const float v = warp_sum(acc[i]);
-      if (j < U && lane == 0) atomicAdd(dw + j, v);
+      if (j < U && lane == 0) part[(size_t)blockIdx.x * (U + 1) + j] = v;
     }
   }
   btot = warp_sum(btot);
@@ -397,7 +470,7 @@ __global__ void aux_upsample_bwd_kernel(const float* __restrict__ h, const float
   if (threadIdx.x == 0) {
     float s = 0.f;
     for (int i = 0; i < nwarps; i++) s += sb[i];
-    atomicAdd(dbias, s);
+    part[(size_t)blockIdx.x * (U + 1) + U] = s;
   }
 }
 
@@ -407,7 +480,7 @@ __global__ void aux_upsample_bwd_kernel(const float* __restrict__ h, const float
 // dlogits may alias logits (in-place: the fused training entry never keeps the logits): every lane finishes reading
 // a row -- including the target logit -- before any lane overwrites it.
 __global__ void cross_entropy_kernel(const float* logits, const int64_t* __restrict__ target,
-                                     double* __restrict__ loss_sum, float* dlogits, int B, int T, int Q,
+                                     double* __restrict__ loss_part, float* dlogits, int B, int T, int Q,
                                      int start, float inv_n) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   const int64_t nrows = (int64_t)B * T;
@@ -451,14 +524,14 @@ __global__ void cross_entropy_kernel(const float* logits, const int64_t* __restr
   if (threadIdx.x == 0) {
     double s = 0.0;
     for (int i = 0; i < nwarps; i++) s += sl[i];
-    atomicAdd(loss_sum, s * (double)inv_n);
+    loss_part[blockIdx.x] = s * (double)inv_n;   // summed in block order by sum_loss_kernel
   }
 }
 
 // Q == 256 fast path: the row lives in registers (two 16-byte loads per lane), one pass for max / exp / sum, two 16-byte
 // stores for the gradient -- instead of three passes of 4-byte loads over the row.
 __global__ void __launch_bounds__(256) cross_entropy_q256_kernel(const float* logits, const int64_t* __restrict__ target,
-                                                                 double* __restrict__ loss_sum, float* dlogits, int B, int T,
+                                                                 double* __restrict__ loss_part, float* dlogits, int B, int T,
                                                                  int start, float inv_n) {
   constexpr int Q = 256;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
@@ -511,13 +584,20 @@ __global__ void __launch_bounds__(256) cross_entropy_q256_kernel(const float* lo
   if (threadIdx.x == 0) {
     double s = 0.0;
     for (int i = 0; i < nwarps; i++) s += sl[i];
-    atomicAdd(loss_sum, s * (double)inv_n);
+    loss_part[blockIdx.x] = s * (double)inv_n;   // summed in block order by sum_loss_kernel
   }
 }
 
 }  // namespace wnb
 
 using namespace wnb;
+
+// *loss_sum += part[0] + part[1] + ... + part[n-1], in that order
+__global__ void sum_loss_kernel(const double* __restrict__ part, double* __restrict__ loss_sum, int n) {
+  double s = 0.0;
+  for (int i = 0; i < n; i++) s += part[i];
+  *loss_sum += s;
+}
 
 extern "C" {
 
@@ -615,19 +695,39 @@ WNB_API int wnb_front_embed_fwd(const int64_t* x, const float* wf, const float* 
 WNB_API int wnb_front_embed_bwd(const int64_t* x, const float* dout, float* dwf, float* dbias, int B, int T, int Q, int R,
                         int ks, void* stream) {
   WNB_REQUIRE(B > 0 && T > 0 && Q > 0 && R > 0 && ks >= 1, "front_embed_bwd: bad shape");
+  WNB_REQUIRE(ks <= 4, "front_embed_bwd: kernel_size <= 4 (got %d)", ks);
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool v4 = R % 4 == 0 && R / 4 <= 512 && (reinterpret_cast<uintptr_t>(dout) & 15) == 0;
+  WNB_REQUIRE(v4 || R <= 512, "front_embed_bwd: n_resch <= 512 unless it is a multiple of 4 (got %d)", R);
   const int64_t nrows = (int64_t)B * T;
-  if (R % 4 == 0 && 256 % (R / 4) == 0 &&
-      ((reinterpret_cast<uintptr_t>(dwf) | reinterpret_cast<uintptr_t>(dout)) & 15) == 0) {
-    const int rows_per_blk = 256 / (R / 4);
-    front_embed_bwd_v4_kernel<<<grid_for(cdiv64(nrows, rows_per_blk) * 256, 256), 256, 0, (cudaStream_t)stream>>>(
-        x, reinterpret_cast<const float4*>(dout), dwf, dbias, B, T, Q, R / 4, ks);
+  float* qpart = static_cast<float*>(scratch_buffer(st, SCRATCH_EMBED, ((size_t)Q * R + nrows) * sizeof(float)));
+  WNB_REQUIRE(qpart, "front_embed_bwd: cannot allocate the scratch buffer");
+  int* tok = reinterpret_cast<int*>(qpart + (size_t)Q * R);
+  token_kernel<<<grid_for(nrows, 256), 256, 0, st>>>(x, tok, nrows, Q);
+  WNB_CHECK_LAUNCH("front_embed_bwd_tokens");
+  const size_t tab_bytes = (size_t)ks * Q * R * sizeof(float);
+  if (v4 && 256 % (R / 4) == 0 && tab_bytes <= 160 * 1024) {
+    // chunked tables in shared memory: one chunk per SM
+    const int nchunks = device_sms();
+    const int64_t chunk = (nrows + nchunks - 1) / nchunks;
+    float* part = static_cast<float*>(scratch_buffer(st, SCRATCH_EMBED_PART, (size_t)nchunks * tab_bytes));
+    WNB_REQUIRE(part, "front_embed_bwd: cannot allocate the scratch buffer");
+    WNB_CUDA(ensure_dynamic_smem(reinterpret_cast<const void*>(front_embed_bwd_chunk_kernel), tab_bytes));
+    front_embed_bwd_chunk_kernel<<<nchunks, 256, tab_bytes, st>>>(tok, reinterpret_cast<const float4*>(dout), part, B, T, Q,
+                                                                  R / 4, ks, chunk);
+    WNB_CHECK_LAUNCH("front_embed_bwd_chunk");
+    const int n = ks * Q * R;
+    front_embed_reduce_kernel<<<(n + 255) / 256, 256, 0, st>>>(part, dwf, qpart, nchunks, n, (ks - 1) * Q * R);
+    WNB_CHECK_LAUNCH("front_embed_bwd_reduce");
+  } else if (v4) {
+    const int Rv = R / 4;
+    front_embed_bwd_kernel<4><<<Q, (512 / Rv) * Rv, 0, st>>>(tok, dout, dwf, qpart, B, T, Q, Rv, ks);
   } else {
-    const int rows_per_block = 64;
-    const int threads = R >= 256 ? 256 : ((R + 31) / 32) * 32;
-    front_embed_bwd_kernel<<<(int)cdiv64(nrows, rows_per_block), threads, 0, (cudaStream_t)stream>>>(
-        x, dout, dwf, dbias, B, T, Q, R, ks, rows_per_block);
+    front_embed_bwd_kernel<1><<<Q, (512 / R) * R, 0, st>>>(tok, dout, dwf, qpart, B, T, Q, R, ks);
   }
   WNB_CHECK_LAUNCH("front_embed_bwd");
+  sum_rows_kernel<<<(R + 127) / 128, 128, 0, st>>>(qpart, R, dbias, Q, R);
+  WNB_CHECK_LAUNCH("front_embed_bwd_bias");
   return WNB_OK;
 }
 
@@ -651,9 +751,17 @@ WNB_API int wnb_aux_upsample_bwd(const float* h, const float* dhaux, float* dw, 
   WNB_REQUIRE(B > 0 && A > 0 && Ap >= A && Tf > 0 && U > 0, "aux_upsample_bwd: bad shape");
   WNB_REQUIRE(A <= 256, "aux_upsample_bwd: n_aux <= 256 (got %d)", A);
   int64_t items = (int64_t)B * Tf;
-  int grid = (int)(items < 148 * 4 ? items : 148 * 4);
-  aux_upsample_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(h, dhaux, dw, dbias, B, A, Ap, Tf, U);
+  int grid = (int)(items < device_sms() * 4 ? items : device_sms() * 4);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* part = static_cast<float*>(scratch_buffer(st, SCRATCH_AUX, (size_t)grid * (U + 1) * sizeof(float)));
+  WNB_REQUIRE(part, "aux_upsample_bwd: cannot allocate the scratch buffer");
+  aux_upsample_bwd_kernel<<<grid, 256, 0, st>>>(h, dhaux, part, B, A, Ap, Tf, U);
   WNB_CHECK_LAUNCH("aux_upsample_bwd");
+  // dw: columns 0 .. U-1 of the partials, dbias: column U
+  sum_rows_kernel<<<(U + 127) / 128, 128, 0, st>>>(part, U + 1, dw, grid, U);
+  WNB_CHECK_LAUNCH("aux_upsample_bwd_w");
+  sum_rows_kernel<<<1, 32, 0, st>>>(part + U, U + 1, dbias, grid, 1);
+  WNB_CHECK_LAUNCH("aux_upsample_bwd_b");
   return WNB_OK;
 }
 
@@ -663,14 +771,17 @@ WNB_API int wnb_cross_entropy(const float* logits, const int64_t* target, double
               T);
   const int64_t n = (int64_t)B * (T - start);
   const int64_t nrows = (int64_t)B * T;
-  int grid = (int)(cdiv64(nrows, 8) < 148 * 8 ? cdiv64(nrows, 8) : 148 * 8);
+  int grid = (int)(cdiv64(nrows, 8) < device_sms() * 8 ? cdiv64(nrows, 8) : device_sms() * 8);
+  cudaStream_t st = (cudaStream_t)stream;
+  double* part = static_cast<double*>(scratch_buffer(st, SCRATCH_LOSS, (size_t)grid * sizeof(double)));
+  WNB_REQUIRE(part, "cross_entropy: cannot allocate the scratch buffer");
   if (Q == 256 && ((reinterpret_cast<uintptr_t>(logits) | reinterpret_cast<uintptr_t>(dlogits)) & 15) == 0)
-    cross_entropy_q256_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(logits, target, loss_sum, dlogits, B, T, start,
-                                                                     1.0f / (float)n);
+    cross_entropy_q256_kernel<<<grid, 256, 0, st>>>(logits, target, part, dlogits, B, T, start, 1.0f / (float)n);
   else
-    cross_entropy_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(logits, target, loss_sum, dlogits, B, T, Q, start,
-                                                                1.0f / (float)n);
+    cross_entropy_kernel<<<grid, 256, 0, st>>>(logits, target, part, dlogits, B, T, Q, start, 1.0f / (float)n);
   WNB_CHECK_LAUNCH("cross_entropy");
+  sum_loss_kernel<<<1, 1, 0, st>>>(part, loss_sum, grid);
+  WNB_CHECK_LAUNCH("cross_entropy_sum");
   return WNB_OK;
 }
 

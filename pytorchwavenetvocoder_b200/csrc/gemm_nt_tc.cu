@@ -1,17 +1,15 @@
 // gemm_nt_tc.cu -- tensor-core GEMM over channels-last activations:
-//     D[t][n] = epi( sum_seg sum_k A_seg[t + shift_seg][k] * W_seg[n][k] )          n < N <= 512
+//     D[t][n] = epi( sum_seg sum_k A_seg[t + shift_seg][k] * W_seg[n][k] )          n < N <= 256 per tile
 // A rows are time steps (K-major operand straight from the (B,T,C) tensor, TMA zero fill outside [0,T) =
-// causal / anti-causal padding), W is a row-major [N][K] weight matrix (K-major operand).  tcgen05.mma
-// kind::tf32, fp32 accumulate in TMEM (whole 128 x N tile; double buffered when N <= 256).
-// Epilogue (8 warps = TMEM lane quarter x alternate 32-column chunks, two per SM sub-partition): + bias, ReLU,
-// * (mask > 0), + residual (operands that do not depend on the accumulator are requested before waiting for it), then
-// a swizzled per-warp staging box and a TMA store or TMA reduce-add (.add.f32) into the (B,T,N) output; gate forward /
-// backward epilogues for the residual blocks.  The kernel is instantiated per epilogue kind (EPI_*) so each variant
-// gets its own register allocation.  Options: column blocks (tiles ordered block-fastest so the A tile is shared
-// through L2), split output, programmatic dependent launch; round 2: two 128-row time tiles per weight chunk
-// (NtTcOpts::m_tiles: the K >= 512 GEMMs were bound by the L2 -> SM weight stream, not by HBM or the tensor pipe), gate
-// epilogues over 64 or 128 gate channels per tile (composed path), epilogue operands staged by the producer as TMA tiles
-// (NtTcOpts::stage_epilogue_operand: measured slower, off by default).
+// causal / anti-causal padding), W is a row-major [N][K] weight matrix (K-major operand).  Hopper wgmma
+// m64nNk8 tf32, fp32 accumulate in registers of one consumer warpgroup; one producer warp streams
+// [64 x 32] activation boxes and [N x 32] weight boxes through an mbarrier ring with TMA.
+// Epilogue: the accumulator is written to shared memory column-major, then each consumer thread owns one time row
+// and 32-column chunks (warp w: rows 32 (w & 1) .., chunks w >> 1, (w >> 1) + 2, ...): + bias, ReLU, * (mask > 0),
+// + residual, then a swizzled per-warp staging box and a TMA store or TMA reduce-add (.add.f32) into the (B,T,N)
+// output; gate forward / backward epilogues for the residual blocks.  The kernel is instantiated per (N, epilogue
+// kind) so each variant gets its own register allocation.  Column blocks (tiles ordered block-fastest so the A tile
+// is shared through L2), split output and programmatic dependent launch as options.
 // Used for: the post network forward (wavenet.py:518-523) and backward, the hoisted skip GEMMs, the gate backward,
 // the residual-stream data gradient dX (two time-shifted segments) with the aux gradient dhaux (reduce-add).
 #include <cuda.h>
@@ -26,19 +24,22 @@
 namespace wnb {
 namespace nt {
 
-constexpr int kTM = 128;
-constexpr int kASub = kTM * 32 * 4;      // 16 KB
+constexpr int kTM = 64;                  // time rows per tile (wgmma M)
+constexpr int kASub = kTM * 32 * 4;      // 8 KB
 constexpr int kStg = 32 * 32 * 4;        // 4 KB
-constexpr int kEpiWarpsN = 8;            // two per SM sub-partition: (TMEM lane quarter) x (alternate 32-column chunks)
-constexpr int kThreadsN = 32 * (2 + kEpiWarpsN);
+constexpr int kConsumers = 128;          // one warpgroup: MMA + epilogue
+constexpr int kThreadsN = kConsumers + 32;
+constexpr int kAccLd = kTM + 4;          // column pitch (floats) of the shared-memory accumulator: conflict-free both ways
+// bytes of the accumulator copy, rounded up so that the staging boxes behind it keep the 1024-byte alignment the
+// 128B-swizzled TMA stores need
+__host__ __device__ constexpr int acc_bytes(int N) { return (N * kAccLd * 4 + 1023) & ~1023; }
 constexpr int kMaxSeg = 4;
 
-struct Seg { int amap; int shift; int K; int bmap; int b_k0; int b_n0; int b_n1;   // b_n1 >= 0: rows of the 2nd half of N
-             int n_lo, n_cnt, fresh; };   // resident weights: accumulator columns [n_lo, n_lo + n_cnt), first MMA overwrites
+struct Seg { int amap; int shift; int K; int bmap; int b_k0; int b_n0; int b_n1; };   // b_n1 >= 0: rows of the 2nd half of N
 struct alignas(64) Params {
-  CUtensorMap maps[11];   // [0..3] A tensors, [4..7] weight matrices, [8] output, [9] second output, [10] epilogue tile
+  CUtensorMap maps[10];   // [0..3] A tensors, [4..7] weight matrices, [8] output, [9] second output
   Seg seg[kMaxSeg];
-  int nseg, N, T, B, nstages, nacc;
+  int nseg, N, T, B, nstages;
   const float* bias; const float* mask; int ldmask; const float* add; int ldadd;
   int relu_out, accumulate;
   // gate epilogues (N == 128 = [64 sigmoid pre | 64 tanh pre] of gate channels gate_c0 .. gate_c0+63 of gate_R):
@@ -55,72 +56,32 @@ struct alignas(64) Params {
   int out2_col0;
   // column blocks (NtTcOpts::n_blocks), dz row pitch and z suppression of the gate-backward epilogue
   int nblk, gate_ld_dz, gate_skip_z;
-  // mt == 2 (NtTcOpts::m_tiles): a CTA tile is TWO 128-row time tiles against ONE weight chunk per k-step -- the
-  // weight chunk is fetched from L2 once per 256 rows instead of once per 128 (the K >= 512 GEMMs are bound by the
-  // L2 -> SM path, not by HBM or the tensor pipe).  The two accumulators are the two TMEM buffers (N <= 256).
-  int mt, stg_boxes;
-  // etile != 0 (NtTcOpts::stage_epilogue_operand): the epilogue's per-row operand -- 1: the dz slice of the gate backward,
-  // 2: the residual `add` of a <= 64-column primary output -- is brought in by the PRODUCER as one [128 x 64] TMA tile per
-  // time tile (maps[10], two swizzled sub-tiles) instead of per-lane row loads from global memory: the epilogue warps
-  // pace these kernels and were stalled on exactly those loads (ncu: 51 % long-scoreboard on L1TEX).
-  int etile;
-  // wres != 0 (NtTcOpts::resident_weights): every weight chunk of every segment is loaded ONCE per CTA into shared memory
-  // (wres_bytes, in front of the ring) and the ring carries activations only -- the residual-block kernels (gate backward,
-  // dX) were paced by the per-SM L2 -> SM ingest, 61 % / 43 % of which was the same 172 / 96 KB of weights again for every
-  // 128-row tile.  Segments name the accumulator columns they touch (zero blocks of a block matrix are skipped).
-  int wres, wres_bytes;
-  // pf > 0: the producer L2-prefetches the activation boxes of the tile `pf` rounds ahead (no shared memory needed): with
-  // 64-80 KB of ring per SM the block kernels were bound by DRAM latency x bytes in flight.  epf: also the epilogue's
-  // per-row operand tile (1: dz slice, 2: residual add) through maps[10].
-  int pf, epf;
   int rev;   // NtTcOpts::reverse
-  int grp;   // resident-weights mode: activation chunks issued per group (see the producer)
 };
 
-// barrier layout in smem: full[nstages] empty[nstages] dfull[2] dempty[2]
-
-// Tuning aid (WNB_PROF=1): cycles each role spends blocked, summed over CTAs.
-enum { NP_P_EMPTY = 0, NP_M_DEMPTY, NP_M_FULL, NP_M_TOTAL, NP_E_DFULL, NP_E_BULK, NP_E_TOTAL, NP_MIN, NP_MAX, NP_COUNT };
-__device__ unsigned long long g_nt_prof[NP_COUNT];
-
-// EPI selects the epilogue at compile time so that each variant gets its own register allocation (the kernel runs
-// 320 threads = 168 registers per thread): 0 plain (bias / add / ReLU / mask / split output), 1 gate forward and
-// gate backward with z output, 2 gate backward without z (the stack path, two 16-channel passes).
+// EPI selects the epilogue at compile time so that each variant gets its own register allocation: 0 plain (bias / add /
+// ReLU / mask / split output), 1 gate forward and gate backward with z output, 2 gate backward without z (the stack path).
 enum { EPI_PLAIN = 0, EPI_GATE = 1, EPI_GATE_BWD_NOZ = 2 };
 
-template <bool PROF, int EPI>
+// 16 consecutive accumulator columns of one row out of the column-major shared-memory copy
+__device__ __forceinline__ void acc_ld16(const float* acc, int col, int row, float (&v)[16]) {
+#pragma unroll
+  for (int i = 0; i < 16; i++) v[i] = acc[(col + i) * kAccLd + row];
+}
+
+template <int N, int EPI>
 __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_constant__ Params p) {
-  long long acc[NP_COUNT] = {};
-  auto wait = [&](uint64_t* bar, uint32_t parity, int k) {
-    if constexpr (PROF) {
-      const long long t = clock64();
-      ptx::mbar_wait(bar, parity);
-      acc[k] += clock64() - t;
-    } else {
-      ptx::mbar_wait(bar, parity);
-    }
-  };
-  const long long t_begin = PROF ? clock64() : 0;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int N = p.N;
-  const int a_bytes = p.mt * kASub;
-  const int stage_bytes = a_bytes + (p.wres ? 0 : N * 128);
-  unsigned char* ring = smem + p.wres_bytes;
-  unsigned char* stg_base = ring + (size_t)p.nstages * stage_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(stg_base + kEpiWarpsN * p.stg_boxes * kStg + (p.etile ? 2 * kASub : 0));
+  constexpr int stage_bytes = kASub + N * 128;
+  unsigned char* ring = smem;
+  float* accs = reinterpret_cast<float*>(ring + (size_t)p.nstages * stage_bytes);
+  unsigned char* stg_base = reinterpret_cast<unsigned char*>(accs) + acc_bytes(N);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stg_base + 4 * 2 * kStg);
   uint64_t* full = bars;
   uint64_t* empty = bars + p.nstages;
-  uint64_t* dfull = bars + 2 * p.nstages;
-  uint64_t* dempty = dfull + 2;
-  uint64_t* efull = dempty + 2;       // epilogue-operand tile landed / consumed (etile)
-  uint64_t* eempty = efull + 1;
-  uint64_t* wfull = eempty + 1;       // resident weights landed (wres)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wfull + 1);
-  unsigned char* ebuf = stg_base + kEpiWarpsN * p.stg_boxes * kStg;   // 2 x [128 x 32] sub-tiles when etile
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int rows_per_tile = kTM * p.mt;
-  const int tiles_per_b = (p.T + rows_per_tile - 1) / rows_per_tile;
+  const int tiles_per_b = (p.T + kTM - 1) / kTM;
   const int ntiles = p.B * tiles_per_b * p.nblk;   // column block fastest: the blocks of one time tile share A via L2
   int kchunks = 0;
   for (int s = 0; s < p.nseg; s++) kchunks += p.seg[s].K / 32;
@@ -128,463 +89,235 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
   if (threadIdx.x == 0) {
     for (int i = 0; i < p.nstages; i++) {
       ptx::mbar_init(&full[i], 1);
-      ptx::mbar_init(&empty[i], 1);
+      ptx::mbar_init(&empty[i], kConsumers);
     }
-    for (int i = 0; i < 2; i++) {
-      ptx::mbar_init(&dfull[i], 1);
-      ptx::mbar_init(&dempty[i], 32 * kEpiWarpsN);
-    }
-    ptx::mbar_init(efull, 1);
-    ptx::mbar_init(eempty, 32 * kEpiWarpsN);
-    ptx::mbar_init(wfull, 1);
     ptx::fence_barrier_init();
   }
-  if (warp == 1) ptx::tmem_alloc<512>(tmem_slot);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  ptx::tmem_base_must_be_zero(*tmem_slot);
-  constexpr uint32_t tmem = 0;
   // programmatic dependent launch: the set-up above overlapped the previous kernel's tail; from here on this
   // kernel reads / writes memory that kernel may have produced
   ptx::pdl_launch_dependents();
   ptx::pdl_wait();
 
-  // single-thread roles are entered through elect.sync (not `lane == 0`): the compiler then knows exactly one
-  // thread is active and issues the uniform-datapath TMA / tcgen05 instructions without a per-thread ELECT loop
-  if (warp == 0) {
+  if (warp == 4) {
+    // =============================== TMA producer ===============================
     if (ptx::elect_one()) {
-      for (int i = 0; i < 11; i++) ptx::prefetch_tmap(&p.maps[i]);
-      uint32_t st = 0, ph = 0, pit = 0;
-      if (p.wres) {   // all weight chunks, once
-        ptx::mbar_arrive_expect_tx(wfull, p.wres_bytes);
-        unsigned char* dst = smem;
-        for (int s = 0; s < p.nseg; s++) {
-          const Seg sg = p.seg[s];
-          for (int kc = 0; kc < sg.K / 32; kc++, dst += sg.n_cnt * 128)
-            ptx::tma_load_2d(dst, &p.maps[sg.bmap], wfull, sg.b_k0 + kc * 32, sg.b_n0 + sg.n_lo);
-        }
-      }
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, pit++) {
+      for (int i = 0; i < 10; i++) ptx::prefetch_tmap(&p.maps[i]);
+      uint32_t st = 0, ph = 0;
+      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const int te = p.rev ? ntiles - 1 - tile : tile;
         const int tt = te / p.nblk, ncol0 = (te - tt * p.nblk) * N;
-        const int b = tt / tiles_per_b, t0 = (tt - b * tiles_per_b) * rows_per_tile;
-        if (p.pf) {
-          const int ptile = tile + p.pf * (int)gridDim.x;
-          if (ptile < ntiles) {
-            const int ptt = (p.rev ? ntiles - 1 - ptile : ptile) / p.nblk, pb = ptt / tiles_per_b, pt0 = (ptt - pb * tiles_per_b) * rows_per_tile;
-            for (int s = 0; s < p.nseg; s++)
-              for (int kc = 0; kc < p.seg[s].K / 32; kc++)
-                for (int mh = 0; mh < p.mt; mh++)
-                  ptx::tma_prefetch_3d(&p.maps[p.seg[s].amap], kc * 32, pt0 + mh * kTM + p.seg[s].shift, pb);
-            if (p.epf) {
-              ptx::tma_prefetch_3d(&p.maps[10], 0, pt0, pb);
-              ptx::tma_prefetch_3d(&p.maps[10], 32, pt0, pb);
-            }
-          }
-        }
-        if (p.etile) {   // the epilogue's operand tile of this time tile goes first: it is needed as soon as the accumulator is
-          wait(eempty, (pit & 1) ^ 1, NP_P_EMPTY);
-          ptx::mbar_arrive_expect_tx(efull, 2 * kASub);
-          ptx::tma_load_3d(ebuf, &p.maps[10], efull, 0, t0, b);
-          ptx::tma_load_3d(ebuf + kASub, &p.maps[10], efull, 32, t0, b);
-        }
+        const int b = tt / tiles_per_b, t0 = (tt - b * tiles_per_b) * kTM;
         for (int s = 0; s < p.nseg; s++) {
           const Seg sg = p.seg[s];
           for (int kc = 0; kc < sg.K / 32; kc++) {
-            wait(&empty[st], ph ^ 1, NP_P_EMPTY);
+            ptx::mbar_wait(&empty[st], ph ^ 1);
             ptx::mbar_arrive_expect_tx(&full[st], stage_bytes);
             unsigned char* dst = ring + (size_t)st * stage_bytes;
-            if (p.wres) {
-              // activation boxes are issued in groups of p.grp consecutive 32-channel chunks (= p.grp x 128 contiguous bytes
-              // of every row) once that many stages are free: DRAM sees whole rows at once instead of one 128-B piece of
-              // every other 256 B now and the next piece a microsecond later
-              int g = sg.K / 32 - kc < p.grp ? sg.K / 32 - kc : p.grp;
-              if (g > p.nstages) g = p.nstages;
-              uint32_t st2 = st, ph2 = ph;
-              for (int i = 1; i < g; i++) {
-                if (++st2 == (uint32_t)p.nstages) { st2 = 0; ph2 ^= 1; }
-                wait(&empty[st2], ph2 ^ 1, NP_P_EMPTY);
-              }
-              for (int i = 0; i < g; i++) {
-                if (i) ptx::mbar_arrive_expect_tx(&full[st], stage_bytes);
-                ptx::tma_load_3d(ring + (size_t)st * stage_bytes, &p.maps[sg.amap], &full[st], (kc + i) * 32, t0 + sg.shift, b);
-                if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
-              }
-              kc += g - 1;
-              continue;
-            }
             ptx::tma_load_3d(dst, &p.maps[sg.amap], &full[st], kc * 32, t0 + sg.shift, b);
-            if (p.mt == 2)   // (rows past T are zero-filled by TMA, the matching stores are clipped)
-              ptx::tma_load_3d(dst + kASub, &p.maps[sg.amap], &full[st], kc * 32, t0 + kTM + sg.shift, b);
             if (sg.b_n1 >= 0) {   // N = two row ranges of N/2 each (sigmoid rows, tanh rows)
-              ptx::tma_load_2d(dst + a_bytes, &p.maps[sg.bmap], &full[st], sg.b_k0 + kc * 32, sg.b_n0);
-              ptx::tma_load_2d(dst + a_bytes + (N / 2) * 128, &p.maps[sg.bmap], &full[st], sg.b_k0 + kc * 32, sg.b_n1);
+              ptx::tma_load_2d(dst + kASub, &p.maps[sg.bmap], &full[st], sg.b_k0 + kc * 32, sg.b_n0);
+              ptx::tma_load_2d(dst + kASub + (N / 2) * 128, &p.maps[sg.bmap], &full[st], sg.b_k0 + kc * 32, sg.b_n1);
             } else {
-              for (int n0 = 0; n0 < N; n0 += 256)
-                ptx::tma_load_2d(dst + a_bytes + n0 * 128, &p.maps[sg.bmap], &full[st], sg.b_k0 + kc * 32, sg.b_n0 + ncol0 + n0);
+              ptx::tma_load_2d(dst + kASub, &p.maps[sg.bmap], &full[st], sg.b_k0 + kc * 32, sg.b_n0 + ncol0);
             }
             if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
           }
         }
       }
     }
-  } else if (warp == 1) {
-    if (ptx::elect_one()) {
-      const int nmma = N > 256 ? 256 : N;
-      const uint32_t idesc = ptx::idesc_tf32(128, nmma);
-      const uint32_t s_lo0 = ptx::desc_lo(ptx::smem_u32(ring), 16);
-      const uint32_t w_lo0 = ptx::desc_lo(ptx::smem_u32(smem), 16);
-      constexpr uint32_t hi = ptx::kDescHiKSw128;
-      if (p.wres) wait(wfull, 0, NP_M_FULL);
-      const uint32_t stage_step = (uint32_t)stage_bytes >> 4;
-      uint32_t st = 0, ph = 0, it = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, it++) {
-        if (p.mt == 2) {
-          // two time tiles per weight chunk: accumulator h (TMEM columns h*N..) belongs to rows t0 + 128 h
-          wait(&dempty[0], (it & 1) ^ 1, NP_M_DEMPTY);
-          wait(&dempty[1], (it & 1) ^ 1, NP_M_DEMPTY);
-          ptx::tc_fence_after();
-          for (int kc = 0; kc < kchunks; kc++) {
-            wait(&full[st], ph, NP_M_FULL);
-            ptx::tc_fence_after();
-            const uint32_t a_lo = s_lo0 + st * stage_step, b_lo = a_lo + (2 * kASub >> 4);
+    return;
+  }
+
+  // =============================== consumer warpgroup: wgmma mainloop + epilogue ===============================
+  const int q = warp & 1;                 // rows 32 q .. 32 q + 31 of the tile in the epilogue
+  const int hf = warp >> 1;               // 0 / 1: this warp takes 32-column chunks hf, hf + 2, ...
+  const int row = q * 32 + lane;
+  unsigned char* stg = stg_base + warp * 2 * kStg;
+  const uint32_t ring_u32 = ptx::smem_u32(ring);
+  uint32_t st = 0, ph = 0, nstore = 0;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int te = p.rev ? ntiles - 1 - tile : tile;
+    const int tt = te / p.nblk, ncol0 = (te - tt * p.nblk) * N;
+    const int b = tt / tiles_per_b, t0 = (tt - b * tiles_per_b) * kTM;
+    float d[N / 2];
 #pragma unroll
-            for (int k = 0; k < 4; k++) {
-              ptx::mma_tf32_ss(tmem, ptx::desc64(a_lo + 2 * k, hi), ptx::desc64(b_lo + 2 * k, hi), idesc, (kc | k) != 0);
-              ptx::mma_tf32_ss(tmem + N, ptx::desc64(a_lo + (kASub >> 4) + 2 * k, hi), ptx::desc64(b_lo + 2 * k, hi), idesc,
-                               (kc | k) != 0);
-            }
-            ptx::tc_commit(&empty[st]);
-            if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
-          }
-          ptx::tc_commit(&dfull[0]);
-          ptx::tc_commit(&dfull[1]);
-          continue;
-        }
-        const uint32_t buf = (p.nacc == 2) ? (it & 1) : 0;
-        const uint32_t use = (p.nacc == 2) ? (it >> 1) : it;
-        wait(&dempty[buf], (use & 1) ^ 1, NP_M_DEMPTY);
-        ptx::tc_fence_after();
-        const uint32_t dcol = buf * N;
-        if (p.wres) {
-          uint32_t b_lo = w_lo0;
-          for (int s = 0; s < p.nseg; s++) {
-            const Seg sg = p.seg[s];
-            const uint32_t idesc_s = ptx::idesc_tf32(128, sg.n_cnt);
-            for (int kc = 0; kc < sg.K / 32; kc++, b_lo += (uint32_t)(sg.n_cnt * 128) >> 4) {
-              wait(&full[st], ph, NP_M_FULL);
-              ptx::tc_fence_after();
-              const uint32_t a_lo = s_lo0 + st * stage_step;
+    for (int i = 0; i < N / 2; i++) d[i] = 0.f;
+    uint32_t prev = 0xFFFFFFFFu;
+    for (int kc = 0; kc < kchunks; kc++) {
+      ptx::mbar_wait(&full[st], ph);
+      ptx::wg_fence();
+      const uint32_t a_addr = ring_u32 + st * stage_bytes, b_addr = a_addr + kASub;
 #pragma unroll
-              for (int k = 0; k < 4; k++)
-                ptx::mma_tf32_ss(tmem + dcol + sg.n_lo, ptx::desc64(a_lo + 2 * k, hi), ptx::desc64(b_lo + 2 * k, hi), idesc_s,
-                                 !(sg.fresh && (kc | k) == 0));
-              ptx::tc_commit(&empty[st]);
-              if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
-            }
-          }
-          ptx::tc_commit(&dfull[buf]);
-          continue;
-        }
-        for (int kc = 0; kc < kchunks; kc++) {
-          wait(&full[st], ph, NP_M_FULL);
-          ptx::tc_fence_after();
-          const uint32_t a_lo = s_lo0 + st * stage_step, b_lo = a_lo + (kASub >> 4);
+      for (int k = 0; k < 4; k++)
+        ptx::wgmma_ss<N>(d, ptx::gmma_desc_k_sw128(a_addr + 32 * k), ptx::gmma_desc_k_sw128(b_addr + 32 * k), 1);
+      ptx::wg_commit();
+      ptx::wg_wait<1>();                   // the previous chunk's MMAs are done: its stage can be refilled
+      if (prev != 0xFFFFFFFFu) ptx::mbar_arrive(&empty[prev]);
+      prev = st;
+      if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
+    }
+    ptx::wg_wait<0>();
+    ptx::wg_touch(d);
+    if (prev != 0xFFFFFFFFu) ptx::mbar_arrive(&empty[prev]);
+    // accumulator -> shared memory (column-major), after every thread is done reading the previous tile's copy
+    ptx::named_bar(1, kConsumers);
+    {
+      const int r0 = 16 * warp + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+      for (int i = 0; i < N / 2; i++) accs[(8 * (i >> 2) + c0 + (i & 1)) * kAccLd + r0 + 8 * ((i >> 1) & 1)] = d[i];
+    }
+    ptx::named_bar(1, kConsumers);
+
+    const int t = t0 + row;
+    const bool row_ok = t < p.T;
+    const size_t grow = (size_t)b * p.T + (row_ok ? t : 0);
+    if constexpr (EPI == EPI_GATE_BWD_NOZ) {
+      // ---- gate backward without the z output (the stack path): two passes of 16 gate channels; the two dpre boxes
+      //      of this warp (d pre-sigmoid, d pre-tanh) are filled side by side and stored with one bulk group ----
+      const int c0 = hf * 32;
+      if (lane == 0) ptx::bulk_wait_read<0>();
+      __syncwarp();
+      const uint32_t sb0 = ptx::smem_u32(stg + lane * 128), sb1 = sb0 + kStg;
+      const float4* bsv = reinterpret_cast<const float4*>(p.bias + c0);
+      const float4* btv = reinterpret_cast<const float4*>(p.bias2 + c0);
+      const float4* dzr = reinterpret_cast<const float4*>(p.gate_dz + grow * p.gate_ld_dz + p.gate_c0 + c0);
+#pragma unroll
+      for (int h2 = 0; h2 < 2; h2++) {
+        const int cc = c0 + h2 * 16;
+        float a[16], g[16], dzp[16];
+        acc_ld16(accs, cc, row, a);
+        acc_ld16(accs, 64 + cc, row, g);
+        if (p.gate_mode == 3) acc_ld16(accs, 128 + cc, row, dzp);
+#pragma unroll
+        for (int jj = 0; jj < 4; jj++) {
+          const float4 d4 = row_ok ? __ldg(dzr + h2 * 4 + jj) : make_float4(0.f, 0.f, 0.f, 0.f);
+          const float4 bs = __ldg(bsv + h2 * 4 + jj), bt = __ldg(btv + h2 * 4 + jj);
+          const float dzs[4] = {d4.x, d4.y, d4.z, d4.w};
+          const float bsa[4] = {bs.x, bs.y, bs.z, bs.w}, bta[4] = {bt.x, bt.y, bt.z, bt.w};
+          float da[4], dg[4];
 #pragma unroll
           for (int k = 0; k < 4; k++) {
-            ptx::mma_tf32_ss(tmem + dcol, ptx::desc64(a_lo + 2 * k, hi), ptx::desc64(b_lo + 2 * k, hi), idesc,
-                             (kc | k) != 0);
-            if (N > 256)
-              ptx::mma_tf32_ss(tmem + dcol + 256, ptx::desc64(a_lo + 2 * k, hi),
-                               ptx::desc64(b_lo + (256 * 128 >> 4) + 2 * k, hi), idesc, (kc | k) != 0);
+            const int i = 4 * jj + k;
+            float dz = dzs[k];
+            if (p.gate_mode == 3) dz += dzp[i];
+            const float sg = 0.5f * ptx::tanh_approx(0.5f * (a[i] + bsa[k])) + 0.5f;
+            const float th = ptx::tanh_approx(g[i] + bta[k]);
+            da[k] = dz * th * sg * (1.f - sg);      // d pre-sigmoid
+            dg[k] = dz * sg * (1.f - th * th);      // d pre-tanh
           }
-          ptx::tc_commit(&empty[st]);
-          if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
+          const uint32_t off = (uint32_t)(((h2 * 4 + jj) ^ (lane & 7)) << 4);
+          ptx::st_shared_v4(sb0 + off, da[0], da[1], da[2], da[3]);
+          ptx::st_shared_v4(sb1 + off, dg[0], dg[1], dg[2], dg[3]);
         }
-        ptx::tc_commit(&dfull[buf]);
       }
-      if constexpr (PROF) acc[NP_M_TOTAL] = clock64() - t_begin;
+      ptx::fence_proxy_async();
+      __syncwarp();
+      if (lane == 0) {
+        ptx::tma_store_3d(&p.maps[9], stg, p.gate_c0 + c0, t0 + q * 32, b);
+        ptx::tma_store_3d(&p.maps[9], stg + kStg, p.gate_R + p.gate_c0 + c0, t0 + q * 32, b);
+        ptx::bulk_commit();
+      }
+      continue;
     }
-  } else {
-    const int q = warp & 3;                 // TMEM lane quarter (hardware restriction: warp id % 4)
-    const int hf = (warp - 2) >> 2;         // 0 / 1: this warp takes 32-column chunks hf, hf + 2, ...
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    unsigned char* stg = stg_base + (warp - 2) * p.stg_boxes * kStg;
-    const uint32_t box_mask = (uint32_t)p.stg_boxes - 1;   // 2 staging boxes per warp (alternating), 1 when mt == 2
-    uint32_t it = 0, nstore = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, it++) {
-     for (int mh = 0; mh < p.mt; mh++) {     // mt == 2: the two 128-row halves of the tile, accumulator mh each
-      const int te = p.rev ? ntiles - 1 - tile : tile;
-      const int tt = te / p.nblk, ncol0 = (te - tt * p.nblk) * N;
-      const int b = tt / tiles_per_b, t0 = (tt - b * tiles_per_b) * rows_per_tile + mh * kTM;
-      const int t = t0 + q * 32 + lane;
-      const bool row_ok = t < p.T;
-      const size_t grow = (size_t)b * p.T + (row_ok ? t : 0);
-      const uint32_t buf = (p.mt == 2) ? (uint32_t)mh : ((p.nacc == 2) ? (it & 1) : 0);
-      const uint32_t use = (p.mt == 2) ? it : ((p.nacc == 2) ? (it >> 1) : it);
-      // operands of the epilogue that do not depend on the accumulator are requested before waiting for it, so
-      // their DRAM latency overlaps the mainloop of this tile: dz of the gate backward, `add` of the first chunk
-      // They are loaded COALESCED -- load i of the warp covers rows 4i .. 4i+3 of its 32-row slab, 8 lanes x 16 B per row (4
-      // full 128-B lines per request; one row per lane was 32 lines per request and cost the gate backward 13 of its 60 us)
-      // -- and transposed to one row per lane through the warp's own staging box once that is free (xpose_pre below).
-      float4 pre[8];
-      const bool pre_dz = EPI != EPI_PLAIN && p.gate_mode >= 2 && hf * 32 < 64 && !p.etile;
-      const bool pre_add = EPI == EPI_PLAIN && p.add && hf * 32 < N && !(p.out2_col0 > 0 && hf * 32 >= p.out2_col0) && !p.etile;
-      if (pre_dz || pre_add) {
-        const float* src = pre_dz ? p.gate_dz + p.gate_c0 + hf * 32 : p.add + ncol0 + hf * 32;
-        const size_t ld = pre_dz ? (size_t)p.gate_ld_dz : (size_t)p.ldadd;
-        const int tr = t0 + q * 32 + (lane >> 3);
-#pragma unroll
-        for (int i = 0; i < 8; i++)
-          pre[i] = (tr + 4 * i < p.T) ? __ldg(reinterpret_cast<const float4*>(src + ((size_t)b * p.T + tr + 4 * i) * ld) + (lane & 7))
-                                      : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      // pre[] (rows 4i + lane/8, 16-B piece lane%8) -> this lane's own row, pieces 0..7, through `box` (free: the caller has
-      // waited for the bulk store that last read it); rows past T arrive as zeros
-      auto xpose_pre = [&](unsigned char* box) {
-        const uint32_t wb = ptx::smem_u32(box);
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-          const int r = 4 * i + (lane >> 3);
-          ptx::st_shared_v4(wb + r * 128 + (((lane & 7) ^ (r & 7)) << 4), pre[i].x, pre[i].y, pre[i].z, pre[i].w);
+    if constexpr (EPI == EPI_GATE) {
+      // ---- gate epilogues: pair sigmoid column c with tanh column GC + c (GC = 64 or 128 gate channels per tile) ----
+      const int GC = p.gate_gc;
+      for (int c0 = hf * 32; c0 < GC; c0 += 64) {
+        float a[32], g[32], dzv[32], dzp[32];
+        acc_ld16(accs, c0, row, *reinterpret_cast<float(*)[16]>(a));
+        acc_ld16(accs, c0 + 16, row, *reinterpret_cast<float(*)[16]>(a + 16));
+        acc_ld16(accs, GC + c0, row, *reinterpret_cast<float(*)[16]>(g));
+        acc_ld16(accs, GC + c0 + 16, row, *reinterpret_cast<float(*)[16]>(g + 16));
+        if (p.gate_mode == 3) {
+          acc_ld16(accs, 2 * GC + c0, row, *reinterpret_cast<float(*)[16]>(dzp));
+          acc_ld16(accs, 2 * GC + c0 + 16, row, *reinterpret_cast<float(*)[16]>(dzp + 16));
         }
-        __syncwarp();
-#pragma unroll
-        for (int j = 0; j < 8; j++) pre[j] = ptx::ld_shared_v4(wb + lane * 128 + ((j ^ (lane & 7)) << 4));
-      };
-      wait(&dfull[buf], use & 1, NP_E_DFULL);
-      ptx::tc_fence_after();
-      if (p.etile == 1) {   // this row's 32 dz channels out of the staged tile (rows past T were zero-filled by TMA)
-        wait(efull, it & 1, NP_E_DFULL);
-        const float4* er = reinterpret_cast<const float4*>(ebuf + hf * kASub + (q * 32 + lane) * 128);
-#pragma unroll
-        for (int j = 0; j < 8; j++) pre[j] = er[j ^ (lane & 7)];
-        ptx::mbar_arrive(eempty);
-      }
-      if constexpr (EPI != EPI_GATE_BWD_NOZ) {
-        if (pre_dz || pre_add) {   // (the box the first chunk will be staged in; same wait as before that store)
-          if (lane == 0) {
-            if (box_mask) ptx::bulk_wait_read<1>(); else ptx::bulk_wait_read<0>();
-          }
-          __syncwarp();
-          xpose_pre(stg + (nstore & box_mask) * kStg);
-        }
-      }
-      if constexpr (EPI == EPI_GATE_BWD_NOZ) {
-        // ---- gate backward without the z output (the stack path): two passes of 16 gate channels keep the live
-        //      registers under the 168 this kernel gets (the 32-channel form below spilled); the two dpre boxes of
-        //      this warp (d pre-sigmoid, d pre-tanh) are filled side by side and stored with one bulk group ----
-        const int c0 = hf * 32;
-        {
-          const long long tb = PROF ? clock64() : 0;
-          if (lane == 0) ptx::bulk_wait_read<0>();
-          __syncwarp();
-          if constexpr (PROF) acc[NP_E_BULK] += clock64() - tb;
-        }
-        if (pre_dz) xpose_pre(stg);
-        const uint32_t sb0 = ptx::smem_u32(stg + lane * 128), sb1 = sb0 + kStg;
-        const float4* bsv = reinterpret_cast<const float4*>(p.bias + c0);
-        const float4* btv = reinterpret_cast<const float4*>(p.bias2 + c0);
-#pragma unroll
-        for (int h2 = 0; h2 < 2; h2++) {
-          const int cc = c0 + h2 * 16;
-          float a[16], g[16], dzp[16];
-          ptx::tmem_ld16(tmem + lane_base + buf * N + cc, a);
-          ptx::tmem_ld16(tmem + lane_base + buf * N + 64 + cc, g);
-          if (p.gate_mode == 3) ptx::tmem_ld16(tmem + lane_base + buf * N + 128 + cc, dzp);
-          float4 bs[4], bt[4];
-#pragma unroll
-          for (int i = 0; i < 4; i++) { bs[i] = __ldg(bsv + h2 * 4 + i); bt[i] = __ldg(btv + h2 * 4 + i); }
-          ptx::tc_wait_ld();
-          if (h2 == 1) {
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&dempty[buf]);   // this warp's share of the accumulator is in registers
-          }
-#pragma unroll
-          for (int jj = 0; jj < 4; jj++) {
-            const float4 d4 = pre[h2 * 4 + jj];   // dz slice, requested before the accumulator wait
-            const float dzs[4] = {d4.x, d4.y, d4.z, d4.w};
-            const float bsa[4] = {bs[jj].x, bs[jj].y, bs[jj].z, bs[jj].w}, bta[4] = {bt[jj].x, bt[jj].y, bt[jj].z, bt[jj].w};
-            float da[4], dg[4];
-#pragma unroll
-            for (int k = 0; k < 4; k++) {
-              const int i = 4 * jj + k;
-              float dz = dzs[k];   // (rows past T: zeros from the loader)
-              if (p.gate_mode == 3) dz += dzp[i];
-              const float sg = 0.5f * ptx::tanh_approx(0.5f * (a[i] + bsa[k])) + 0.5f;
-              const float th = ptx::tanh_approx(g[i] + bta[k]);
-              da[k] = dz * th * sg * (1.f - sg);      // d pre-sigmoid
-              dg[k] = dz * sg * (1.f - th * th);      // d pre-tanh
-            }
-            const uint32_t off = (uint32_t)(((h2 * 4 + jj) ^ (lane & 7)) << 4);
-            ptx::st_shared_v4(sb0 + off, da[0], da[1], da[2], da[3]);
-            ptx::st_shared_v4(sb1 + off, dg[0], dg[1], dg[2], dg[3]);
-          }
-        }
-        ptx::fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          ptx::tma_store_3d(&p.maps[9], stg, p.gate_c0 + c0, t0 + q * 32, b);
-          ptx::tma_store_3d(&p.maps[9], stg + kStg, p.gate_R + p.gate_c0 + c0, t0 + q * 32, b);
-          ptx::bulk_commit();
-        }
-        continue;
-      }
-      if constexpr (EPI == EPI_GATE) {
-        // ---- gate epilogues: pair sigmoid column c with tanh column GC + c (GC = 64 or 128 gate channels per tile) ----
-        const int GC = p.gate_gc;
-        for (int c0 = hf * 32; c0 < GC; c0 += 64) {
-          float a[32], g[32];
-          {
-            float lo[16], hi[16];
-            ptx::tmem_ld16(tmem + lane_base + buf * N + c0, lo);
-            ptx::tmem_ld16(tmem + lane_base + buf * N + c0 + 16, hi);
-            ptx::tc_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; i++) { a[i] = lo[i]; a[16 + i] = hi[i]; }
-            ptx::tmem_ld16(tmem + lane_base + buf * N + GC + c0, lo);
-            ptx::tmem_ld16(tmem + lane_base + buf * N + GC + c0 + 16, hi);
-            ptx::tc_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; i++) { g[i] = lo[i]; g[16 + i] = hi[i]; }
-          }
-          float dzp[32];
-          if (p.gate_mode == 3) {
-            float lo[16], hi[16];
-            ptx::tmem_ld16(tmem + lane_base + buf * N + 2 * GC + c0, lo);
-            ptx::tmem_ld16(tmem + lane_base + buf * N + 2 * GC + c0 + 16, hi);
-            ptx::tc_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; i++) { dzp[i] = lo[i]; dzp[16 + i] = hi[i]; }
-          }
-          if (c0 + 64 >= GC) {   // this warp's last chunk: its share of the accumulator is in registers
-            ptx::tc_fence_before();
-            ptx::mbar_arrive(&dempty[buf]);
-          }
-          float dzv[32];
-          if (p.gate_mode == 1) {
-            // forward: z only
-#pragma unroll
-            for (int i = 0; i < 32; i++) {
-              const float sg = 0.5f * ptx::tanh_approx(0.5f * (a[i] + __ldg(p.bias + c0 + i))) + 0.5f;
-              dzv[i] = sg * ptx::tanh_approx(g[i] + __ldg(p.bias2 + c0 + i));
-            }
-            unsigned char* sb = stg + (nstore & box_mask) * kStg;
-            {
-              const long long tb = PROF ? clock64() : 0;
-              if (lane == 0) {
-                if (box_mask) ptx::bulk_wait_read<1>(); else ptx::bulk_wait_read<0>();
-              }
-              __syncwarp();
-              if constexpr (PROF) acc[NP_E_BULK] += clock64() - tb;
-            }
-            float4* dstrow = reinterpret_cast<float4*>(sb + lane * 128);
-#pragma unroll
-            for (int j = 0; j < 8; j++)
-              dstrow[j ^ (lane & 7)] = make_float4(dzv[4 * j], dzv[4 * j + 1], dzv[4 * j + 2], dzv[4 * j + 3]);
-            ptx::fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) {
-              ptx::tma_store_3d(&p.maps[8], sb, p.gate_c0 + c0, t0 + q * 32, b);
-              ptx::bulk_commit();
-            }
-            nstore++;
-            continue;
-          }
-          if (row_ok) {
-            const float4* dr = reinterpret_cast<const float4*>(p.gate_dz + grow * p.gate_ld_dz + p.gate_c0 + c0);
-            const bool use_pre = pre_dz && c0 == hf * 32;   // the first chunk was requested before the accumulator wait
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-              const float4 d4 = use_pre ? pre[j] : __ldg(dr + j);
-              dzv[4 * j] = d4.x; dzv[4 * j + 1] = d4.y; dzv[4 * j + 2] = d4.z; dzv[4 * j + 3] = d4.w;
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; i++) dzv[i] = 0.f;
-          }
-          if (p.gate_mode == 3) {
-#pragma unroll
-            for (int i = 0; i < 32; i++) dzv[i] += dzp[i];
-          }
+        if (p.gate_mode == 1) {
+          // forward: z only
 #pragma unroll
           for (int i = 0; i < 32; i++) {
             const float sg = 0.5f * ptx::tanh_approx(0.5f * (a[i] + __ldg(p.bias + c0 + i))) + 0.5f;
-            const float th = ptx::tanh_approx(g[i] + __ldg(p.bias2 + c0 + i));
-            const float dz = dzv[i];
-            a[i] = dz * th * sg * (1.f - sg);      // d pre-sigmoid
-            g[i] = dz * sg * (1.f - th * th);      // d pre-tanh
-            dzv[i] = sg * th;                      // z
+            dzv[i] = sg * ptx::tanh_approx(g[i] + __ldg(p.bias2 + c0 + i));
           }
+          unsigned char* sb = stg + (nstore & 1) * kStg;
+          if (lane == 0) ptx::bulk_wait_read<1>();
+          __syncwarp();
+          float4* dstrow = reinterpret_cast<float4*>(sb + lane * 128);
 #pragma unroll
-          for (int which = 0; which < 3; which++) {
-            if (which == 0 && p.gate_skip_z) continue;   // (constant trip count: a / g / dzv stay in registers)
-            const float* src = which == 0 ? dzv : (which == 1 ? a : g);
-            unsigned char* sb = stg + (nstore & box_mask) * kStg;
-            {
-              const long long tb = PROF ? clock64() : 0;
-              if (lane == 0) {
-                if (box_mask) ptx::bulk_wait_read<1>(); else ptx::bulk_wait_read<0>();
-              }
-              __syncwarp();
-              if constexpr (PROF) acc[NP_E_BULK] += clock64() - tb;
-            }
-            float4* dstrow = reinterpret_cast<float4*>(sb + lane * 128);
-#pragma unroll
-            for (int j = 0; j < 8; j++)
-              dstrow[j ^ (lane & 7)] = make_float4(src[4 * j], src[4 * j + 1], src[4 * j + 2], src[4 * j + 3]);
-            ptx::fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) {
-              if (which == 0) ptx::tma_store_3d(&p.maps[8], sb, p.gate_c0 + c0, t0 + q * 32, b);
-              else ptx::tma_store_3d(&p.maps[9], sb, (which == 1 ? 0 : p.gate_R) + p.gate_c0 + c0, t0 + q * 32, b);
-              ptx::bulk_commit();
-            }
-            nstore++;
+          for (int j = 0; j < 8; j++)
+            dstrow[j ^ (lane & 7)] = make_float4(dzv[4 * j], dzv[4 * j + 1], dzv[4 * j + 2], dzv[4 * j + 3]);
+          ptx::fence_proxy_async();
+          __syncwarp();
+          if (lane == 0) {
+            ptx::tma_store_3d(&p.maps[8], sb, p.gate_c0 + c0, t0 + q * 32, b);
+            ptx::bulk_commit();
           }
+          nstore++;
+          continue;
         }
-        continue;
+        if (row_ok) {
+          const float4* dr = reinterpret_cast<const float4*>(p.gate_dz + grow * p.gate_ld_dz + p.gate_c0 + c0);
+#pragma unroll
+          for (int j = 0; j < 8; j++) {
+            const float4 d4 = __ldg(dr + j);
+            dzv[4 * j] = d4.x; dzv[4 * j + 1] = d4.y; dzv[4 * j + 2] = d4.z; dzv[4 * j + 3] = d4.w;
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < 32; i++) dzv[i] = 0.f;
+        }
+        if (p.gate_mode == 3) {
+#pragma unroll
+          for (int i = 0; i < 32; i++) dzv[i] += dzp[i];
+        }
+#pragma unroll
+        for (int i = 0; i < 32; i++) {
+          const float sg = 0.5f * ptx::tanh_approx(0.5f * (a[i] + __ldg(p.bias + c0 + i))) + 0.5f;
+          const float th = ptx::tanh_approx(g[i] + __ldg(p.bias2 + c0 + i));
+          const float dz = dzv[i];
+          a[i] = dz * th * sg * (1.f - sg);      // d pre-sigmoid
+          g[i] = dz * sg * (1.f - th * th);      // d pre-tanh
+          dzv[i] = sg * th;                      // z
+        }
+#pragma unroll
+        for (int which = 0; which < 3; which++) {
+          if (which == 0 && p.gate_skip_z) continue;
+          const float* src = which == 0 ? dzv : (which == 1 ? a : g);
+          unsigned char* sb = stg + (nstore & 1) * kStg;
+          if (lane == 0) ptx::bulk_wait_read<1>();
+          __syncwarp();
+          float4* dstrow = reinterpret_cast<float4*>(sb + lane * 128);
+#pragma unroll
+          for (int j = 0; j < 8; j++)
+            dstrow[j ^ (lane & 7)] = make_float4(src[4 * j], src[4 * j + 1], src[4 * j + 2], src[4 * j + 3]);
+          ptx::fence_proxy_async();
+          __syncwarp();
+          if (lane == 0) {
+            if (which == 0) ptx::tma_store_3d(&p.maps[8], sb, p.gate_c0 + c0, t0 + q * 32, b);
+            else ptx::tma_store_3d(&p.maps[9], sb, (which == 1 ? 0 : p.gate_R) + p.gate_c0 + c0, t0 + q * 32, b);
+            ptx::bulk_commit();
+          }
+          nstore++;
+        }
       }
-      if constexpr (EPI == EPI_PLAIN) {
-      if (hf * 32 >= N) {  // N == 32: the second warp of the pair has no chunk
-        ptx::tc_fence_before();
-        ptx::mbar_arrive(&dempty[buf]);
-      }
+      continue;
+    }
+    if constexpr (EPI == EPI_PLAIN) {
       for (int c0 = hf * 32; c0 < N; c0 += 64) {
         float v[32];
-        {
-          float lo[16], hi[16];
-          ptx::tmem_ld16(tmem + lane_base + buf * N + c0, lo);
-          ptx::tmem_ld16(tmem + lane_base + buf * N + c0 + 16, hi);
-          ptx::tc_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 16; i++) { v[i] = lo[i]; v[16 + i] = hi[i]; }
-        }
-        if (c0 + 64 >= N) {  // this warp's last chunk is in registers: the accumulator can be overwritten
-          ptx::tc_fence_before();
-          ptx::mbar_arrive(&dempty[buf]);
-        }
+        acc_ld16(accs, c0, row, *reinterpret_cast<float(*)[16]>(v));
+        acc_ld16(accs, c0 + 16, row, *reinterpret_cast<float(*)[16]>(v + 16));
         const bool second = p.out2_col0 > 0 && c0 >= p.out2_col0;
         if (p.bias && !second) {
 #pragma unroll
           for (int i = 0; i < 32; i++) v[i] += __ldg(p.bias + ncol0 + c0 + i);
         }
-        if (p.etile == 2 && c0 < 64) {   // staged residual tile: sub-tile c0 / 32, this thread's row
-          wait(efull, it & 1, NP_E_DFULL);
-          const float4* er = reinterpret_cast<const float4*>(ebuf + (c0 >> 5) * kASub + (q * 32 + lane) * 128);
-#pragma unroll
-          for (int j = 0; j < 8; j++) {
-            const float4 a = er[j ^ (lane & 7)];
-            v[4 * j] += a.x; v[4 * j + 1] += a.y; v[4 * j + 2] += a.z; v[4 * j + 3] += a.w;
-          }
-          ptx::mbar_arrive(eempty);
-        } else if (p.add && row_ok && !second) {
+        if (p.add && row_ok && !second) {
           const float4* ar = reinterpret_cast<const float4*>(p.add + grow * p.ldadd + ncol0 + c0);
-          const bool use_pre = pre_add && c0 == hf * 32;
 #pragma unroll
           for (int j = 0; j < 8; j++) {
-            const float4 a = use_pre ? pre[j] : __ldg(ar + j);
+            const float4 a = __ldg(ar + j);
             v[4 * j] += a.x; v[4 * j + 1] += a.y; v[4 * j + 2] += a.z; v[4 * j + 3] += a.w;
           }
         }
@@ -601,15 +334,9 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
             v[4 * j + 2] = m.z > 0.f ? v[4 * j + 2] : 0.f; v[4 * j + 3] = m.w > 0.f ? v[4 * j + 3] : 0.f;
           }
         }
-        unsigned char* sb = stg + (nstore & box_mask) * kStg;
-        {
-          const long long tb = PROF ? clock64() : 0;
-          if (lane == 0) {
-            if (box_mask) ptx::bulk_wait_read<1>(); else ptx::bulk_wait_read<0>();
-          }
-          __syncwarp();
-          if constexpr (PROF) acc[NP_E_BULK] += clock64() - tb;
-        }
+        unsigned char* sb = stg + (nstore & 1) * kStg;
+        if (lane == 0) ptx::bulk_wait_read<1>();
+        __syncwarp();
         float4* dstrow = reinterpret_cast<float4*>(sb + lane * 128);
 #pragma unroll
         for (int j = 0; j < 8; j++)
@@ -624,26 +351,9 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
         }
         nstore++;
       }
-      }  // EPI_PLAIN
-     }  // mh
-    }
-    if (lane == 0) ptx::bulk_wait<0>();
-    if constexpr (PROF) {
-      if (warp == 2 && lane == 0) {
-        acc[NP_E_TOTAL] = clock64() - t_begin;
-        atomicMin(&g_nt_prof[NP_MIN], (unsigned long long)acc[NP_E_TOTAL]);
-        atomicMax(&g_nt_prof[NP_MAX], (unsigned long long)acc[NP_E_TOTAL]);
-      }
     }
   }
-  if constexpr (PROF) {
-    if (warp <= 1 || (warp == 2 && lane == 0))   // single-thread roles: only the elected lane has counts
-      for (int k = 0; k < NP_MIN; k++)
-        if (acc[k]) atomicAdd(&g_nt_prof[k], (unsigned long long)acc[k]);
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc<512>(tmem);
+  if (lane == 0) ptx::bulk_wait<0>();
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -670,17 +380,6 @@ static bool map3(CUtensorMap* m, const float* base, int C, int T, int B, int box
              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
-// (B, T, C) view with row pitch ld floats (a channel slice of a wider tensor)
-static bool map3ld(CUtensorMap* m, const float* base, int C, int ld, int T, int B, int box_rows) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return false;
-  cuuint64_t gdim[3] = {(cuuint64_t)C, (cuuint64_t)T, (cuuint64_t)B};
-  cuuint64_t gstr[2] = {(cuuint64_t)ld * 4, (cuuint64_t)ld * 4 * (cuuint64_t)T};
-  cuuint32_t box[3] = {32, (cuuint32_t)box_rows, 1}, es[3] = {1, 1, 1};
-  return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), gdim, gstr, box, es,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
 static bool map2(CUtensorMap* m, const float* base, int K, int Nrows, int box_rows) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return false;
@@ -692,13 +391,28 @@ static bool map2(CUtensorMap* m, const float* base, int K, int Nrows, int box_ro
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-}  // namespace nt
-
-int nt_default_m_tiles() {
-  static int mt = 0;
-  if (!mt) { const char* e = getenv("WNB_NT_MT"); mt = (e && e[0] == '1') ? 1 : 2; }
-  return mt;
+template <int N, int EPI>
+static cudaError_t launch_n(int grid, size_t smem, cudaStream_t st, const Params& p) {
+  cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(gemm_nt_tc_kernel<N, EPI>), smem);
+  if (e != cudaSuccess) return e;
+  return launch_pdl(gemm_nt_tc_kernel<N, EPI>, grid, kThreadsN, smem, st, p);
 }
+
+template <int EPI>
+static cudaError_t launch_epi(int N, int grid, size_t smem, cudaStream_t st, const Params& p) {
+  switch (N) {
+    case 32: return launch_n<32, EPI>(grid, smem, st, p);
+    case 64: return launch_n<64, EPI>(grid, smem, st, p);
+    case 96: return launch_n<96, EPI>(grid, smem, st, p);
+    case 128: return launch_n<128, EPI>(grid, smem, st, p);
+    case 160: return launch_n<160, EPI>(grid, smem, st, p);
+    case 192: return launch_n<192, EPI>(grid, smem, st, p);
+    case 224: return launch_n<224, EPI>(grid, smem, st, p);
+    default: return launch_n<256, EPI>(grid, smem, st, p);
+  }
+}
+
+}  // namespace nt
 
 int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, const float* bias, const float* mask,
                int ldmask, const float* add, int ldadd, int relu_out, int accumulate, int B, int T, cudaStream_t st,
@@ -711,38 +425,25 @@ int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, con
   }
   Params p;
   memset(&p, 0, sizeof(p));
-  const int nbox = gate ? N / 2 : (N > 256 ? 256 : N);   // (gate: two boxes of GC = N/2 rows, sigmoid rows and tanh rows)
-  // resident weights: the segments' column ranges must tile [0, N) front to back -- a range either starts where the
-  // covered prefix ends (its first MMA overwrites) or lies inside it (accumulates)
-  bool wres = opts && opts->resident_weights && !gate && N <= 256 && !(opts->n_blocks > 1) && opts->m_tiles != 2;
-  int wres_bytes = 0, covered = 0;
-  int n_lo[kMaxSeg], n_cnt[kMaxSeg], fresh[kMaxSeg];
-  for (int s = 0; s < nseg && wres; s++) {
-    n_cnt[s] = segs[s].n_cnt > 0 ? segs[s].n_cnt : N;
-    n_lo[s] = segs[s].n_cnt > 0 ? segs[s].n_lo : 0;
-    if (n_cnt[s] % 16 != 0 || n_lo[s] % 32 != 0 || n_lo[s] + n_cnt[s] > N) wres = false;
-    else if (n_lo[s] == covered) { fresh[s] = 1; covered += n_cnt[s]; }
-    else if (n_lo[s] + n_cnt[s] <= covered) fresh[s] = 0;
-    else wres = false;
-    wres_bytes += (segs[s].K / 32) * n_cnt[s] * 128;
+  p.nblk = (opts && opts->n_blocks > 1) ? opts->n_blocks : 1;
+  if (N == 512) {   // the accumulator of one tile is at most 256 columns: two column blocks
+    if (gate || gate_dz || out2 || p.nblk > 1) {
+      set_error("gemm_nt_tc: N = 512 is for plain epilogues without column blocks");
+      return WNB_ERR_INVALID;
+    }
+    N = 256;
+    p.nblk = 2;
   }
-  if (wres && covered != N) wres = false;
-  if (opts && opts->resident_weights && !wres) {
-    set_error("gemm_nt_tc: resident weights need plain segments whose column ranges tile [0, N)");
-    return WNB_ERR_INVALID;
-  }
+  const int nbox = gate ? N / 2 : N;   // (gate: two boxes of GC = N/2 rows, sigmoid rows and tanh rows)
   for (int s = 0; s < nseg; s++) {
     if (segs[s].K % 32 != 0) { set_error("gemm_nt_tc: K must be a multiple of 32"); return WNB_ERR_INVALID; }
     if (!map3(&p.maps[s], segs[s].a, segs[s].CA, T, B, kTM) ||
-        !map2(&p.maps[4 + s], segs[s].w, segs[s].w_cols, segs[s].w_rows, wres ? n_cnt[s] : nbox)) {
+        !map2(&p.maps[4 + s], segs[s].w, segs[s].w_cols, segs[s].w_rows, nbox)) {
       set_error("gemm_nt_tc: tensor map creation failed");
       return WNB_ERR_CUDA;
     }
-    p.seg[s] = Seg{s, segs[s].shift, segs[s].K, 4 + s, segs[s].k0, segs[s].n0, -1, wres ? n_lo[s] : 0, wres ? n_cnt[s] : N,
-                   wres ? fresh[s] : (s == 0)};
+    p.seg[s] = Seg{s, segs[s].shift, segs[s].K, 4 + s, segs[s].k0, segs[s].n0, -1};
   }
-  p.wres = wres ? 1 : 0;
-  p.wres_bytes = wres ? wres_bytes : 0;
   for (int s = nseg; s < 4; s++) { p.maps[s] = p.maps[0]; p.maps[4 + s] = p.maps[4]; }
   if (!map3(&p.maps[8], out, ld_out, T, B, 32)) { set_error("gemm_nt_tc: output map failed"); return WNB_ERR_CUDA; }
   p.maps[9] = p.maps[8];
@@ -779,94 +480,40 @@ int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, con
     p.out2_col0 = out2_col0;
   }
   p.nseg = nseg; p.N = N; p.T = T; p.B = B;
-  p.nblk = (opts && opts->n_blocks > 1) ? opts->n_blocks : 1;
   p.gate_ld_dz = (opts && opts->gate_ld_dz > 0) ? opts->gate_ld_dz : p.gate_R;
   p.gate_skip_z = (opts && opts->gate_skip_z) ? 1 : 0;
-  if (p.nblk > 1 && (p.gate_mode || out2 || N > 256)) {
-    set_error("gemm_nt_tc: column blocks are for plain epilogues with N <= 256");
+  if (p.nblk > 1 && (p.gate_mode || out2)) {
+    set_error("gemm_nt_tc: column blocks are for plain epilogues");
     return WNB_ERR_INVALID;
   }
   if (!p.gate_mode) p.bias = bias;   // (the gate modes have already installed their own bias pointers)
   p.mask = mask; p.ldmask = ldmask; p.add = add; p.ldadd = ldadd;
   p.relu_out = relu_out; p.accumulate = accumulate;
-  p.nacc = N <= 256 ? 2 : 1;
-  p.mt = (opts && opts->m_tiles == 2) ? 2 : 1;
-  if (p.mt == 2 && ((p.gate_mode && !gate) || N > 256)) {
-    set_error("gemm_nt_tc: m_tiles = 2 is for plain / general gate epilogues with N <= 256");
+  p.rev = (opts && opts->reverse) ? 1 : 0;
+  const int epi = !p.gate_mode ? EPI_PLAIN : ((p.gate_mode >= 2 && p.gate_skip_z) ? EPI_GATE_BWD_NOZ : EPI_GATE);
+  if (epi == EPI_GATE_BWD_NOZ && (p.gate_gc != 64 || (reinterpret_cast<uintptr_t>(p.gate_dz) & 15) || p.gate_ld_dz % 4)) {
+    set_error("gemm_nt_tc: the gate backward without z needs 64 gate channels and a 16-byte aligned dz");
     return WNB_ERR_INVALID;
   }
-  p.stg_boxes = p.mt == 2 ? 1 : 2;
-  {  // resident-weights launches with a plain epilogue: one staging box per warp leaves room for two more activation stages
-    static int one = -1;
-    if (one < 0) { const char* e = getenv("WNB_NT_STG1"); one = (e && e[0] == '0') ? 0 : 1; }   // (dX: 47.4 -> 46.4 us)
-    if (one && p.wres && !p.gate_mode) p.stg_boxes = 1;
-  }
-  p.maps[10] = p.maps[8];
-  static int pf_dist = -1;
-  if (pf_dist < 0) { const char* e = getenv("WNB_NT_PF"); pf_dist = e ? atoi(e) : 0; if (pf_dist < 0 || pf_dist > 4) pf_dist = 0; }
-  static int grp = 0;
-  if (!grp) { const char* e = getenv("WNB_NT_GRP"); grp = e ? atoi(e) : 1; if (grp < 1 || grp > 4) grp = 1; }
-  p.grp = grp;
-  p.rev = (opts && opts->reverse) ? 1 : 0;
-  p.pf = p.wres ? pf_dist : 0;
-  if (p.mt == 1 && ((opts && opts->stage_epilogue_operand) || p.pf)) {
-    // 1: gate-backward dz slice (EPI_GATE_BWD_NOZ, R = 64 shorthand), 2: residual add of a <= 64-column primary output
-    const bool stage = opts && opts->stage_epilogue_operand;
-    const bool dz_ok = p.gate_mode >= 2 && p.gate_skip_z && p.gate_R == 64 && p.gate_c0 == 0 && gate_dz &&
-                       (reinterpret_cast<uintptr_t>(gate_dz) & 15) == 0 && p.gate_ld_dz % 4 == 0;
-    const int primary = out2 ? out2_col0 : N;
-    const bool add_ok = !p.gate_mode && add && !mask && primary == 64 && p.nblk == 1 &&
-                        (reinterpret_cast<uintptr_t>(add) & 15) == 0 && ldadd % 4 == 0;
-    int kind = 0;
-    if (dz_ok && map3ld(&p.maps[10], gate_dz, 64, p.gate_ld_dz, T, B, kTM)) kind = 1;
-    else if (add_ok && map3ld(&p.maps[10], add, 64, ldadd, T, B, kTM)) kind = 2;
-    if (stage) p.etile = kind; else p.epf = kind;
-  }
-  const int ebytes = p.etile ? 2 * kASub : 0;
-  const int stage_bytes = p.mt * kASub + (p.wres ? 0 : N * 128);
-  int nst = (int)((227 * 1024 - 1024 - 512 - kEpiWarpsN * p.stg_boxes * kStg - ebytes - p.wres_bytes) / stage_bytes);
-  static int max_stages = 0;
-  if (!max_stages) { const char* e = getenv("WNB_NT_MAXSTAGES"); max_stages = e ? atoi(e) : 4; if (max_stages < 2) max_stages = 2; }
-  const int cap = p.wres ? 8 : max_stages;   // (activation-only stages are 16 KB: take what is left)
-  if (nst > cap) nst = cap;
+  // shared memory: ring stages (A box + weight box) | accumulator copy | 4 warps x 2 staging boxes | barriers.  When three
+  // stages fit in half of the SM, two CTAs share it and one's epilogue overlaps the other's mainloop.
+  const int stage_bytes = kASub + N * 128;
+  const int fixed = acc_bytes(N) + 4 * 2 * kStg + 1024 + 256;
+  const int sm_bytes = 227 * 1024, half = 113 * 1024;
+  const int ctas = fixed + 3 * stage_bytes <= half ? 2 : 1;
+  int nst = ((ctas == 2 ? half : sm_bytes) - fixed) / stage_bytes;
+  if (nst > 6) nst = 6;
   if (nst < 2) { set_error("gemm_nt_tc: N too large"); return WNB_ERR_INVALID; }
   p.nstages = nst;
-  const size_t smem = (size_t)p.wres_bytes + (size_t)nst * stage_bytes + kEpiWarpsN * p.stg_boxes * kStg + ebytes + 512 + 1024;
-  WNB_CUDA(ensure_dynamic_smem(reinterpret_cast<const void*>(gemm_nt_tc_kernel<false, 0>), smem));
-  WNB_CUDA(ensure_dynamic_smem(reinterpret_cast<const void*>(gemm_nt_tc_kernel<false, 1>), smem));
-  WNB_CUDA(ensure_dynamic_smem(reinterpret_cast<const void*>(gemm_nt_tc_kernel<false, 2>), smem));
-  WNB_CUDA(ensure_dynamic_smem(reinterpret_cast<const void*>(gemm_nt_tc_kernel<true, 0>), smem));
-  WNB_CUDA(ensure_dynamic_smem(reinterpret_cast<const void*>(gemm_nt_tc_kernel<true, 1>), smem));
-  WNB_CUDA(ensure_dynamic_smem(reinterpret_cast<const void*>(gemm_nt_tc_kernel<true, 2>), smem));
+  const size_t smem = (size_t)fixed + (size_t)nst * stage_bytes;
   const int sms = device_sms();
-  const int ntiles = B * ((T + kTM * p.mt - 1) / (kTM * p.mt)) * p.nblk;
-  const int grid = ntiles < sms ? ntiles : sms;
-  const int epi = !p.gate_mode ? EPI_PLAIN : ((p.gate_mode >= 2 && p.gate_skip_z) ? EPI_GATE_BWD_NOZ : EPI_GATE);
-  static int prof = -1;
-  if (prof < 0) { const char* e = getenv("WNB_PROF"); prof = (e && e[0] == '1') ? 1 : 0; }
-  if (prof) {
-    unsigned long long zero[NP_COUNT] = {}, h[NP_COUNT];
-    zero[NP_MIN] = ~0ull;
-    WNB_CUDA(cudaMemcpyToSymbol(g_nt_prof, zero, sizeof(zero)));
-    if (epi == EPI_PLAIN) gemm_nt_tc_kernel<true, 0><<<grid, kThreadsN, smem, st>>>(p);
-    else if (epi == EPI_GATE) gemm_nt_tc_kernel<true, 1><<<grid, kThreadsN, smem, st>>>(p);
-    else gemm_nt_tc_kernel<true, 2><<<grid, kThreadsN, smem, st>>>(p);
-    WNB_CHECK_LAUNCH("gemm_nt_tc");
-    WNB_CUDA(cudaStreamSynchronize(st));
-    WNB_CUDA(cudaMemcpyFromSymbol(h, g_nt_prof, sizeof(h)));
-    int kc = 0;
-    for (int i = 0; i < nseg; i++) kc += segs[i].K / 32;
-    fprintf(stderr, "wnb200 nt prof N=%d kchunks=%d gate=%d stages=%d (kcycles/CTA): P:empty=%.1f M:dempty=%.1f M:full=%.1f "
-            "M:total=%.1f E:dfull=%.1f E:bulk=%.1f E:total=%.1f cta min=%.1f max=%.1f\n", N, kc, p.gate_mode, nst,
-            h[0] / 1e3 / grid, h[1] / 1e3 / grid, h[2] / 1e3 / grid, h[3] / 1e3 / grid, h[4] / 1e3 / grid,
-            h[5] / 1e3 / grid, h[6] / 1e3 / grid, h[7] / 1e3, h[8] / 1e3);
-    return WNB_OK;
-  }
+  const int ntiles = B * ((T + kTM - 1) / kTM) * p.nblk;
+  const int grid = ntiles < sms * ctas ? ntiles : sms * ctas;
   cudaError_t le;
-  if (epi == EPI_PLAIN) le = launch_pdl(gemm_nt_tc_kernel<false, 0>, grid, kThreadsN, smem, st, p);
-  else if (epi == EPI_GATE) le = launch_pdl(gemm_nt_tc_kernel<false, 1>, grid, kThreadsN, smem, st, p);
-  else le = launch_pdl(gemm_nt_tc_kernel<false, 2>, grid, kThreadsN, smem, st, p);
-  (void)le;   // reported by WNB_CHECK_LAUNCH below
+  if (epi == EPI_PLAIN) le = launch_epi<EPI_PLAIN>(N, grid, smem, st, p);
+  else if (epi == EPI_GATE) le = launch_epi<EPI_GATE>(N, grid, smem, st, p);
+  else le = launch_epi<EPI_GATE_BWD_NOZ>(N, grid, smem, st, p);
+  if (le != cudaSuccess) { set_error("gemm_nt_tc: launch failed: %s", cudaGetErrorString(le)); return WNB_ERR_CUDA; }
   WNB_CHECK_LAUNCH("gemm_nt_tc");
   return WNB_OK;
 }

@@ -85,7 +85,7 @@ WNB_API int wnb_make_train_batch(const float* wave, const void* feat, const int3
                   cap_s > T && cap_f >= Tf,
               "make_train_batch: bad arguments");
   const int work = (T + 1 > D * Tf) ? T + 1 : D * Tf;
-  dim3 grid((unsigned)((work + 255) / 256 < 148 ? (work + 255) / 256 : 148), (unsigned)B);
+  dim3 grid((unsigned)((work + 255) / 256 < device_sms() ? (work + 255) / 256 : device_sms()), (unsigned)B);
   make_train_batch_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(wave, feat, frame_of_sample, s0, hop, U, cap_s, cap_f, mean,
                                                                  scale, x, t, h, B, T, Tf, D, feat_f64, (float)(mu - 1),
                                                                  log(1.0 + (double)(mu - 1)));   // wavenet.py:27 mu = mu - 1

@@ -11,7 +11,7 @@
 //                              fp32 atomics), colsum_kernel: bias gradients.
 //
 // All activations are channels-last (B,T,C).  Everything here is fp32 FFMA: this is the parity path and
-// the fallback for shapes the tcgen05 path (resblock_tc.cu) does not cover.
+// the fallback for shapes the tensor-core paths do not cover.
 #include <stdlib.h>
 
 #include "gemm_simt.cuh"
@@ -341,8 +341,8 @@ static int launch_colsum(const float* a, int lda, int M, int64_t rows, float* ou
 }
 
 static int pick_tchunk(int B, int T, int tiles) {
-  // aim for ~2 waves of CTAs over 148 SMs; chunks are multiples of 16 time steps
-  int64_t want = 148 * 2;
+  // aim for ~2 waves of CTAs over the SMs; chunks are multiples of 16 time steps
+  int64_t want = (int64_t)device_sms() * 2;
   int nsplit = (int)((want + (int64_t)tiles * B - 1) / ((int64_t)tiles * B));
   if (nsplit < 1) nsplit = 1;
   int chunk = (T + nsplit - 1) / nsplit;
@@ -351,18 +351,8 @@ static int pick_tchunk(int B, int T, int tiles) {
   return chunk;
 }
 
-// N == 512 GEMMs of the post network run as two 256-column blocks: the accumulators are then double-buffered and the
-// epilogue of one tile overlaps the mainloop of the next (-0.2 ms on the 10 ms step); WNB_POST_SPLIT=0 switches it off
-// Time tiles per weight chunk in the post-network GEMMs.  Measured on B200 (same box, 20 steps each): ONE tile with
-// double-buffered accumulators beats two tiles by 0.12-0.16 ms per step here -- K is 256 / 512 (short main loops) and the
-// epilogues are heavy (bias + ReLU, sign masks read from memory), so overlapping the epilogue with the next tile's main
-// loop is worth more than halving the weight traffic; the K = 1920 skip GEMM and the store-only dZ_all GEMM are the
-// opposite case.  WNB_POST_MT=2 selects the two-tile form.
-static int post_m_tiles() {
-  static const int mt = [] { const char* e = getenv("WNB_POST_MT"); return (e && e[0] == '2') ? 2 : 1; }();
-  return mt;
-}
-
+// N == 512 GEMMs of the post network as two explicit 256-column blocks (WNB_POST_SPLIT=0: one N = 512 call, which
+// gemm_nt_tc splits the same way)
 static bool post_split(int S) {
   static int on = -1;
   if (on < 0) { const char* e = getenv("WNB_POST_SPLIT"); on = (e && e[0] == '0') ? 0 : 1; }
@@ -399,7 +389,7 @@ static int wgrad_tc_full(const float* a, int CA, int M, const float* b, int CB, 
 }
 
 // C (M x N, ldc) += A^T B, db (M) += colsum A, with A = channels [0, M) of a (CA), B = channels [0, N) of b (CB):
-// up to 4 M-blocks per launch (their accumulators share TMEM) and the N axis split into column groups handled by
+// up to 4 M-blocks per launch and the N axis split into column groups handled by
 // different CTAs (WgOpts::n_split), so a 512 x 512 gradient is ONE launch that streams A and B once from HBM.
 static int wgrad_tc_split(const float* a, int CA, int M, const float* b, int CB, int N, float* c, int ldc, float* db,
                           int B, int T, cudaStream_t st) {
@@ -428,7 +418,7 @@ static int wgrad_tc_split(const float* a, int CA, int M, const float* b, int CB,
 
 // Weight gradient with A = the channel concatenation [a0 (C0) | a1 (C1)] (a1 may be null), M = rows used,
 // B = channels [0, N) of tensor b (CB channels) read at time t + shift:  C (M x N, ldc) += A^T B, db (M) += colsum A.
-// M-blocks of 128 rows are batched per launch as far as TMEM allows; N goes in chunks of <= 224 columns.
+// M-blocks of 128 rows are batched per launch (up to 5); N goes in chunks of <= 224 columns.
 static int wgrad_tc_concat(const float* a0, int C0, const float* a1, int C1, int M, const float* b, int CB, int N,
                            int shift, float* c, int ldc, float* db, int B, int T, cudaStream_t st) {
   // The N axis is split into column groups handled by different CTAs of ONE launch (WgOpts::n_split, as wgrad_tc_split
@@ -438,14 +428,11 @@ static int wgrad_tc_concat(const float* a0, int C0, const float* a1, int C1, int
   int rc;
   const int groups = N / 32;
   if (N % 32 != 0 || groups < 1) { set_error("wgrad_tc_concat: N must be a multiple of 32"); return WNB_ERR_INVALID; }
-  // column groups of <= 128 columns per CTA (largest divisor of N/32 up to 4): three M-blocks (+ bias column group) then
-  // share the 512 TMEM columns, the tile [384 x 128] is close to square
+  // column groups of <= 128 columns per CTA (largest divisor of N/32 up to 4)
   int nB = 1;
   for (int g = 4; g >= 1; g--)
     if (groups % g == 0 && groups / g <= 128) { nB = g; break; }
-  const int cols = 32 * (nB + (db ? 1 : 0));
-  int per_launch = 512 / cols;
-  if (per_launch > 5) per_launch = 5;
+  int per_launch = 5;
   {  // same number of launches, evenly filled (4 M-blocks: 2 + 2 rather than 3 + 1)
     const int mblocks = (M + 127) / 128, launches = (mblocks + per_launch - 1) / per_launch;
     per_launch = (mblocks + launches - 1) / launches;
@@ -481,22 +468,16 @@ static int wgrad_tc_concat(const float* a0, int C0, const float* a1, int C1, int
   return WNB_OK;
 }
 
-// shapes the composed tensor-core path covers (generic tcgen05 GEMMs + gate epilogues per 64-channel chunk)
+// shapes the composed tensor-core path covers (generic wgmma GEMMs + gate epilogues per 64-channel chunk)
 static bool composed_tc_supported(int R, int S, int Ap, int ks) {
   return R % 64 == 0 && nt_tc_n_ok(R) && nt_tc_n_ok(S) && Ap % 32 == 0 && Ap <= 256 && ks >= 1 && ks <= 3;
 }
 
-// implemented in resblock_tc.cu
-int resblock_fwd_tc(const FwdParams& p, cudaStream_t st);
-bool resblock_fwd_tc_supported(int R, int S, int Ap, int ks);
-
 // gate channels per composed gate GEMM, and the column blocking / two-time-tile option of the plain composed GEMMs
 static int composed_gc(int R) { return (R % 128 == 0) ? 128 : 64; }
 static NtTcOpts plain_opts(int N) {
-  NtTcOpts o{1, 0, 0, 0, 1, 0};
+  NtTcOpts o{1};
   if (N > 256 && N % 256 == 0) o.n_blocks = N / 256;
-  static const int cmt = [] { const char* e = getenv("WNB_COMPOSED_MT"); return (e && e[0] == '1') ? 1 : 2; }();
-  if (N / o.n_blocks <= 256) o.m_tiles = cmt == 1 ? 1 : nt_default_m_tiles();
   return o;
 }
 
@@ -512,11 +493,10 @@ static int resblock_fwd_composed(const FwdParams& p, cudaStream_t st) {
   // 128 gate channels (N = 256) and two time tiles per CTA tile when R allows: the activation tile [x taps | aux] is
   // re-read R/128 instead of R/64 times and every weight chunk serves 256 rows (these GEMMs are L2 -> SM bound)
   const int GC = composed_gc(R);
-  const NtTcOpts og{1, 0, 0, 0, nt_default_m_tiles(), 0};
-  for (int c0 = 0; c0 < R; c0 += GC) {
+    for (int c0 = 0; c0 < R; c0 += GC) {
     const NtTcGate g{1, c0, R, p.b1 + c0, p.b1 + R + c0, nullptr, nullptr};
     if ((rc = gemm_nt_tc(segs, ns, 2 * GC, p.zsave, R, nullptr, nullptr, 0, nullptr, 0, 0, 0, p.B, p.T, st, nullptr, nullptr,
-                         nullptr, 0, 0, &g, &og)) != WNB_OK)
+                         nullptr, 0, 0, &g)) != WNB_OK)
       return rc;
   }
   if (p.xout) {
@@ -545,11 +525,21 @@ WNB_API int wnb_resblock_fwd(const float* xin, const float* haux, const float* w
   WNB_REQUIRE(xin && haux && w1 && b1 && w2 && b2 && skip, "resblock_fwd: null pointer");
   FwdParams p{xin, haux, w1, b1, w2, b2, xout, skip, zsave, B, T, R, S, Ap, ks, dilation, skip_init};
   if (math_mode == WNB_MATH_TF32) {
-    if (resblock_fwd_tc_supported(R, S, Ap, ks)) return resblock_fwd_tc(p, (cudaStream_t)stream);
+    if (resblock_fwd_skip_supported(R, S, Ap, ks)) {
+      WNB_REQUIRE(!zsave, "resblock_fwd: the fused per-block kernel keeps z on chip (pass no zsave)");
+      return resblock_fwd_skip(xin, haux, w1, b1, w2, b2, xout, skip, B, T, S, dilation, skip_init, (cudaStream_t)stream);
+    }
     WNB_REQUIRE(composed_tc_supported(R, S, Ap, ks), "resblock_fwd: shape R=%d S=%d Ap=%d ks=%d not supported by the "
-                "tcgen05 paths (use WNB_MATH_FP32)", R, S, Ap, ks);
-    WNB_REQUIRE(zsave, "resblock_fwd: the composed tcgen05 path needs the zsave (B,T,R) scratch buffer");
-    return resblock_fwd_composed(p, (cudaStream_t)stream);
+                "tensor-core paths (use WNB_MATH_FP32)", R, S, Ap, ks);
+    if (zsave) return resblock_fwd_composed(p, (cudaStream_t)stream);
+    // no z scratch from the caller: a stream-ordered (B,T,R) buffer for the duration of the call
+    cudaStream_t st = (cudaStream_t)stream;
+    float* z = nullptr;
+    WNB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&z), (size_t)B * T * R * sizeof(float), st));
+    p.zsave = z;
+    const int rc = resblock_fwd_composed(p, st);
+    WNB_CUDA(cudaFreeAsync(z, st));
+    return rc;
   }
   WNB_REQUIRE(math_mode == WNB_MATH_FP32, "resblock_fwd: unknown math_mode %d", math_mode);
   const size_t smem = sizeof(TileSmem<8>) + (size_t)R * kBsLd * sizeof(float);
@@ -576,8 +566,8 @@ WNB_API int wnb_causal_conv1d_fwd(const float* x, const float* w, const float* b
 
 WNB_API int wnb_resblock_fwd_supported(int R, int S, int Ap, int ks, int math_mode) {
   if (R <= 0 || S <= 0 || Ap <= 0 || ks < 1) return 0;
-  if (math_mode == WNB_MATH_TF32)   // 1 = fused kernel, 2 = composed tcgen05 path (needs the zsave scratch)
-    return resblock_fwd_tc_supported(R, S, Ap, ks) ? 1 : (composed_tc_supported(R, S, Ap, ks) ? 2 : 0);
+  if (math_mode == WNB_MATH_TF32)   // 1 = fused per-block kernel, 2 = composed tensor-core path (zsave scratch)
+    return resblock_fwd_skip_supported(R, S, Ap, ks) ? 1 : (composed_tc_supported(R, S, Ap, ks) ? 2 : 0);
   return (sizeof(TileSmem<8>) + (size_t)R * kBsLd * sizeof(float)) <= 227 * 1024 ? 1 : 0;
 }
 
@@ -620,11 +610,10 @@ WNB_API int wnb_resblock_bwd(const float* xin, const float* haux, const float* d
     for (int j = 0; j < ks; j++) sg[ns++] = NtTcSeg{xin, R, -(ks - 1 - j) * dilation, R, w1, 2 * R, K1, j * R, 0};
     sg[ns++] = NtTcSeg{haux, Ap, 0, Ap, w1, 2 * R, K1, ks * R, 0};
     const int GC = composed_gc(R);
-    const NtTcOpts og{1, 0, 0, 0, nt_default_m_tiles(), 0};
-    for (int c0 = 0; c0 < R; c0 += GC) {   // gate recompute + z + dpre, GC gate channels per launch
+        for (int c0 = 0; c0 < R; c0 += GC) {   // gate recompute + z + dpre, GC gate channels per launch
       const NtTcGate g{2, c0, R, b1 + c0, b1 + R + c0, dz, dpre};
       if ((rc = gemm_nt_tc(sg, ns, 2 * GC, z, R, nullptr, nullptr, 0, nullptr, 0, 0, 0, B, T, st, nullptr, nullptr, nullptr, 0,
-                           0, &g, &og)) != WNB_OK)
+                           0, &g)) != WNB_OK)
         return rc;
     }
     {  // dxin = dout + sum_j dpre(t + (ks-1-j)d) W1[:, tap j]
@@ -713,7 +702,7 @@ WNB_API int wnb_resblock_bwd(const float* xin, const float* haux, const float* d
       if ((rc = wgrad_tc(a, 1, b, 3, dw1, K1, 128, db1, B, T, st)) != WNB_OK) return rc;
     }
     // dW2 (R+S x R) += [dout | dskip]^T z,  db2 = column sums of [dout | dskip]: row blocks of 128, up to 5 per
-    // launch (their accumulators share TMEM, so z and dskip are streamed once)
+    // launch (z and dskip are streamed once, through L2)
     const WgOperand bz[1] = {{z, R, 0, 2, 0}};
     const int row_first = dout ? 0 : R;
     WgBlock blk[5];
@@ -777,18 +766,18 @@ WNB_API int wnb_post_fwd(float* skip, const float* wp1, const float* bp1, const 
     // tensor-core GEMMs with fused bias / ReLU epilogues
     const int64_t n4 = (int64_t)B * T * S / 4;
     if (!skip_rectified) {
-      relu_inplace_kernel<<<148 * 8, 256, 0, st>>>(reinterpret_cast<float4*>(skip), n4);
+      relu_inplace_kernel<<<device_sms() * 8, 256, 0, st>>>(reinterpret_cast<float4*>(skip), n4);
       WNB_CHECK_LAUNCH("relu_inplace");
     }
     const NtTcSeg s1[1] = {{skip, S, 0, S, wp1, S, S, 0, 0}};
     if (post_split(S)) {   // two 256-column blocks: double-buffered accumulators, epilogue overlapped with the next tile
-      const NtTcOpts o{2, 0, 0, 0, post_m_tiles()};
+      const NtTcOpts o{2};
       if ((rc = gemm_nt_tc(s1, 1, S / 2, r1, S, bp1, nullptr, 0, nullptr, 0, 1, 0, B, T, st, nullptr, nullptr, nullptr, 0, 0,
                            nullptr, &o)) != WNB_OK)
         return rc;
     } else if ((rc = gemm_nt_tc(s1, 1, S, r1, S, bp1, nullptr, 0, nullptr, 0, 1, 0, B, T, st)) != WNB_OK) return rc;
     const NtTcSeg s2[1] = {{r1, S, 0, S, wp2, Q, S, 0, 0}};
-    const NtTcOpts o2{1, 0, 0, 0, Q <= 256 ? post_m_tiles() : 1};
+    const NtTcOpts o2{1};
     return gemm_nt_tc(s2, 1, Q, logits, Q, bp2, nullptr, 0, nullptr, 0, 0, 0, B, T, st, nullptr, nullptr, nullptr, 0, 0,
                       nullptr, &o2);
   }
@@ -822,7 +811,7 @@ WNB_API int wnb_post_bwd(const float* skip, const float* r1, const float* dlogit
     const NtTcSeg s1[1] = {{dlogits, Q, 0, Q, wp2t, S, Q, 0, 0}};
     const NtTcSeg s2[1] = {{dh1, S, 0, S, wp1t, S, S, 0, 0}};
     if (post_split(S)) {
-      const NtTcOpts o{2, 0, 0, 0, post_m_tiles()};
+      const NtTcOpts o{2};
       if ((rc = gemm_nt_tc(s1, 1, S / 2, dh1, S, nullptr, r1, S, nullptr, 0, 0, 0, B, T, st, nullptr, nullptr, nullptr, 0, 0,
                            nullptr, &o)) != WNB_OK)
         return rc;

@@ -9,18 +9,18 @@
 // GEMM runs once after the last block (gemm_nt_tc, K = L*R).  Per block the traffic drops from 814 MB to 177 MB at
 // the bench shape; Z_all (1.4 GB there) is also what the backward needs for the skip-weight gradient.
 //
-// Per 128-sample time tile:
-//   GEMM-1  D1[128 x 128] = [x(t-d) | x(t) | aux(t)] [128 x 160] * W1^T      tcgen05.mma kind::tf32, SS, W1 resident
-//   gate    z = sigmoid(D1[:, :64] + b) * tanh(D1[:, 64:] + b)              TMEM -> registers -> TMEM and -> Z_all
-//   GEMM-2  D2[128 x 64]  = z * W2res^T                                     A operand from TMEM, W2res resident
-//   out     xout = D2 + b2res + x(t)   (x(t) was copied from the A stage into registers when the tile landed, so
-//           the single A stage is released as soon as GEMM-1 has read it and the next tile's TMA load overlaps the
-//           gate / GEMM-2 / epilogue of this one)
-// Roles (352 threads): warp 0 TMA producer (dynamic tile scheduler), warp 1 MMA issuer (GEMM-1 of the next tile and
-// GEMM-2 of this one in whichever order their inputs arrive; D1 is double-buffered), warp 2 loads the weights
-// once, warps 3-10 epilogue (TMEM lane quarter x column half).  fp32 storage, tf32 multiplies, fp32 accumulate.
+// Per 64-sample time tile (one consumer warpgroup, accumulators in registers):
+//   GEMM-1  D1[64 x 128] = [x(t-d) | x(t) | aux(t)] [64 x 160] * W1^T      wgmma m64n128k8 tf32, both operands from
+//                                                                          shared memory, W1 resident
+//   gate    z = sigmoid(D1[:, :64] + b) * tanh(D1[:, 64:] + b)              registers -> swizzled staging tile -> Z_all
+//   GEMM-2  D2[64 x 64]   = z * W2res^T                                     wgmma m64n64k8, A = the z staging tile
+//   out     xout = D2 + b2res + x(t)   (x(t) is copied from the A stage into registers right after GEMM-1, so the A
+//           stage is refilled while the gate / GEMM-2 / epilogue of this tile run)
+// Roles (288 threads): two consumer warpgroups, each with its own A stage and staging tiles, working on alternate
+// tiles (one's GEMMs overlap the other's epilogue); warp 8 = TMA producer (weights once, then the activation tiles
+// of both warpgroups from a dynamic tile scheduler).  fp32 storage, tf32 multiplies, fp32 accumulate.
 //
-// Shared memory: W1 80 KB | W2res 16 KB | A stage 80 KB | staging 8 x 4 KB.   TMEM: D1 2 x 128 | z 64 | D2 64 columns.
+// Shared memory: W1 80 KB | W2res 16 KB | per warpgroup: A stage 40 KB, staging 16 KB.
 #include <cuda.h>
 
 #include <cstdio>
@@ -32,31 +32,28 @@
 namespace wnb {
 namespace tcz {
 
-constexpr int kTM = 128;
+constexpr int kTM = 64;
 constexpr int kR = 64;
 constexpr int kAp = 32;
 constexpr int kK1 = 2 * kR + kAp;        // 160
-constexpr int kSubBytes = kTM * 32 * 4;  // one [128 x 32 fp32] swizzled sub-tile
+constexpr int kSubBytes = kTM * 32 * 4;  // one [64 x 32 fp32] swizzled sub-tile
 constexpr int kNSubA = kK1 / 32;         // 5
-constexpr int kW2SubBytes = 64 * 32 * 4;
-constexpr int kStgBytes = 32 * 32 * 4;
-constexpr int kEpiWarps = 8;
-constexpr int kEpiThreads = 32 * kEpiWarps;
+constexpr int kW1SubBytes = 2 * kR * 32 * 4;   // [128 x 32]
+constexpr int kW2SubBytes = kR * 32 * 4;       // [64 x 32]
+constexpr int kNWG = 2;
 constexpr int kOffW1 = 0;
-constexpr int kOffW2 = kOffW1 + kNSubA * kSubBytes;
+constexpr int kOffW2 = kOffW1 + kNSubA * kW1SubBytes;
 constexpr int kOffA = kOffW2 + 2 * kW2SubBytes;
-constexpr int kOffStg = kOffA + kNSubA * kSubBytes;
-constexpr int kOffBar = kOffStg + kEpiWarps * kStgBytes;
+constexpr int kOffStg = kOffA + kNWG * kNSubA * kSubBytes;
+constexpr int kOffBar = kOffStg + kNWG * 2 * kSubBytes;
 constexpr int kSmemBytes = kOffBar + 256 + 1024;
-constexpr int kThreadsZ = 32 * (3 + kEpiWarps);
-constexpr uint32_t kColD1 = 0 /* two buffers of 128 */, kColZ = 256, kColD2 = 320;
+constexpr int kThreadsZ = 128 * kNWG + 32;
 
 struct alignas(64) Maps {
   CUtensorMap x, haux, w1, w2, xout, z;
 };
 
-enum { B_W = 0, B_AFULL, B_AEMPTY, B_D1F0, B_D1F1, B_D1E0, B_D1E1, B_ZF, B_D2F, B_D2E, B_TILE0, B_TILE1, B_COUNT };
-static_assert(8 * B_COUNT + 16 <= 256, "barrier block");
+enum { B_W = 0, B_AFULL0, B_AEMPTY0 = B_AFULL0 + kNWG, B_COUNT = B_AEMPTY0 + kNWG };
 
 // dynamic tile scheduler: `sched` = {next tile, CTAs done}, two device words owned by the launching (device, stream)
 // (common.cuh sched_counters): launches on different streams never share them.
@@ -67,8 +64,7 @@ resblock_fwd_z_kernel(const __grid_constant__ Maps maps, const float* __restrict
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBar);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + kOffBar + 8 * B_COUNT);
-  volatile int* tile_ring = reinterpret_cast<volatile int*>(smem + kOffBar + 8 * B_COUNT + 8);  // 2 entries
+  volatile int* tile_slot = reinterpret_cast<volatile int*>(smem + kOffBar + 8 * B_COUNT);  // one per warpgroup
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_b = (T + kTM - 1) / kTM;
@@ -76,252 +72,346 @@ resblock_fwd_z_kernel(const __grid_constant__ Maps maps, const float* __restrict
 
   if (threadIdx.x == 0) {
     ptx::mbar_init(&bars[B_W], 1);
-    ptx::mbar_init(&bars[B_AFULL], 1);
-    ptx::mbar_init(&bars[B_AEMPTY], kEpiThreads + 1);   // every epilogue thread (x copied) + GEMM-1 commit
-    ptx::mbar_init(&bars[B_D1F0], 1); ptx::mbar_init(&bars[B_D1F1], 1);
-    ptx::mbar_init(&bars[B_D1E0], kEpiThreads); ptx::mbar_init(&bars[B_D1E1], kEpiThreads);
-    ptx::mbar_init(&bars[B_ZF], kEpiThreads);
-    ptx::mbar_init(&bars[B_D2F], 1);
-    ptx::mbar_init(&bars[B_D2E], kEpiThreads);
-    ptx::mbar_init(&bars[B_TILE0], 1);
-    ptx::mbar_init(&bars[B_TILE1], 1);
+    for (int g = 0; g < kNWG; g++) {
+      ptx::mbar_init(&bars[B_AFULL0 + g], 1);
+      ptx::mbar_init(&bars[B_AEMPTY0 + g], 128);
+    }
     ptx::fence_barrier_init();
   }
-  if (warp == 1) ptx::tmem_alloc<512>(tmem_slot);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  ptx::tmem_base_must_be_zero(*tmem_slot);
-  constexpr uint32_t tmem = 0;
   // programmatic dependent launch: the set-up above overlapped the previous kernel's tail; from here on this
   // kernel reads / writes memory that kernel may have produced
   ptx::pdl_launch_dependents();
   ptx::pdl_wait();
 
-  if (warp == 0) {
-    // =============================== TMA producer: activation tiles ===============================
+  if (warp == 4 * kNWG) {
+    // =============================== TMA producer ===============================
     if (ptx::elect_one()) {
       ptx::prefetch_tmap(&maps.x); ptx::prefetch_tmap(&maps.haux);
-      // rev: time tiles from the end of the tensor backwards -- a block whose producer ran front to back finds the rows
-      // that block wrote LAST still in L2 (stack.cu alternates the direction from block to block)
-      int tile = rev ? ntiles - 1 - (int)blockIdx.x : (int)blockIdx.x;
-      for (uint32_t it = 0;; it++) {
-        tile_ring[it & 1] = tile;                  // publish the tile (or the stop mark) to the other roles
-        ptx::mbar_arrive(&bars[B_TILE0 + (it & 1)]);
-        if (tile < 0) break;
-        const int b = tile / tiles_per_b, t0 = (tile - b * tiles_per_b) * kTM;
-        ptx::mbar_wait(&bars[B_AEMPTY], (it & 1) ^ 1);
-        ptx::mbar_arrive_expect_tx(&bars[B_AFULL], kNSubA * kSubBytes);
-        unsigned char* sA = smem + kOffA;
-        ptx::tma_load_3d(sA + 0 * kSubBytes, &maps.x, &bars[B_AFULL], 0, t0 - d, b);
-        ptx::tma_load_3d(sA + 1 * kSubBytes, &maps.x, &bars[B_AFULL], 32, t0 - d, b);
-        ptx::tma_load_3d(sA + 2 * kSubBytes, &maps.x, &bars[B_AFULL], 0, t0, b);
-        ptx::tma_load_3d(sA + 3 * kSubBytes, &maps.x, &bars[B_AFULL], 32, t0, b);
-        ptx::tma_load_3d(sA + 4 * kSubBytes, &maps.haux, &bars[B_AFULL], 0, t0, b);
-        tile = (int)(atomicAdd(&sched[0], 1u) + gridDim.x);
-        if (tile >= ntiles) tile = -1;
-        else if (rev) tile = ntiles - 1 - tile;
-        if (tile >= 0) {
-          // there is room for only one A stage, so the next tile cannot be loaded yet -- but it can be pulled into
-          // L2 now, which turns the exposed DRAM latency of its load into an L2 hit
-          const int nb = tile / tiles_per_b, nt0 = (tile - nb * tiles_per_b) * kTM;
-          ptx::tma_prefetch_3d(&maps.x, 0, nt0, nb);
-          ptx::tma_prefetch_3d(&maps.x, 32, nt0, nb);
-          ptx::tma_prefetch_3d(&maps.haux, 0, nt0, nb);
-          if (d >= kTM) {   // (for d < 128 most of x(t-d) is the previous tile of the same row: already in L2)
-            ptx::tma_prefetch_3d(&maps.x, 0, nt0 - d, nb);
-            ptx::tma_prefetch_3d(&maps.x, 32, nt0 - d, nb);
-          }
-        }
-      }
-    }
-  } else if (warp == 2) {
-    // =============================== weights: loaded once, resident ===============================
-    if (ptx::elect_one()) {
       ptx::prefetch_tmap(&maps.w1); ptx::prefetch_tmap(&maps.w2);
-      ptx::mbar_arrive_expect_tx(&bars[B_W], kNSubA * kSubBytes + (has_xout ? 2 * kW2SubBytes : 0));
-      for (int j = 0; j < kNSubA; j++) ptx::tma_load_2d(smem + kOffW1 + j * kSubBytes, &maps.w1, &bars[B_W], j * 32, 0);
+      ptx::mbar_arrive_expect_tx(&bars[B_W], kNSubA * kW1SubBytes + (has_xout ? 2 * kW2SubBytes : 0));
+      for (int j = 0; j < kNSubA; j++) ptx::tma_load_2d(smem + kOffW1 + j * kW1SubBytes, &maps.w1, &bars[B_W], j * 32, 0);
       if (has_xout) {
         ptx::tma_load_2d(smem + kOffW2, &maps.w2, &bars[B_W], 0, 0);
         ptx::tma_load_2d(smem + kOffW2 + kW2SubBytes, &maps.w2, &bars[B_W], 32, 0);
       }
-    }
-  } else if (warp == 1) {
-    // =============================== MMA issuer ===============================
-    if (ptx::elect_one()) {
-      constexpr uint32_t idesc1 = ptx::idesc_tf32(128, 128);
-      constexpr uint32_t idesc2 = ptx::idesc_tf32(128, 64);
-      const uint32_t a_lo0 = ptx::desc_lo(ptx::smem_u32(smem + kOffA), 16);
-      const uint32_t w1_lo0 = ptx::desc_lo(ptx::smem_u32(smem + kOffW1), 16);
-      const uint32_t w2_lo0 = ptx::desc_lo(ptx::smem_u32(smem + kOffW2), 16);
-      constexpr uint32_t hi = ptx::kDescHiKSw128;
-      ptx::mbar_wait(&bars[B_W], 0);
-      // GEMM-1 of tile it+1 (into the other D1 buffer) and GEMM-2 of tile it are issued in whichever order their
-      // inputs become ready -- the next A stage landing, or the gate of tile it finishing -- so the tensor pipe
-      // works on the next tile while the epilogue warps are still in the gate of this one.
-      auto gemm1 = [&](uint32_t it) {
-        ptx::tc_fence_after();
-#pragma unroll
-        for (int j = 0; j < kNSubA; j++)
-#pragma unroll
-          for (int k = 0; k < 4; k++)
-            ptx::mma_tf32_ss(tmem + kColD1 + (it & 1) * 128, ptx::desc64(a_lo0 + j * (kSubBytes >> 4) + 2 * k, hi),
-                             ptx::desc64(w1_lo0 + j * (kSubBytes >> 4) + 2 * k, hi), idesc1, (j | k) != 0);
-        ptx::tc_commit(&bars[B_D1F0 + (it & 1)]);
-        ptx::tc_commit(&bars[B_AEMPTY]);   // GEMM-1 has read the A stage
-      };
-      ptx::mbar_wait(&bars[B_TILE0], 0);
-      if (tile_ring[0] >= 0) {
-        ptx::mbar_wait(&bars[B_AFULL], 0);
-        gemm1(0);
-        for (uint32_t it = 0;; it++) {
-          const uint32_t nx = it + 1;
-          ptx::mbar_wait(&bars[B_TILE0 + (nx & 1)], (nx >> 1) & 1);
-          bool need1 = tile_ring[nx & 1] >= 0;
-          const bool has_next = need1;
-          bool need2 = has_xout != 0;
-          ptx::SpinGuard guard;
-          while (need1 || need2) {
-            if (need2 && ptx::mbar_try_wait(&bars[B_ZF], it & 1) && ptx::mbar_try_wait(&bars[B_D2E], (it & 1) ^ 1)) {
-              ptx::tc_fence_after();
-#pragma unroll
-              for (int kk = 0; kk < 2; kk++)
-#pragma unroll
-                for (int k = 0; k < 4; k++)
-                  ptx::mma_tf32_ts(tmem + kColD2, tmem + kColZ + kk * 32 + k * 8,
-                                   ptx::desc64(w2_lo0 + kk * (kW2SubBytes >> 4) + 2 * k, hi), idesc2, (kk | k) != 0);
-              ptx::tc_commit(&bars[B_D2F]);
-              need2 = false;
-              continue;
-            }
-            // D1 buffer nx & 1 was last read by the gate of tile nx - 2
-            if (need1 && ptx::mbar_try_wait(&bars[B_AFULL], nx & 1) &&
-                ptx::mbar_try_wait(&bars[B_D1E0 + (nx & 1)], ((nx >> 1) & 1) ^ 1)) {
-              gemm1(nx);
-              need1 = false;
-              continue;
-            }
-            if (guard.expired()) {
-              printf("wnb200: resblock_fwd_z MMA issuer timed out after 20 s (block %d)\n", blockIdx.x);
-              __trap();
-            }
-          }
-          if (!has_next) break;
+      // rev: time tiles from the end of the tensor backwards -- a block whose producer ran front to back finds the rows
+      // that block wrote LAST still in L2 (stack.cu alternates the direction from block to block)
+      int tile = rev ? ntiles - 1 - (int)blockIdx.x : (int)blockIdx.x;
+      if ((int)blockIdx.x >= ntiles) tile = -1;
+      int stops = 0;
+      for (uint32_t it = 0; stops < kNWG; it++) {
+        const int g = it % kNWG;
+        const uint32_t use = it / kNWG;
+        ptx::mbar_wait(&bars[B_AEMPTY0 + g], (use & 1) ^ 1);
+        tile_slot[g] = tile;                  // publish the tile (or the stop mark) to warpgroup g
+        if (tile < 0) {
+          ptx::mbar_arrive(&bars[B_AFULL0 + g]);
+          stops++;
+          continue;
         }
+        const int b = tile / tiles_per_b, t0 = (tile - b * tiles_per_b) * kTM;
+        ptx::mbar_arrive_expect_tx(&bars[B_AFULL0 + g], kNSubA * kSubBytes);
+        unsigned char* sA = smem + kOffA + g * kNSubA * kSubBytes;
+        ptx::tma_load_3d(sA + 0 * kSubBytes, &maps.x, &bars[B_AFULL0 + g], 0, t0 - d, b);
+        ptx::tma_load_3d(sA + 1 * kSubBytes, &maps.x, &bars[B_AFULL0 + g], 32, t0 - d, b);
+        ptx::tma_load_3d(sA + 2 * kSubBytes, &maps.x, &bars[B_AFULL0 + g], 0, t0, b);
+        ptx::tma_load_3d(sA + 3 * kSubBytes, &maps.x, &bars[B_AFULL0 + g], 32, t0, b);
+        ptx::tma_load_3d(sA + 4 * kSubBytes, &maps.haux, &bars[B_AFULL0 + g], 0, t0, b);
+        tile = (int)(atomicAdd(&sched[0], 1u) + gridDim.x);
+        if (tile >= ntiles) tile = -1;
+        else if (rev) tile = ntiles - 1 - tile;
       }
     }
   } else {
-    // =============================== epilogue warps (3..10) ===============================
-    const int q = warp & 3;                         // TMEM lane quarter this warp may access
-    const int hf = (warp - 3) >> 2;                 // which 32 of the 64 channels
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    const int row = q * 32 + lane;                  // time row inside the tile
-    unsigned char* sb = smem + kOffStg + (warp - 3) * kStgBytes;
-    const uint32_t sb_row = ptx::smem_u32(sb + lane * 128);
-    const unsigned char* sX = smem + kOffA + (2 + hf) * kSubBytes;  // x(t) sub-tile holding this warp's channels
-    const float4* b1v = reinterpret_cast<const float4*>(b1);
-    const float4* b2v = reinterpret_cast<const float4*>(b2 + hf * 32);
-    for (uint32_t it = 0;; it++) {
-      ptx::mbar_wait(&bars[B_TILE0 + (it & 1)], (it >> 1) & 1);
-      const int tile = tile_ring[it & 1];
+    // =============================== consumer warpgroup g ===============================
+    const int g = warp >> 2, wq = warp & 3, tid = threadIdx.x & 127;
+    const int r0 = 16 * wq + (lane >> 2), cq = 2 * (lane & 3);   // fragment rows r0, r0 + 8; columns 8 j + cq (+1)
+    unsigned char* sA = smem + kOffA + g * kNSubA * kSubBytes;
+    unsigned char* stg = smem + kOffStg + g * 2 * kSubBytes;       // [64 x 64]: z, then xout, as two swizzled sub-tiles
+    const uint32_t a_u32 = ptx::smem_u32(sA), w1_u32 = ptx::smem_u32(smem + kOffW1);
+    const uint32_t w2_u32 = ptx::smem_u32(smem + kOffW2), stg_u32 = ptx::smem_u32(stg);
+    const int bar_id = 1 + g;
+    ptx::mbar_wait(&bars[B_W], 0);
+    for (uint32_t j = 0;; j++) {
+      ptx::mbar_wait(&bars[B_AFULL0 + g], j & 1);
+      const int tile = tile_slot[g];
       if (tile < 0) break;
       const int b = tile / tiles_per_b, t0 = (tile - b * tiles_per_b) * kTM;
-      // ---- x(t) for the residual: A stage -> registers, then the stage can be refilled ----
+      // ---- GEMM-1 ----
+      float d1[64];
+#pragma unroll
+      for (int i = 0; i < 64; i++) d1[i] = 0.f;
+      ptx::wg_fence();
+#pragma unroll
+      for (int s = 0; s < kNSubA; s++)
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+          ptx::wgmma_ss<128>(d1, ptx::gmma_desc_k_sw128(a_u32 + s * kSubBytes + 32 * k),
+                             ptx::gmma_desc_k_sw128(w1_u32 + s * kW1SubBytes + 32 * k), 1);
+      ptx::wg_commit();
+      ptx::wg_wait<0>();
+      ptx::wg_touch(d1);
+      // ---- x(t) for the residual: A stage -> registers (fragment positions), then the stage can be refilled ----
       float xr[32];
-      // (the wait also orders this thread's AEMPTY arrival after the previous phase of that barrier completed)
-      ptx::mbar_wait(&bars[B_AFULL], it & 1);
       if (has_xout) {
-        const float4* xp = reinterpret_cast<const float4*>(sX + row * 128);
 #pragma unroll
-        for (int j = 0; j < 8; j++) {
-          const float4 xv = xp[j ^ (row & 7)];
-          xr[4 * j] = xv.x; xr[4 * j + 1] = xv.y; xr[4 * j + 2] = xv.z; xr[4 * j + 3] = xv.w;
+        for (int i = 0; i < 32; i += 2) {
+          const int r = r0 + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + cq;
+          const float2 v = *reinterpret_cast<const float2*>(sA + (2 + (c >> 5)) * kSubBytes + ptx::sw128_off(r, c & 31));
+          xr[i] = v.x; xr[i + 1] = v.y;
         }
       }
-      ptx::mbar_arrive(&bars[B_AEMPTY]);
-      // ---- gate: z = sigmoid(a) * tanh(g), 16 channels at a time, TMEM -> regs -> TMEM (+ kept for the store) ----
-      ptx::mbar_wait(&bars[B_D1F0 + (it & 1)], (it >> 1) & 1);
-      ptx::tc_fence_after();
-      const uint32_t d1col = kColD1 + (it & 1) * 128;
-      float zr[32];
+      ptx::mbar_arrive(&bars[B_AEMPTY0 + g]);
+      // ---- gate: z = sigmoid(a) * tanh(g) on the fragments (column c and 64 + c are registers i and i + 32) ----
+      float z[32];
 #pragma unroll
-      for (int gg = 0; gg < 2; gg++) {
-        const int g = hf * 2 + gg;
-        float a[16], t[16], z[16];
-        ptx::tmem_ld16(tmem + lane_base + d1col + g * 16, a);
-        ptx::tmem_ld16(tmem + lane_base + d1col + 64 + g * 16, t);
-        float4 ba[4], bt[4];
-#pragma unroll
-        for (int i = 0; i < 4; i++) { ba[i] = __ldg(b1v + g * 4 + i); bt[i] = __ldg(b1v + 16 + g * 4 + i); }
-        ptx::tc_wait_ld();
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-          const float bav[4] = {ba[i].x, ba[i].y, ba[i].z, ba[i].w}, btv[4] = {bt[i].x, bt[i].y, bt[i].z, bt[i].w};
-#pragma unroll
-          for (int k = 0; k < 4; k++) {
-            const float av = a[4 * i + k] + bav[k], tv = t[4 * i + k] + btv[k];
-            z[4 * i + k] = (0.5f * ptx::tanh_approx(0.5f * av) + 0.5f) * ptx::tanh_approx(tv);
-            zr[gg * 16 + 4 * i + k] = z[4 * i + k];
-          }
-        }
-        if (has_xout) ptx::tmem_st16(tmem + lane_base + kColZ + g * 16, z);
+      for (int i = 0; i < 32; i++) {
+        const int c = 8 * (i >> 2) + cq + (i & 1);
+        const float av = d1[i] + __ldg(b1 + c), tv = d1[i + 32] + __ldg(b1 + kR + c);
+        z[i] = (0.5f * ptx::tanh_approx(0.5f * av) + 0.5f) * ptx::tanh_approx(tv);
       }
-      if (has_xout) ptx::tc_wait_st();
-      ptx::tc_fence_before();
-      ptx::mbar_arrive(&bars[B_ZF]);
-      ptx::mbar_arrive(&bars[B_D1E0 + (it & 1)]);
-      // ---- z -> Z_all slice ----
-      if (lane == 0) ptx::bulk_wait_read<0>();
-      __syncwarp();
+      // ---- z -> staging (the previous tile's xout store must have read it) -> Z_all slice ----
+      if (tid == 0) ptx::bulk_wait_read<0>();
+      ptx::named_bar(bar_id, 128);
 #pragma unroll
-      for (int j = 0; j < 8; j++)
-        ptx::st_shared_v4(sb_row + ((j ^ (lane & 7)) << 4), zr[4 * j], zr[4 * j + 1], zr[4 * j + 2], zr[4 * j + 3]);
+      for (int i = 0; i < 32; i += 2) {
+        const int r = r0 + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + cq;
+        *reinterpret_cast<float2*>(stg + (c >> 5) * kSubBytes + ptx::sw128_off(r, c & 31)) = make_float2(z[i], z[i + 1]);
+      }
       ptx::fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        ptx::tma_store_3d(&maps.z, sb, zcol0 + hf * 32, t0 + q * 32, b);
+      ptx::named_bar(bar_id, 128);
+      if (tid == 0) {
+        ptx::tma_store_3d(&maps.z, stg, zcol0, t0, b);
+        ptx::tma_store_3d(&maps.z, stg + kSubBytes, zcol0 + 32, t0, b);
         ptx::bulk_commit();
       }
       if (!has_xout) continue;
-      // ---- residual output ----
-      float4 bv[8];
+      // ---- GEMM-2 from the z staging tile ----
+      float d2[32];
 #pragma unroll
-      for (int j = 0; j < 8; j++) bv[j] = __ldg(b2v + j);
-      ptx::mbar_wait(&bars[B_D2F], it & 1);
-      ptx::tc_fence_after();
-      float v[32];
-      {
-        float lo[16], hi[16];
-        ptx::tmem_ld16(tmem + lane_base + kColD2 + hf * 32, lo);
-        ptx::tmem_ld16(tmem + lane_base + kColD2 + hf * 32 + 16, hi);
-        ptx::tc_wait_ld();
+      for (int i = 0; i < 32; i++) d2[i] = 0.f;
+      ptx::wg_fence();
 #pragma unroll
-        for (int i = 0; i < 16; i++) { v[i] = lo[i]; v[16 + i] = hi[i]; }
+      for (int kk = 0; kk < 2; kk++)
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+          ptx::wgmma_ss<64>(d2, ptx::gmma_desc_k_sw128(stg_u32 + kk * kSubBytes + 32 * k),
+                            ptx::gmma_desc_k_sw128(w2_u32 + kk * kW2SubBytes + 32 * k), 1);
+      ptx::wg_commit();
+      ptx::wg_wait<0>();
+      ptx::wg_touch(d2);
+      // ---- residual output: xout = D2 + b2 + x(t), through the same staging tile once the z store has read it ----
+      if (tid == 0) ptx::bulk_wait_read<0>();
+      ptx::named_bar(bar_id, 128);
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int r = r0 + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + cq;
+        const float2 bv = __ldg(reinterpret_cast<const float2*>(b2 + c));
+        *reinterpret_cast<float2*>(stg + (c >> 5) * kSubBytes + ptx::sw128_off(r, c & 31)) =
+            make_float2(d2[i] + bv.x + xr[i], d2[i + 1] + bv.y + xr[i + 1]);
       }
-      ptx::tc_fence_before();
-      ptx::mbar_arrive(&bars[B_D2E]);
-#pragma unroll
-      for (int j = 0; j < 8; j++) {
-        v[4 * j] += bv[j].x + xr[4 * j]; v[4 * j + 1] += bv[j].y + xr[4 * j + 1];
-        v[4 * j + 2] += bv[j].z + xr[4 * j + 2]; v[4 * j + 3] += bv[j].w + xr[4 * j + 3];
-      }
-      if (lane == 0) ptx::bulk_wait_read<0>();
-      __syncwarp();
-#pragma unroll
-      for (int j = 0; j < 8; j++)
-        ptx::st_shared_v4(sb_row + ((j ^ (lane & 7)) << 4), v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
       ptx::fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        ptx::tma_store_3d(&maps.xout, sb, hf * 32, t0 + q * 32, b);
+      ptx::named_bar(bar_id, 128);
+      if (tid == 0) {
+        ptx::tma_store_3d(&maps.xout, stg, 0, t0, b);
+        ptx::tma_store_3d(&maps.xout, stg + kSubBytes, 32, t0, b);
         ptx::bulk_commit();
       }
     }
-    if (lane == 0) ptx::bulk_wait<0>();
+    if (tid == 0) ptx::bulk_wait<0>();
   }
-  ptx::tc_fence_before();
   __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc<512>(tmem);
+  if (threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(&sched[1], 1u) == gridDim.x - 1) {  // last CTA out: re-arm the scheduler for the next launch
+      sched[0] = 0;
+      sched[1] = 0;
+    }
+  }
+}
+
+
+// ---------------------------------------------------------------------------------------------------------------
+// Per-block form WITH skip accumulation (wnb_resblock_fwd, reference wavenet.py:525-536 one block at a time):
+// GEMM-1 + gate as above, then the W2 row chunks -- [64 x 64] each: the residual chunk (unless this is the last
+// block) and the S/64 skip chunks -- stream from L2 through a TMA ring and each is one wgmma m64n64 from the z staging
+// tile: xout = D + b2 + x(t) (TMA store), skip += D + b2 (TMA reduce-add; TMA store when skip_init).  Every skip
+// element receives exactly one add per launch.  One consumer warpgroup + one producer warp (W2 does not fit resident
+// next to W1).  Shared memory: W1 80 KB | A stage 40 KB | z staging 16 KB | 2 output staging 32 KB | W2 ring 32 KB.
+namespace tcs {
+constexpr int kSNSlot = 2;
+constexpr int kSChunkBytes = 2 * kW2SubBytes;                 // [64 rows x 64] as two [64 x 32] sub-tiles
+constexpr int kSOffW1 = 0;
+constexpr int kSOffA = kSOffW1 + kNSubA * kW1SubBytes;
+constexpr int kSOffZ = kSOffA + kNSubA * kSubBytes;
+constexpr int kSOffOut = kSOffZ + 2 * kSubBytes;
+constexpr int kSOffRing = kSOffOut + 2 * 2 * kSubBytes;
+constexpr int kSOffBar = kSOffRing + kSNSlot * kSChunkBytes;
+constexpr int kSSmemBytes = kSOffBar + 256 + 1024;
+constexpr int kSThreads = 128 + 32;
+struct alignas(64) Maps { CUtensorMap x, haux, w1, w2, xout, skip; };
+enum { SB_W = 0, SB_AFULL, SB_AEMPTY, SB_WF0, SB_WE0 = SB_WF0 + kSNSlot, SB_COUNT = SB_WE0 + kSNSlot };
+}  // namespace tcs
+
+__global__ void __launch_bounds__(tcs::kSThreads, 1)
+resblock_fwd_skip_kernel(const __grid_constant__ tcs::Maps maps, const float* __restrict__ b1, const float* __restrict__ b2,
+                         int B, int T, int S, int d, int has_xout, int skip_init, unsigned int* __restrict__ sched) {
+  using namespace tcs;
+  extern __shared__ unsigned char smem_raw[];
+  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kSOffBar);
+  volatile int* tile_slot = reinterpret_cast<volatile int*>(smem + kSOffBar + 8 * SB_COUNT);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tiles_per_b = (T + kTM - 1) / kTM;
+  const int ntiles = B * tiles_per_b;
+  const int nchunks = (has_xout ? 1 : 0) + S / 64;
+  const int row0 = has_xout ? 0 : kR;      // first W2 row of chunk 0
+
+  if (threadIdx.x == 0) {
+    ptx::mbar_init(&bars[SB_W], 1);
+    ptx::mbar_init(&bars[SB_AFULL], 1);
+    ptx::mbar_init(&bars[SB_AEMPTY], 128);
+    for (int i = 0; i < kSNSlot; i++) { ptx::mbar_init(&bars[SB_WF0 + i], 1); ptx::mbar_init(&bars[SB_WE0 + i], 128); }
+    ptx::fence_barrier_init();
+  }
+  __syncthreads();
+  ptx::pdl_launch_dependents();
+  ptx::pdl_wait();
+
+  if (warp == 4) {
+    // =============================== TMA producer: W1 once, then per tile the A stage and the W2 chunks ===============
+    if (ptx::elect_one()) {
+      ptx::prefetch_tmap(&maps.x); ptx::prefetch_tmap(&maps.haux); ptx::prefetch_tmap(&maps.w1); ptx::prefetch_tmap(&maps.w2);
+      ptx::mbar_arrive_expect_tx(&bars[SB_W], kNSubA * kW1SubBytes);
+      for (int j = 0; j < kNSubA; j++) ptx::tma_load_2d(smem + kSOffW1 + j * kW1SubBytes, &maps.w1, &bars[SB_W], j * 32, 0);
+      int tile = (int)blockIdx.x < ntiles ? (int)blockIdx.x : -1;
+      uint32_t slot = 0, wph = 0;
+      for (uint32_t it = 0;; it++) {
+        ptx::mbar_wait(&bars[SB_AEMPTY], (it & 1) ^ 1);
+        tile_slot[0] = tile;
+        if (tile < 0) { ptx::mbar_arrive(&bars[SB_AFULL]); break; }
+        const int b = tile / tiles_per_b, t0 = (tile - b * tiles_per_b) * kTM;
+        ptx::mbar_arrive_expect_tx(&bars[SB_AFULL], kNSubA * kSubBytes);
+        unsigned char* sA = smem + kSOffA;
+        ptx::tma_load_3d(sA + 0 * kSubBytes, &maps.x, &bars[SB_AFULL], 0, t0 - d, b);
+        ptx::tma_load_3d(sA + 1 * kSubBytes, &maps.x, &bars[SB_AFULL], 32, t0 - d, b);
+        ptx::tma_load_3d(sA + 2 * kSubBytes, &maps.x, &bars[SB_AFULL], 0, t0, b);
+        ptx::tma_load_3d(sA + 3 * kSubBytes, &maps.x, &bars[SB_AFULL], 32, t0, b);
+        ptx::tma_load_3d(sA + 4 * kSubBytes, &maps.haux, &bars[SB_AFULL], 0, t0, b);
+        for (int c = 0; c < nchunks; c++) {
+          ptx::mbar_wait(&bars[SB_WE0 + slot], wph ^ 1);
+          ptx::mbar_arrive_expect_tx(&bars[SB_WF0 + slot], kSChunkBytes);
+          unsigned char* dst = smem + kSOffRing + slot * kSChunkBytes;
+          ptx::tma_load_2d(dst, &maps.w2, &bars[SB_WF0 + slot], 0, row0 + c * 64);
+          ptx::tma_load_2d(dst + kW2SubBytes, &maps.w2, &bars[SB_WF0 + slot], 32, row0 + c * 64);
+          if (++slot == kSNSlot) { slot = 0; wph ^= 1; }
+        }
+        tile = (int)(atomicAdd(&sched[0], 1u) + gridDim.x);
+        if (tile >= ntiles) tile = -1;
+      }
+    }
+  } else {
+    // =============================== consumer warpgroup ===============================
+    const int wq = warp & 3, tid = threadIdx.x;
+    const int r0 = 16 * wq + (lane >> 2), cq = 2 * (lane & 3);
+    unsigned char* sA = smem + kSOffA;
+    unsigned char* zst = smem + kSOffZ;
+    const uint32_t a_u32 = ptx::smem_u32(sA), w1_u32 = ptx::smem_u32(smem + kSOffW1), z_u32 = ptx::smem_u32(zst);
+    uint32_t slot = 0, wph = 0, nout = 0;
+    ptx::mbar_wait(&bars[SB_W], 0);
+    for (uint32_t j = 0;; j++) {
+      ptx::mbar_wait(&bars[SB_AFULL], j & 1);
+      const int tile = tile_slot[0];
+      if (tile < 0) break;
+      const int b = tile / tiles_per_b, t0 = (tile - b * tiles_per_b) * kTM;
+      float d1[64];
+#pragma unroll
+      for (int i = 0; i < 64; i++) d1[i] = 0.f;
+      ptx::wg_fence();
+#pragma unroll
+      for (int s = 0; s < kNSubA; s++)
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+          ptx::wgmma_ss<128>(d1, ptx::gmma_desc_k_sw128(a_u32 + s * kSubBytes + 32 * k),
+                             ptx::gmma_desc_k_sw128(w1_u32 + s * kW1SubBytes + 32 * k), 1);
+      ptx::wg_commit();
+      ptx::wg_wait<0>();
+      ptx::wg_touch(d1);
+      float xr[32];
+      if (has_xout) {
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+          const int r = r0 + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + cq;
+          const float2 v = *reinterpret_cast<const float2*>(sA + (2 + (c >> 5)) * kSubBytes + ptx::sw128_off(r, c & 31));
+          xr[i] = v.x; xr[i + 1] = v.y;
+        }
+      }
+      ptx::mbar_arrive(&bars[SB_AEMPTY]);
+      // ---- gate -> z staging tile (the A operand of every W2 chunk; the previous tile's MMAs have all completed) ----
+      ptx::named_bar(1, 128);
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int r = r0 + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + cq;
+        float zz[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          const float av = d1[i + h] + __ldg(b1 + c + h), tv = d1[i + h + 32] + __ldg(b1 + kR + c + h);
+          zz[h] = (0.5f * ptx::tanh_approx(0.5f * av) + 0.5f) * ptx::tanh_approx(tv);
+        }
+        *reinterpret_cast<float2*>(zst + (c >> 5) * kSubBytes + ptx::sw128_off(r, c & 31)) = make_float2(zz[0], zz[1]);
+      }
+      ptx::fence_proxy_async();
+      ptx::named_bar(1, 128);
+      // ---- W2 chunks: residual (unless last block), then skip ----
+      for (int c = 0; c < nchunks; c++) {
+        const bool is_res = has_xout && c == 0;
+        const int col0 = is_res ? 0 : (c - (has_xout ? 1 : 0)) * 64;   // channel offset inside xout / skip
+        const float* bias = b2 + (is_res ? 0 : kR + col0);
+        ptx::mbar_wait(&bars[SB_WF0 + slot], wph);
+        const uint32_t w_u32 = ptx::smem_u32(smem + kSOffRing + slot * kSChunkBytes);
+        float d2[32];
+#pragma unroll
+        for (int i = 0; i < 32; i++) d2[i] = 0.f;
+        ptx::wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < 2; kk++)
+#pragma unroll
+          for (int k = 0; k < 4; k++)
+            ptx::wgmma_ss<64>(d2, ptx::gmma_desc_k_sw128(z_u32 + kk * kSubBytes + 32 * k),
+                              ptx::gmma_desc_k_sw128(w_u32 + kk * kW2SubBytes + 32 * k), 1);
+        ptx::wg_commit();
+        ptx::wg_wait<0>();
+        ptx::wg_touch(d2);
+        ptx::mbar_arrive(&bars[SB_WE0 + slot]);
+        if (++slot == kSNSlot) { slot = 0; wph ^= 1; }
+        unsigned char* ost = smem + kSOffOut + (nout & 1) * 2 * kSubBytes;
+        if (tid == 0) ptx::bulk_wait_read<1>();   // the store that last read this staging tile has drained
+        ptx::named_bar(1, 128);
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+          const int r = r0 + 8 * ((i >> 1) & 1), cc = 8 * (i >> 2) + cq;
+          const float2 bv = __ldg(reinterpret_cast<const float2*>(bias + cc));
+          float v0 = d2[i] + bv.x, v1 = d2[i + 1] + bv.y;
+          if (is_res) { v0 += xr[i]; v1 += xr[i + 1]; }
+          *reinterpret_cast<float2*>(ost + (cc >> 5) * kSubBytes + ptx::sw128_off(r, cc & 31)) = make_float2(v0, v1);
+        }
+        ptx::fence_proxy_async();
+        ptx::named_bar(1, 128);
+        if (tid == 0) {
+          for (int h = 0; h < 2; h++) {
+            if (is_res) ptx::tma_store_3d(&maps.xout, ost + h * kSubBytes, 32 * h, t0, b);
+            else if (skip_init) ptx::tma_store_3d(&maps.skip, ost + h * kSubBytes, col0 + 32 * h, t0, b);
+            else ptx::tma_reduce_add_3d(&maps.skip, ost + h * kSubBytes, col0 + 32 * h, t0, b);
+          }
+          ptx::bulk_commit();
+        }
+        nout++;
+      }
+    }
+    if (tid == 0) ptx::bulk_wait<0>();
+  }
+  __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence();
     if (atomicAdd(&sched[1], 1u) == gridDim.x - 1) {  // last CTA out: re-arm the scheduler for the next launch
@@ -384,9 +474,9 @@ int resblock_fwd_z(const float* xin, const float* haux, const float* w1, const f
     return WNB_ERR_INVALID;
   }
   Maps maps;
-  bool ok = map_act(&maps.x, xin, kR, kR, T, B, 128) && map_act(&maps.haux, haux, kAp, kAp, T, B, 128) &&
-            map_mat(&maps.w1, w1, kK1, 2 * kR, 128) && map_mat(&maps.w2, w2res ? w2res : w1, kR, kR, 64) &&
-            map_act(&maps.xout, xout ? xout : xin, kR, kR, T, B, 32) && map_act(&maps.z, zall, ldz, ldz, T, B, 32);
+  bool ok = map_act(&maps.x, xin, kR, kR, T, B, kTM) && map_act(&maps.haux, haux, kAp, kAp, T, B, kTM) &&
+            map_mat(&maps.w1, w1, kK1, 2 * kR, 2 * kR) && map_mat(&maps.w2, w2res ? w2res : w1, kR, kR, kR) &&
+            map_act(&maps.xout, xout ? xout : xin, kR, kR, T, B, kTM) && map_act(&maps.z, zall, ldz, ldz, T, B, kTM);
   if (!ok) {
     set_error("resblock_fwd_z: cuTensorMapEncodeTiled failed or is unavailable");
     return WNB_ERR_CUDA;
@@ -400,6 +490,39 @@ int resblock_fwd_z(const float* xin, const float* haux, const float* w1, const f
   if (launch_pdl(resblock_fwd_z_kernel, grid, kThreadsZ, kSmemBytes, st, maps, b1, b2res ? b2res : b1, B, T, d,
                  xout ? 1 : 0, zcol0, sched, reverse ? 1 : 0) != cudaSuccess) { /* reported below */ }
   WNB_CHECK_LAUNCH("resblock_fwd_z");
+  return WNB_OK;
+}
+
+bool resblock_fwd_skip_supported(int R, int S, int Ap, int ks) {
+  return R == tcz::kR && ks == 2 && Ap == tcz::kAp && S >= 64 && S % 64 == 0;
+}
+
+// One block in the per-block form: xout (B,T,R) or null (last block), skip (B,T,S) = or += the block's skip output.
+int resblock_fwd_skip(const float* xin, const float* haux, const float* w1, const float* b1, const float* w2,
+                      const float* b2, float* xout, float* skip, int B, int T, int S, int d, int skip_init,
+                      cudaStream_t st) {
+  using namespace tcz;
+  if ((reinterpret_cast<uintptr_t>(b1) | reinterpret_cast<uintptr_t>(b2)) & 15) {
+    set_error("resblock_fwd: b1 / b2 must be 16-byte aligned");
+    return WNB_ERR_INVALID;
+  }
+  tcs::Maps maps;
+  bool ok = map_act(&maps.x, xin, kR, kR, T, B, kTM) && map_act(&maps.haux, haux, kAp, kAp, T, B, kTM) &&
+            map_mat(&maps.w1, w1, kK1, 2 * kR, 2 * kR) && map_mat(&maps.w2, w2, kR, kR + S, kR) &&
+            map_act(&maps.xout, xout ? xout : xin, kR, kR, T, B, kTM) && map_act(&maps.skip, skip, S, S, T, B, kTM);
+  if (!ok) {
+    set_error("resblock_fwd: cuTensorMapEncodeTiled failed or is unavailable");
+    return WNB_ERR_CUDA;
+  }
+  WNB_CUDA(ensure_dynamic_smem(reinterpret_cast<const void*>(resblock_fwd_skip_kernel), tcs::kSSmemBytes));
+  const int sms = device_sms();
+  unsigned int* sched = sched_counters(st);
+  if (!sched) { set_error("resblock_fwd: cannot allocate the scheduler words"); return WNB_ERR_CUDA; }
+  const int ntiles = B * ((T + kTM - 1) / kTM);
+  const int grid = ntiles < sms ? ntiles : sms;
+  if (launch_pdl(resblock_fwd_skip_kernel, grid, tcs::kSThreads, tcs::kSSmemBytes, st, maps, b1, b2, B, T, S, d,
+                 xout ? 1 : 0, skip_init, sched) != cudaSuccess) { /* reported below */ }
+  WNB_CHECK_LAUNCH("resblock_fwd_skip");
   return WNB_OK;
 }
 

@@ -29,25 +29,9 @@ static int pick_block(int total, const int* cands, int n) {
   return 0;
 }
 
-// WNB_STAGE_EPI=1 stages the epilogue operands (gate-backward dz slice, dX residual) through TMA tiles loaded by the producer
-// warp instead of per-lane global row loads.  Built on the ncu finding that the epilogue warps stall on L1TEX, measured
-// on B200 -- and SLOWER: gate backward 59.3 -> 66.2 us, dX 51.6 -> 58.8 us per block (one pipeline stage less and one more
-// serial job for the single producer thread cost more than the row loads).  Off by default; kept as a measured negative.
-static int stage_epi() {
-  static const int on = [] { const char* e = getenv("WNB_STAGE_EPI"); return (e && e[0] == '1') ? 1 : 0; }();
-  return on;
-}
-
-// The gate-backward and dX GEMMs of a block keep their weights (96 / 80 KB) in shared memory for the whole launch instead
-// of streaming them from L2 for every 128-row tile; WNB_NT_WRES=0 restores the streaming ring (A/B runs).
-static int resident_w() {
-  static const int on = [] { const char* e = getenv("WNB_NT_WRES"); return (e && e[0] == '0') ? 0 : 1; }();
-  return on && !stage_epi();
-}
-
 // Consecutive kernels of the block chain walk the time tiles in opposite directions (forward: odd blocks backwards;
 // backward: gate backward front to back, dX back to front), so each starts on the rows its producer wrote last -- still
-// in the 126 MB L2 -- instead of on the ones written a tensor ago.  WNB_ALT_DIR=0: every kernel front to back.
+// in the 50 MB L2 -- instead of on the ones written a tensor ago.  WNB_ALT_DIR=0: every kernel front to back.
 static int alternate_dir() {
   static const int on = [] { const char* e = getenv("WNB_ALT_DIR"); return (e && e[0] == '0') ? 0 : 1; }();
   return on;
@@ -86,10 +70,8 @@ WNB_API int wnb_skip_gemm(const float* zall, const float* wskip, const float* bs
   WNB_REQUIRE(zall && wskip && skip && B > 0 && T > 0 && K % 32 == 0 && S % 32 == 0 && (S <= 256 || S == 512),
               "skip_gemm: bad arguments");
   const NtTcSeg seg[1] = {{zall, K, 0, K, wskip, S, K, 0, 0}};
-  // 256 rows x (<=256 columns) per CTA tile: every Wskip chunk is fetched from L2 once per 256 rows (K = L*R is long,
-  // the GEMM is bound by the L2 -> SM path: DESIGN.md section 3)
-  const int nblk = S > 256 ? S / 256 : 1;
-  const NtTcOpts o{nblk, 0, 0, 0, nt_default_m_tiles()};
+  const int nblk = S > 256 ? S / 256 : 1;   // (a tile's accumulator is at most 256 columns)
+  const NtTcOpts o{nblk};
   return gemm_nt_tc(seg, 1, S / nblk, skip, S, bskip, nullptr, 0, nullptr, 0, relu ? 1 : 0, 0, B, T, (cudaStream_t)stream,
                     nullptr, nullptr, nullptr, 0, 0, nullptr, &o);
 }
@@ -160,7 +142,7 @@ WNB_API int wnb_stack_bwd(const float* xs, const float* haux, const float* zall,
     const int nb = pick_block(ldz, cands, 5);
     WNB_REQUIRE(nb > 0, "stack_bwd: L*R must be a multiple of 32");
     const NtTcSeg seg[1] = {{dskip, S, 0, S, wskip_t, ldz, S, 0, 0}};
-    const NtTcOpts o{ldz / nb, 0, 0, 0, nt_default_m_tiles()};
+    const NtTcOpts o{ldz / nb};
     ProfScope ps(WNB_PROF_DZALL_GEMM, st);
     if ((rc = gemm_nt_tc(seg, 1, nb, dzall, ldz, nullptr, nullptr, 0, nullptr, 0, 0, 0, B, T, st, nullptr, nullptr, nullptr,
                          0, 0, nullptr, &o)) != WNB_OK)
@@ -179,12 +161,9 @@ WNB_API int wnb_stack_bwd(const float* xs, const float* haux, const float* zall,
        // matrix wgate_l = [[W1, 0], [0, W2res^T]] (3R x (K1+R)): accumulator columns 0..2R-1 are the gate
        // pre-activations, columns 2R..3R-1 the residual part of dz; the epilogue turns both into dpre.
       const float* wg = wgate + (size_t)l * 3 * R * (K1 + R);
-      // (resident weights: the zero blocks are skipped -- the first three segments touch accumulator columns 0..2R-1, the
-      //  dout segment columns 2R..3R-1)
-      const NtTcSeg sg[4] = {{xin, R, -d, R, wg, 3 * R, K1 + R, 0, 0, 0, 2 * R}, {xin, R, 0, R, wg, 3 * R, K1 + R, R, 0, 0, 2 * R},
-                             {haux, Ap, 0, Ap, wg, 3 * R, K1 + R, 2 * R, 0, 0, 2 * R},
-                             {dout, R, 0, R, wg, 3 * R, K1 + R, K1, 0, 2 * R, R}};
-      const NtTcOpts o{1, ldz, 1, dout ? 1 : 0, 1, stage_epi(), resident_w()};
+      const NtTcSeg sg[4] = {{xin, R, -d, R, wg, 3 * R, K1 + R, 0, 0}, {xin, R, 0, R, wg, 3 * R, K1 + R, R, 0},
+                             {haux, Ap, 0, Ap, wg, 3 * R, K1 + R, 2 * R, 0}, {dout, R, 0, R, wg, 3 * R, K1 + R, K1, 0}};
+      const NtTcOpts o{1, ldz, 1, dout ? 1 : 0};
       ProfScope ps(WNB_PROF_GATE_BWD, st);
       if ((rc = gemm_nt_tc(sg, dout ? 4 : 3, dout ? 3 * R : 2 * R, dxin /* z output suppressed */, R,
                            b1 + (size_t)l * 2 * R, nullptr, 0, nullptr, 0, 0, 0, B, T, st, dzl, dpre, nullptr, 0, 0,
@@ -194,16 +173,17 @@ WNB_API int wnb_stack_bwd(const float* xs, const float* haux, const float* zall,
     // dxin = dout + dpre(t+d) W1[:, tap0] + dpre(t) W1[:, tap1]   and   dhaux += dpre(t) W1[:, aux]
     if (dhaux) {
       ProfScope ps(WNB_PROF_DX_GEMM, st);
-      // (the unshifted segment covers all R + Ap columns and goes first; the shifted one only adds to the R dx columns)
-      const NtTcSeg sx[2] = {{dpre, 2 * R, 0, 2 * R, w1tl, K1, 2 * R, 0, R, 0, R + Ap}, {dpre, 2 * R, d, 2 * R, w1tl, R, 2 * R, 0, 0, 0, R}};
-      const NtTcOpts ox{1, 0, 0, 0, 1, stage_epi(), resident_w(), alternate_dir()};
+      // (the shifted segment sees w1t as an R-row matrix: its rows R.. are TMA zero fill, only the unshifted tap feeds the
+      //  aux columns)
+      const NtTcSeg sx[2] = {{dpre, 2 * R, 0, 2 * R, w1tl, K1, 2 * R, 0, R}, {dpre, 2 * R, d, 2 * R, w1tl, R, 2 * R, 0, 0}};
+      const NtTcOpts ox{1, 0, 0, 0, alternate_dir()};
       if ((rc = gemm_nt_tc(sx, 2, R + Ap, dxin, R, nullptr, nullptr, 0, dout, R, 0, 0, B, T, st, nullptr, nullptr, dhaux,
                            Ap, R, nullptr, &ox)) != WNB_OK)
         return rc;
     } else {
       ProfScope ps(WNB_PROF_DX_GEMM, st);
       const NtTcSeg sx[2] = {{dpre, 2 * R, d, 2 * R, w1tl, K1, 2 * R, 0, 0}, {dpre, 2 * R, 0, 2 * R, w1tl, K1, 2 * R, 0, R}};
-      const NtTcOpts ox{1, 0, 0, 0, 1, stage_epi(), resident_w(), alternate_dir()};
+      const NtTcOpts ox{1, 0, 0, 0, alternate_dir()};
       if ((rc = gemm_nt_tc(sx, 2, R, dxin, R, nullptr, nullptr, 0, dout, R, 0, 0, B, T, st, nullptr, nullptr, nullptr, 0, 0,
                            nullptr, &ox)) != WNB_OK)
         return rc;
@@ -236,21 +216,12 @@ WNB_API int wnb_stack_bwd(const float* xs, const float* haux, const float* zall,
     if ((rc = wgrad_tc_blocks(&blk, 1, bz, 1, R, B, T, st, &o)) != WNB_OK) return rc;
   }
 
-  {  // dWskip (S x L*R) += dskip^T Z_all, dbskip = column sums of dskip.  M-blocks per launch x columns per CTA is a
-     // trade: fewer M-blocks leave TMEM for wider column groups (fewer CTAs re-reading the same dskip tile through L2,
-     // fewer wasted bias columns per MMA) at the price of one launch per group of M-blocks.  Measured at the bench
-     // shape: 4 M-blocks x 96 columns = one 827 us launch, 2 M-blocks x 192 columns = two 313 us launches.
-     // WNB_DWSKIP_MB overrides (1..4).
-    static int mb_per_launch = 0;
-    if (!mb_per_launch) {
-      const char* e = getenv("WNB_DWSKIP_MB");
-      mb_per_launch = e ? atoi(e) : 2;
-      if (mb_per_launch < 1 || mb_per_launch > 4) mb_per_launch = 2;
-    }
+  {  // dWskip (S x L*R) += dskip^T Z_all, dbskip = column sums of dskip: every 128-row M-block of dskip in one launch,
+     // the L*R columns of Z_all in groups of up to 7 x 32 handled by different CTAs
     const int groups = ldz / 32;
-    const int nmb = (S + 127) / 128 < mb_per_launch ? (S + 127) / 128 : mb_per_launch;
+    const int nmb = (S + 127) / 128;
     int nB = 0;
-    for (int c = 512 / nmb / 32 - 1 < 7 ? 512 / nmb / 32 - 1 : 7; c >= 1 && !nB; c--)
+    for (int c = 7; c >= 1 && !nB; c--)
       if (groups % c == 0 && groups / c <= 128) nB = c;
     WNB_REQUIRE(nB > 0, "stack_bwd: cannot split L*R into column groups");
     for (int r0 = 0; r0 < S; r0 += 128 * nmb) {

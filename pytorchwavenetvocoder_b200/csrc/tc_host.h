@@ -1,4 +1,4 @@
-// tc_host.h -- host-side entry points of the tcgen05 kernels (internal; the C ABI is include/wnb200.h).
+// tc_host.h -- host-side entry points of the tensor-core (wgmma) kernels (internal; the C ABI is include/wnb200.h).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -27,10 +27,7 @@ int wgrad_tc(const WgOperand* a_ops, int na_ops, const WgOperand* b_ops, int nb_
 // ---- NT GEMM (gemm_nt_tc.cu):  out[b,t,n] = sum_seg sum_k A_seg[b,t+shift,k] W_seg[n0+n][k0+k]  (+ epilogues) ----
 // One segment: activation tensor (B,T,CA) read at rows t+shift, channels [0,K); weight matrix w (rows x ldw,
 // K-contiguous) rows [n0, n0+N), columns [k0, k0+K).
-struct NtTcSeg { const float* a; int CA; int shift; int K; const float* w; int w_rows; int w_cols; int k0; int n0;
-                 // NtTcOpts::resident_weights only: this segment touches output columns [n_lo, n_lo + n_cnt) (weight rows
-                 // n0 + n_lo ..); n_cnt == 0 means all N.  Lets a block matrix skip its zero blocks.
-                 int n_lo = 0; int n_cnt = 0; };
+struct NtTcSeg { const float* a; int CA; int shift; int K; const float* w; int w_rows; int w_cols; int k0; int n0; };
 // gate epilogue request: mode 1 = forward (z out), 2 = backward (dz in, z + dpre out); channels c0..c0+63 of R
 struct NtTcGate { int mode; int c0; int R; const float* bias_sig; const float* bias_tanh; const float* dz; float* dpre; };
 struct NtTcOpts {
@@ -39,17 +36,9 @@ struct NtTcOpts {
   int gate_ld_dz;    // row pitch (floats) of the gate-backward dz input (0: gate_R)
   int gate_skip_z;   // gate-backward: do not write z
   int gate_fused_dz; // gate-backward shorthand with N == 192: accumulator columns 128..191 are added to dz
-  int m_tiles;       // 2: a CTA tile is two 128-row time tiles sharing every weight chunk (plain epilogue, N <= 256):
-                     //    halves the L2 -> SM weight traffic of the K >= 512 GEMMs (skip, dZ_all, post network)
-  int stage_epilogue_operand;   // 1: the gate-backward dz slice / a 64-column residual `add` reaches the epilogue as a TMA
-                                //    tile loaded by the producer warp instead of per-lane row loads (gate backward, dX)
-  int resident_weights;   // 1: all weight chunks live in shared memory for the whole launch (loaded once per CTA), the ring
-                          //    carries activations only; needs sum_seg K * n_cnt * 4 bytes (<= ~140 KB) and m_tiles == 1
-  int reverse;            // 1: time tiles are processed from the end of the tensor backwards (a kernel that consumes what the
-                          //    previous launch wrote front to back finds the rows written last still in L2)
+  int reverse;       // 1: time tiles are processed from the end of the tensor backwards (a kernel that consumes what the
+                     //    previous launch wrote front to back finds the rows written last still in L2)
 };
-// default of NtTcOpts::m_tiles for the K >= 512 GEMMs: 2, WNB_NT_MT=1 in the environment restores one tile per CTA
-int nt_default_m_tiles();
 int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, const float* bias, const float* mask,
                int ldmask, const float* add, int ldadd, int relu_out, int accumulate, int B, int T, cudaStream_t st,
                const float* gate_dz = nullptr, float* gate_dpre = nullptr, float* out2 = nullptr, int ld_out2 = 0,
@@ -60,5 +49,11 @@ bool resblock_fwd_z_supported(int R, int Ap, int ks);
 int resblock_fwd_z(const float* xin, const float* haux, const float* w1, const float* b1, const float* w2res,
                    const float* b2res, float* xout, float* zall, int ldz, int zcol0, int B, int T, int d,
                    cudaStream_t st, int reverse = 0);   // reverse: time tiles from the end of the tensor backwards
+
+// ---- fused residual block, per-block form with skip accumulation (resblock_z.cu) ----------------------------------
+bool resblock_fwd_skip_supported(int R, int S, int Ap, int ks);
+int resblock_fwd_skip(const float* xin, const float* haux, const float* w1, const float* b1, const float* w2,
+                      const float* b2, float* xout, float* skip, int B, int T, int S, int d, int skip_init,
+                      cudaStream_t st);
 
 }  // namespace wnb

@@ -1,11 +1,12 @@
-// tc_ptx.cuh -- thin inline-PTX wrappers for the Blackwell (sm_100a) async machinery used by
-// resblock_tc.cu: mbarrier, TMA (cp.async.bulk.tensor load / store / reduce-add), tcgen05 (TMEM alloc,
-// mma kind::tf32 SS and TS, commit, ld/st, fences).  Descriptor encodings follow the bit layouts of the
-// UMMA SmemDescriptor / InstrDescriptor (cute/arch/mma_sm100_desc.hpp in CUTLASS 3.8+).
+// tc_ptx.cuh -- thin inline-PTX wrappers for the Hopper (sm_90a) async machinery of the tensor-core kernels:
+// mbarrier, TMA (cp.async.bulk.tensor load / store / reduce-add), wgmma (fences, commit / wait groups, shared-memory
+// matrix descriptors; the MMA wrappers themselves are in wgmma_tf32.cuh), named barriers.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "wgmma_tf32.cuh"
 
 namespace wnb {
 namespace ptx {
@@ -26,7 +27,7 @@ __device__ __forceinline__ bool elect_one() {
 
 // ---------------------------------------------------------------- programmatic dependent launch
 // Kernels launched with launch_pdl() (common.cuh) may become resident while the previous kernel of the stream is
-// still draining: everything up to pdl_wait() (barrier init, TMEM allocation, tensor-map prefetch) overlaps that
+// still draining: everything up to pdl_wait() (barrier init, tensor-map prefetch) overlaps that
 // kernel's tail; pdl_wait() returns once the previous kernel has completed and its writes are visible.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -143,102 +144,33 @@ __device__ __forceinline__ void bulk_wait() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------- wgmma
+// Shared-memory matrix descriptor of a K-major operand tile in the 128B-swizzled layout TMA writes with
+// CU_TENSOR_MAP_SWIZZLE_128B: rows of 32 fp32 (128 B), 8-row groups 1024 B apart (SBO), LBO unused.  The tile must start
+// on a 1024-byte boundary; the k-th group of 8 tf32 inside the row is addressed by adding 32 k bytes (2 k in the
+// descriptor's 16-byte units) to the start address.
+__device__ __forceinline__ uint64_t gmma_desc_k_sw128(uint32_t saddr) {
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// all previously issued tcgen05.mma of this thread arrive on `bar` when they complete
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// K-major, 128B-swizzled operand tile: rows at 128 B pitch, 8-row groups 1024 B apart (SBO), LBO unused (=1)
-__device__ __forceinline__ uint64_t smem_desc_k_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// Descriptor halves.  The low word carries the 16-byte-granular start address (bits 0-13) and LBO (bits 16-29), so
-// stepping through a tile is ONE integer add on the low word (no carry: shared memory addresses are < 256 KB);
-// the high word (SBO, version, swizzle mode) is a constant.  Keeping both in warp-uniform registers matters: the
-// MMA issuer is a single thread, and every extra instruction per tcgen05.mma lowers the issue rate.
-__device__ __forceinline__ uint32_t desc_lo(uint32_t saddr, uint32_t lbo_bytes) {
-  return ((saddr >> 4) & 0x3FFF) | ((lbo_bytes >> 4) << 16);
-}
-constexpr uint32_t kDescHiKSw128 = 64u | (1u << 14) | (2u << 29);      // SBO 1024 B, SWIZZLE_128B (K-major)
-constexpr uint32_t kDescHiMnSw128B32 = 32u | (1u << 14) | (1u << 29);  // SBO 512 B, SWIZZLE_128B_BASE32B (MN-major)
-__device__ __forceinline__ uint64_t desc64(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
-// Every kernel here allocates all 512 TMEM columns of its SM (1 CTA / SM), so the allocation starts at column 0,
-// lane 0.  Checking that once lets TMEM addresses be compile-time constants instead of values read back from
-// shared memory (which the compiler must treat as per-thread and move to uniform registers with an ELECT loop
-// in front of every tcgen05.mma).
-__device__ __forceinline__ void tmem_base_must_be_zero(uint32_t t) {
-  if (t != 0) {
-    printf("wnb200: unexpected TMEM base %u (block %d)\n", t, blockIdx.x);
-    __trap();
-  }
-}
-// tf32 x tf32 -> f32, both operands K-major
-__host__ __device__ constexpr uint32_t idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem]^T
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            bool accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]^T
-__device__ __forceinline__ void mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                            bool accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate)
-      : "memory");
-}
-
-// 32 lanes x 32 bit, 16 consecutive columns -> 16 registers per thread (thread i <-> lane base+i)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+// keeps the compiler from moving accumulator reads / writes across a wgmma wait
+template <int R>
+__device__ __forceinline__ void wg_touch(float (&d)[R]) {
 #pragma unroll
-  for (int i = 0; i < 16; i++) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-      "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-      "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])),
-      "r"(__float_as_uint(v[11])), "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])),
-      "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-      : "memory");
+// barrier over `threads` threads (a multiple of 32) of the CTA; id 0 is __syncthreads
+__device__ __forceinline__ void named_bar(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+// byte offset of element (row r, column c < 32) in a [rows x 32 fp32] tile written by TMA with 128B swizzle
+__device__ __forceinline__ uint32_t sw128_off(int r, int c) {
+  return (uint32_t)(r * 128 + ((((c >> 2) ^ r) & 7) << 4) + ((c & 3) << 2));
 }
 
 __device__ __forceinline__ float tanh_approx(float x) {

@@ -1,15 +1,17 @@
 // wgrad_tc.cu -- tensor-core weight gradients:  C[m][n] += sum_{b,t} A[b][t][m] * Bm[b][t+shift][n]
 //
-// The reduction index is TIME.  With channels-last activations a TMA box [64 time rows x 32 channels]
-// (128B swizzle with 32B atoms, the only swizzle tf32 MN-major operands accept) is directly an MN-major UMMA operand: the 32 contiguous channels are the M (or N) index,
-// the rows are K.  So both operands of every weight-gradient GEMM come straight from the activation /
-// gradient tensors with no transpose, and tcgen05.mma kind::tf32 (a_major = b_major = MN) contracts
-// 8 time steps per instruction into a [128 x N] fp32 accumulator that stays resident in TMEM for ALL
-// time tiles a CTA owns.  One persistent CTA per SM, 3 warp roles (TMA producer, MMA issuer, epilogue);
-// at the end the accumulator is flushed once with fp32 vector reductions (red.global.add.v4.f32).
-// Launch shapes: up to 5 M-blocks sharing one B operand; column groups of B across CTAs (n_split, A shared through
-// L2); segments = many independent problems of one structure (every residual block's dW1) in one launch, the CTAs
-// splitting the flattened (segment, time tile) space with two alternating accumulator sets.
+// The reduction index is TIME.  With channels-last activations a TMA box [32 time rows x 32 channels] is an MN-major
+// tile, and Hopper's tf32 wgmma takes K-major operands only.  So per 32-step stage the two consumer warpgroups
+//   - transpose the B sub-tiles (up to 7 x 32 channels) into one K-major [N x 32] tile in shared memory, and
+//   - read their A fragments (64 of the 128 M-block rows each) straight from the swizzled A sub-tiles into registers,
+// then issue wgmma m64nNk8 (A from registers, B from shared memory; double-buffered, so the transpose of the next stage
+// overlaps the MMAs of this one) into an fp32 accumulator that stays in registers for ALL time tiles a CTA owns.  At the
+// end every CTA writes its accumulator to its own slot of a scratch buffer and wgrad_reduce_kernel adds the slots of a
+// segment into C in slot order: no atomics, so the gradients do not depend on how the CTAs were scheduled.
+// A third role, one producer warp, streams the stages with TMA through an mbarrier ring.
+// Launch shapes: up to 5 M-blocks sharing one B operand (one CTA set per M-block); column groups of B across CTAs
+// (n_split, A shared through L2); segments = many independent problems of one structure (every residual block's dW1)
+// in one launch, `ksplit` CTAs per segment, each on a contiguous range of its time tiles.
 //
 // Generic over "sub-tile lists": A = 4 groups of 32 channels (M = 128), B = up to 7 groups (N <= 224),
 // each group = (tensor map, channel offset, time shift); dilated taps are just shifted groups, zero filled
@@ -29,13 +31,14 @@ namespace wg {
 
 constexpr int kMaxMB = 5;                    // M-blocks (128 rows each) sharing one B operand per launch
 constexpr int kMaxB = 8, kMaxMaps = 6, kMaxOps = 2 * kMaxMB + 8;
-constexpr int kThreadsW = 192;
+constexpr int kConsumers = 256;              // two warpgroups: rows 0..63 and 64..127 of the M-block
+constexpr int kThreadsW = kConsumers + 32;
 constexpr int kMaxSeg = 64;
+constexpr int kTK = 32;                      // time rows per stage (K of one stage)
+constexpr int kSub = kTK * 128;              // one [32 x 32 fp32] swizzled sub-tile
 
 // One TMA load per operand and stage: the tensor (B,T,C) is mapped 4-D as {32 ch, T, C/32 groups, B} with a box of
-// {32, tk, groups, 1}, which lands in shared memory as `groups` consecutive [tk x 32] swizzled sub-tiles -- exactly
-// the per-group layout the MMA descriptors expect.  (The producer is ONE thread: with a load per 32-channel group
-// its issue time, not HBM, bounded the wide launches.)
+// {32, 32, groups, 1}, which lands in shared memory as `groups` consecutive [32 x 32] swizzled sub-tiles.
 struct Op { int map; int cgrp0; int shift; int flags; int seg_cgrp_stride; int dst_group; };   // flags: WG_* of tc_host.h
 struct alignas(64) Params {
   CUtensorMap maps[kMaxMaps];
@@ -45,120 +48,79 @@ struct alignas(64) Params {
   int m_valid[kMaxMB];           // rows >= m_valid are padding (not written)
   float* db[kMaxMB];             // per block (128) or null
   int T, B, tiles_per_b, ntiles, nstages;
-  int tk;                        // time rows per stage (K of one stage): 64, 32 or 16
-  int vec4;                      // C blocks are 16-byte aligned with ldc % 4 == 0: flush with red.v4
   int n_split;                   // column groups of the B operand handled by different CTAs (WgOpts)
-  // segments (WgOpts::nseg > 1): nseg independent problems of identical structure (one per residual block) in one
-  // launch; the CTAs split the flattened (segment, time tile) space, accumulator sets alternate between segments
+  int ksplit;                    // CTAs per (M-block, column group, segment), each on a contiguous range of time tiles
+  float* part;                   // one [128 x N] accumulator slot per CTA
+  int ncols;                     // N: columns of a slot (32 * nB, + 32 for the ones group)
   int nseg, c_seg_stride, db_seg_stride;
   int seg_shift[kMaxSeg];
 };
 
-__device__ __forceinline__ uint64_t smem_desc_mn_sw128(uint32_t saddr, uint32_t lbo_bytes) {
-  // MN-major tf32 operands have exactly one legal swizzled layout: SWIZZLE_128B_BASE32B (layout type 1), the
-  // smem image of a TMA box written with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B: rows of 32 contiguous floats
-  // (the MN index) at 128 B pitch, 32-byte atoms XOR-ed with (row & 3); canonical form
-  // ((4,8,m),(4,k)):((1,4,LBO),(32,SBO)) in floats: MN groups LBO apart, 4-row k-groups SBO = 512 B apart.
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | (32ull << 32) |
-         (1ull << 46) | (1ull << 61);
-}
-__host__ __device__ constexpr uint32_t idesc_tf32_mn(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
-}
-
-// Tuning aid (WNB_PROF=1): cycles each role spends blocked, summed over CTAs (see tools/fwd_prof.py).
-enum { WP_P_EMPTY = 0, WP_M_FULL, WP_M_TOTAL, WP_E_FLUSH, WP_MIN, WP_MAX, WP_COUNT };
-__device__ unsigned long long g_wg_prof[WP_COUNT];
-
-template <bool PROF>
+template <int N>
 __global__ void __launch_bounds__(kThreadsW, 1) wgrad_tc_kernel(const __grid_constant__ Params p) {
-  long long acc[WP_COUNT] = {};
-  auto wait = [&](uint64_t* bar, uint32_t parity, int k) {
-    if constexpr (PROF) {
-      const long long t = clock64();
-      ptx::mbar_wait(bar, parity);
-      acc[k] += clock64() - t;
-    } else {
-      ptx::mbar_wait(bar, parity);
-    }
-  };
-  const long long t_begin = PROF ? clock64() : 0;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int nsubB = p.nB + (p.use_ones ? 1 : 0);
-  const int kSubBytes = p.tk * 128;          // [tk x 32 fp32] swizzled sub-tile
-  const int nA = 4 * p.nMB;
-  const int stage_bytes = (nA + nsubB) * kSubBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)p.nstages * stage_bytes);
+  const int stage_bytes = (4 + p.nB) * kSub;
+  unsigned char* bT = smem;                                   // 2 x K-major [N x 32] B tile (+ the ones rows)
+  unsigned char* ring = smem + 2 * N * 128;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + (size_t)p.nstages * stage_bytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + p.nstages;
-  uint64_t* done = bars + 2 * p.nstages;        // [2]: accumulator set s holds a finished segment
-  uint64_t* accfree = done + 2;                 // [2]: the epilogue has flushed accumulator set s
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accfree + 2);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int N = 32 * nsubB;
 
-  // tiles owned by this CTA: contiguous range (better L2 locality for shifted taps)
-  // with n_split column groups, CTA (g, s) = (blockIdx % n_split, blockIdx / n_split): neighbouring CTAs stream the
-  // same time range (A operand shared through L2) for different 32*nB-channel groups of the B operand
-  const int ng = blockIdx.x % p.n_split, tsplit = blockIdx.x / p.n_split, ntsplit = gridDim.x / p.n_split;
+  // CTA -> (M-block, column group, segment, time split); with n_split column groups neighbouring CTAs stream the same
+  // time range (A operand shared through L2) for different 32*nB-channel groups of the B operand.  Tiles are indexed
+  // f = seg * ntiles + tile; a CTA's range lies inside one segment.
+  const int mb = blockIdx.x % p.nMB;
+  const int rest = blockIdx.x / p.nMB;
+  const int ng = rest % p.n_split, r2 = rest / p.n_split;
+  const int seg0 = r2 / p.ksplit, tsplit = r2 % p.ksplit;
   const int bcol0 = ng * 32 * p.nB;
-  const int total_tiles = p.ntiles * p.nseg;    // flattened (segment, tile) index f = seg * ntiles + tile
-  const int per = (total_tiles + ntsplit - 1) / ntsplit;
-  const int tile_begin = tsplit * per;
-  const int tile_end = min(total_tiles, tile_begin + per);
-  const uint32_t acc_cols = (uint32_t)p.nMB * (32u * nsubB);   // TMEM columns of one accumulator set
-  const int my_tiles = max(0, tile_end - tile_begin);
+  const int per = (p.ntiles + p.ksplit - 1) / p.ksplit;
+  const int tile_begin = seg0 * p.ntiles + min(p.ntiles, tsplit * per);
+  const int tile_end = seg0 * p.ntiles + min(p.ntiles, (tsplit + 1) * per);
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < p.nstages; i++) {
       ptx::mbar_init(&full[i], 1);
-      ptx::mbar_init(&empty[i], 1);
+      ptx::mbar_init(&empty[i], kConsumers);
     }
-    for (int i = 0; i < 2; i++) { ptx::mbar_init(&done[i], 1); ptx::mbar_init(&accfree[i], 128); }
     ptx::fence_barrier_init();
   }
-  if (p.use_ones) {
-    // the ones group of every stage: filled once, never touched by TMA
-    for (int s = 0; s < p.nstages; s++) {
-      float4* o = reinterpret_cast<float4*>(smem + (size_t)s * stage_bytes + (nA + p.nB) * kSubBytes);
-      for (int i = threadIdx.x; i < kSubBytes / 16; i += kThreadsW) o[i] = make_float4(1.f, 1.f, 1.f, 1.f);
+  if (p.use_ones) {   // the ones rows of both transposed B tiles: filled once, never overwritten
+    for (int h = 0; h < 2; h++) {
+      float4* o = reinterpret_cast<float4*>(bT + h * N * 128 + p.nB * 32 * 128);
+      for (int i = threadIdx.x; i < 32 * 128 / 16; i += kThreadsW) o[i] = make_float4(1.f, 1.f, 1.f, 1.f);
     }
-    ptx::fence_proxy_async();
   }
-  if (warp == 1) ptx::tmem_alloc<512>(tmem_slot);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  ptx::tmem_base_must_be_zero(*tmem_slot);
-  constexpr uint32_t tmem = 0;
   // programmatic dependent launch: the set-up above overlapped the previous kernel's tail; from here on this
   // kernel reads / writes memory that kernel may have produced
   ptx::pdl_launch_dependents();
   ptx::pdl_wait();
 
-  // single-thread roles are entered through elect.sync (not `lane == 0`): the compiler then knows exactly one
-  // thread is active and issues the uniform-datapath TMA / tcgen05 instructions without a per-thread ELECT loop
-  if (warp == 0) {
-    if (my_tiles > 0 && ptx::elect_one()) {
+  if (warp == kConsumers / 32) {
+    // =============================== TMA producer ===============================
+    if (tile_begin < tile_end && ptx::elect_one()) {
       for (int i = 0; i < kMaxMaps; i++) ptx::prefetch_tmap(&p.maps[i]);
       uint32_t s = 0, ph = 0;
-      // (segment, batch, tile-in-batch) advance incrementally: this thread's instruction count per stage is what
-      // bounds the wide launches, so no divisions in the loop
       int seg = tile_begin / p.ntiles, b = (tile_begin - seg * p.ntiles) / p.tiles_per_b;
       int tb = tile_begin - seg * p.ntiles - b * p.tiles_per_b;
+      const int nA = 4 * p.nMB;
       for (int f = tile_begin; f < tile_end; f++) {
-        const int t0 = tb * p.tk;
-        wait(&empty[s], ph ^ 1, WP_P_EMPTY);
-        ptx::mbar_arrive_expect_tx(&full[s], (nA + p.nB) * kSubBytes);
-        unsigned char* st = smem + (size_t)s * stage_bytes;
+        const int t0 = tb * kTK;
+        ptx::mbar_wait(&empty[s], ph ^ 1);
+        ptx::mbar_arrive_expect_tx(&full[s], stage_bytes);
+        unsigned char* st = ring + (size_t)s * stage_bytes;
         for (int i = 0; i < p.nops; i++) {
           const Op o = p.ops[i];
+          int dst;
+          if (o.dst_group >= nA) dst = 4 + o.dst_group - nA;                               // B operand
+          else if (o.dst_group >= 4 * mb && o.dst_group < 4 * mb + 4) dst = o.dst_group - 4 * mb;   // this M-block's A
+          else continue;
           const int cg = o.cgrp0 + (o.dst_group >= nA ? bcol0 >> 5 : 0) + seg * o.seg_cgrp_stride;
           const int t = t0 + ((o.flags & WG_SEG_SHIFT) ? p.seg_shift[seg] : o.shift);
-          ptx::tma_load_4d(st + o.dst_group * kSubBytes, &p.maps[o.map], &full[s], 0, t, cg,
-                           (o.flags & WG_LAYERED) ? seg * p.B + b : b);
+          ptx::tma_load_4d(st + dst * kSub, &p.maps[o.map], &full[s], 0, t, cg, (o.flags & WG_LAYERED) ? seg * p.B + b : b);
         }
         if (++s == (uint32_t)p.nstages) { s = 0; ph ^= 1; }
         if (++tb == p.tiles_per_b) {
@@ -167,106 +129,95 @@ __global__ void __launch_bounds__(kThreadsW, 1) wgrad_tc_kernel(const __grid_con
         }
       }
     }
-  } else if (warp == 1) {
-    if (my_tiles > 0 && ptx::elect_one()) {
-      const uint32_t idesc = idesc_tf32_mn(128, N);
-      // MN-major tf32 operands have exactly one legal swizzled layout, SWIZZLE_128B_BASE32B (see tc_ptx.cuh): MN
-      // groups are LBO = one sub-tile apart, 4-row k-groups 512 B apart, one MMA K-step (8 rows) = 1024 B.
-      const uint32_t s_lo0 = ptx::desc_lo(ptx::smem_u32(smem), kSubBytes);
-      constexpr uint32_t hi = ptx::kDescHiMnSw128B32;
-      const uint32_t stage_step = (uint32_t)stage_bytes >> 4, sub_step = (uint32_t)kSubBytes >> 4;
-      const int ksteps = p.tk / 8;
-      uint32_t s = 0, ph = 0, it = 0, nsegs_done = 0;
-      int next_boundary = (tile_begin / p.ntiles + 1) * p.ntiles;   // first flattened index of the next segment
-      for (int f = tile_begin; f < tile_end; f++, it++) {
-        if (f == next_boundary) {   // segment boundary inside this CTA's range: hand the finished set to the epilogue
-          ptx::tc_commit(&done[nsegs_done & 1]);
-          nsegs_done++;
-          next_boundary += p.ntiles;
-          it = 0;
-          if (nsegs_done >= 2) {   // the set about to be reused was handed over two segments ago
-            ptx::mbar_wait(&accfree[nsegs_done & 1], ((nsegs_done >> 1) - 1) & 1);
-            ptx::tc_fence_after();
-          }
-        }
-        const uint32_t dcol = (nsegs_done & 1) * acc_cols;
-        wait(&full[s], ph, WP_M_FULL);
-        ptx::tc_fence_after();
-        const uint32_t a_lo = s_lo0 + s * stage_step, b_lo = a_lo + nA * sub_step;
-        for (int mb = 0; mb < p.nMB; mb++) {
-          const uint32_t am_lo = a_lo + mb * 4 * sub_step;
-          for (int k = 0; k < ksteps; k++)
-            ptx::mma_tf32_ss(tmem + dcol + mb * N, ptx::desc64(am_lo + k * 64, hi), ptx::desc64(b_lo + k * 64, hi), idesc,
-                             (it | k) != 0);
-        }
-        ptx::tc_commit(&empty[s]);
-        if (++s == (uint32_t)p.nstages) { s = 0; ph ^= 1; }
-      }
-      ptx::tc_commit(&done[nsegs_done & 1]);
-      if constexpr (PROF) acc[WP_M_TOTAL] = clock64() - t_begin;
-    }
-  } else if (my_tiles > 0) {
-    // epilogue: flush each finished accumulator set once (one per segment of this CTA's range)
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-    const int nchunk = N / 16;
-    const int first_seg = tile_begin / p.ntiles, last_seg = (tile_end - 1) / p.ntiles;
-    long long t_flush = 0;
-    for (int k = 0; k <= last_seg - first_seg; k++) {
-      const int seg = first_seg + k, aset = k & 1;
-      ptx::mbar_wait(&done[aset], (k >> 1) & 1);
-      ptx::tc_fence_after();
-      if (PROF && k == 0) t_flush = clock64();
-      const uint32_t dcol = aset * acc_cols;
-      for (int mb = 0; mb < p.nMB; mb++) {
-        float* cbase = p.c[mb] + (size_t)seg * p.c_seg_stride;
-        for (int ci = 0; ci < nchunk; ci++) {
-          // every CTA flushes the same addresses: start at a CTA-dependent chunk so the atomics spread out
-          const int c0 = ((ci + blockIdx.x) % nchunk) * 16;
-          float v[16];
-          ptx::tmem_ld16(tmem + lane_base + dcol + mb * N + c0, v);
-          ptx::tc_wait_ld();
-          if (row < p.m_valid[mb]) {
-            if (c0 < 32 * p.nB) {
-              float* dst = cbase + (size_t)row * p.ldc + bcol0 + c0;
-              if (p.vec4) {   // 16-byte vector reductions: a quarter of the L2 atomic operations
-#pragma unroll
-                for (int i = 0; i < 16; i += 4)
-                  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + i), "f"(v[i]), "f"(v[i + 1]),
-                               "f"(v[i + 2]), "f"(v[i + 3])
-                               : "memory");
-              } else {
-#pragma unroll
-                for (int i = 0; i < 16; i++) atomicAdd(dst + i, v[i]);
-              }
-            } else if (c0 == 32 * p.nB && p.db[mb] && ng == 0) {
-              atomicAdd(p.db[mb] + (size_t)seg * p.db_seg_stride + row, v[0]);
-            }
-          }
-        }
-      }
-      ptx::tc_fence_before();
-      ptx::mbar_arrive(&accfree[aset]);
-    }
-    if constexpr (PROF) {
-      if (warp == 2) {
-        acc[WP_E_FLUSH] = clock64() - t_flush;
-        if (lane == 0) {
-          atomicMin(&g_wg_prof[WP_MIN], (unsigned long long)(clock64() - t_begin));
-          atomicMax(&g_wg_prof[WP_MAX], (unsigned long long)(clock64() - t_begin));
-        }
-      }
-    }
+    return;
   }
-  if constexpr (PROF) {
-    if (warp <= 1 || (warp == 2 && lane == 0))   // single-thread roles: only the elected lane has counts
-      for (int k = 0; k < WP_MIN; k++)
-        if (acc[k]) atomicAdd(&g_wg_prof[k], (unsigned long long)acc[k]);
+
+  // =============================== consumers: transpose B, wgmma, flush ===============================
+  const int wgi = warp >> 2, wq = warp & 3;
+  const int g = lane >> 2, tq = lane & 3;
+  const int m0 = 64 * wgi + 16 * wq + g;          // A rows m0 and m0 + 8 of this thread's fragments
+  float d[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; i++) d[i] = 0.f;
+  auto write_slot = [&]() {   // this CTA's accumulator -> its scratch slot (every row and column, zeros included)
+    float* slot = p.part + (size_t)blockIdx.x * 128 * N;
+#pragma unroll
+    for (int i = 0; i < N / 2; i += 2) {
+      const int m = m0 + 8 * ((i >> 1) & 1), n = 8 * (i >> 2) + 2 * tq;
+      *reinterpret_cast<float2*>(slot + (size_t)m * N + n) = make_float2(d[i], d[i + 1]);
+    }
+  };
+  uint32_t s = 0, ph = 0;
+  const int nvec = p.nB * 32 * 32 / 4;            // float4 pieces of the B sub-tiles
+  // Stage i: B transposed into bT[i & 1], A fragments into register set i & 1, the ring stage released, then the MMAs of
+  // stage i are issued and those of stage i - 1 waited for -- so the transpose of stage i + 1 overlaps the MMAs of stage i.
+  // (wgmma reads its A registers asynchronously: the set of stage i is not touched again before stage i + 2.)
+  uint32_t a0[4][4], a1[4][4];
+  auto stage = [&](uint32_t (&a)[4][4], unsigned char* bTh) {
+    ptx::mbar_wait(&full[s], ph);
+    const unsigned char* st = ring + (size_t)s * stage_bytes;
+    ptx::named_bar(1, kConsumers);   // every consumer has waited for the MMAs of stage i - 2: bTh may be overwritten
+    for (int idx = threadIdx.x; idx < nvec; idx += kConsumers) {
+      const int grp = idx >> 8, r = (idx >> 3) & 31, c4 = idx & 7;   // B group, time row, 4-channel piece
+      const float4 v = *reinterpret_cast<const float4*>(st + (4 + grp) * kSub + r * 128 + ((c4 ^ (r & 7)) << 4));
+      const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int n = grp * 32 + c4 * 4 + j;
+        *reinterpret_cast<float*>(bTh + ptx::sw128_off(n, r)) = vv[j];
+      }
+    }
+#pragma unroll
+    for (int kk = 0; kk < 4; kk++) {
+      const int k = 8 * kk + tq;
+#pragma unroll
+      for (int h = 0; h < 4; h++) {
+        const int m = m0 + 8 * (h & 1), kr = k + 4 * (h >> 1);
+        a[kk][h] = *reinterpret_cast<const uint32_t*>(st + (m >> 5) * kSub + ptx::sw128_off(kr, m & 31));
+      }
+    }
+    ptx::mbar_arrive(&empty[s]);     // this thread's reads of the ring stage are done
+    if (++s == (uint32_t)p.nstages) { s = 0; ph ^= 1; }
+    ptx::fence_proxy_async();
+    ptx::named_bar(1, kConsumers);
+    ptx::wg_fence();
+    const uint32_t b_u32 = ptx::smem_u32(bTh);
+#pragma unroll
+    for (int kk = 0; kk < 4; kk++) ptx::wgmma_rs<N>(d, a[kk], ptx::gmma_desc_k_sw128(b_u32 + 32 * kk), 1);
+    ptx::wg_commit();
+    ptx::wg_wait<1>();
+  };
+  for (int f = tile_begin; f < tile_end; f += 2) {
+    stage(a0, bT);
+    if (f + 1 < tile_end) stage(a1, bT + N * 128);
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc<512>(tmem);
+  ptx::wg_wait<0>();
+  ptx::wg_touch(d);
+  write_slot();
+}
+
+// C[seg][m][bcol0 + n] += sum over the ksplit slots of (M-block, column group, segment), in slot order; column 32 nB
+// (the ones group) is the bias gradient db[seg][m] (column group 0 only)
+__global__ void wgrad_reduce_kernel(const __grid_constant__ Params p) {
+  const int nc = 32 * p.nB + p.use_ones;
+  const int64_t total = (int64_t)p.nseg * p.n_split * p.nMB * 128 * nc;
+  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    int64_t r = idx;
+    const int n = (int)(r % nc); r /= nc;
+    const int m = (int)(r % 128); r /= 128;
+    const int mb = (int)(r % p.nMB); r /= p.nMB;
+    const int ng = (int)(r % p.n_split);
+    const int seg = (int)(r / p.n_split);
+    if (m >= p.m_valid[mb]) continue;
+    if (n >= 32 * p.nB && (ng != 0 || !p.db[mb])) continue;
+    float sum = 0.f;
+    for (int j = 0; j < p.ksplit; j++) {
+      const int64_t slot = ((int64_t)(seg * p.ksplit + j) * p.n_split + ng) * p.nMB + mb;
+      sum += p.part[(slot * 128 + m) * p.ncols + n];
+    }
+    if (n < 32 * p.nB) p.c[mb][(size_t)seg * p.c_seg_stride + (size_t)m * p.ldc + ng * 32 * p.nB + n] += sum;
+    else p.db[mb][(size_t)seg * p.db_seg_stride + m] += sum;
+  }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -285,16 +236,23 @@ static EncodeTiledFn get_encode() {
 }
 
 // (B, T, C) fp32 channels-last tensor seen as {32 ch, T, C/32 groups, B} (the group axis OUTSIDE time, so that the box
-// {32, tk, groups, 1} lands in shared memory group-major: `groups` consecutive [tk x 32] sub-tiles)
-static bool make_act_map(CUtensorMap* m, const float* base, int C, int T, int B, int tk, int groups) {
+// {32, 32, groups, 1} lands in shared memory group-major: `groups` consecutive [32 x 32] sub-tiles)
+static bool make_act_map(CUtensorMap* m, const float* base, int C, int T, int B, int groups) {
   EncodeTiledFn enc = get_encode();
   if (!enc || C % 32 != 0) return false;
   cuuint64_t gdim[4] = {32, (cuuint64_t)T, (cuuint64_t)(C / 32), (cuuint64_t)B};
   cuuint64_t gstr[3] = {(cuuint64_t)C * 4, 128, (cuuint64_t)C * 4 * (cuuint64_t)T};
-  cuuint32_t box[4] = {32, (cuuint32_t)tk, (cuuint32_t)groups, 1}, es[4] = {1, 1, 1, 1};
+  cuuint32_t box[4] = {32, (cuuint32_t)kTK, (cuuint32_t)groups, 1}, es[4] = {1, 1, 1, 1};
   return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), gdim, gstr, box, es,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+template <int N>
+static cudaError_t launch_n(int grid, size_t smem, cudaStream_t st, const Params& p) {
+  cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(wgrad_tc_kernel<N>), smem);
+  if (e != cudaSuccess) return e;
+  return launch_pdl(wgrad_tc_kernel<N>, grid, kThreadsW, smem, st, p);
 }
 
 }  // namespace wg
@@ -314,20 +272,10 @@ int wgrad_tc_blocks(const WgBlock* blocks, int nblocks, const WgOperand* b_ops, 
   p.use_ones = any_db ? 1 : 0;
   if (p.nB < 1 || p.nB > kMaxB - 1) { set_error("wgrad_tc: 1..7 B groups"); return WNB_ERR_INVALID; }
   const int N = 32 * (p.nB + p.use_ones);
-  if (N * nblocks > 512) { set_error("wgrad_tc: accumulators exceed TMEM (%d x %d columns)", nblocks, N); return WNB_ERR_INVALID; }
-  // rows per stage: HBM needs several stages of loads in flight per SM (ncu: 2 stages of 64 rows ran at 40 % of
-  // peak), so take the largest of {64, 32, 16} that still leaves at least 4 stages
-  const int groups = 4 * nblocks + p.nB + p.use_ones;
-  int tk = 64;
-  static int min_stages = 0;
-  if (!min_stages) { const char* e = getenv("WNB_WG_MINSTAGES"); min_stages = e ? atoi(e) : 2; if (min_stages < 2) min_stages = 2; }
-  while (tk > 16 && (220 * 1024) / (groups * tk * 128) < min_stages) tk >>= 1;
-  const int sub = tk * 128;
-  const int stage_bytes = groups * sub;
-  int nst = (220 * 1024) / stage_bytes;
+  const int stage_bytes = (4 + p.nB) * kSub;
+  int nst = (227 * 1024 - 1024 - 256 - 2 * N * 128) / stage_bytes;
   if (nst > 8) nst = 8;
   if (nst < 2) { set_error("wgrad_tc: stage too large"); return WNB_ERR_INVALID; }
-  p.tk = tk;
   p.nstages = nst;
 
   int nmaps = 0;
@@ -338,7 +286,7 @@ int wgrad_tc_blocks(const WgBlock* blocks, int nblocks, const WgOperand* b_ops, 
       if (map_base[i] == o.base && map_c[i] == o.C && map_g[i] == o.groups) return i;
     if (nmaps >= kMaxMaps) return -1;
     const int nseg_map = (opts && opts->nseg > 1 && (o.flags & WG_LAYERED)) ? opts->nseg : 1;
-    if (!make_act_map(&p.maps[nmaps], o.base, o.C, T, B * nseg_map, tk, o.groups)) return -1;
+    if (!make_act_map(&p.maps[nmaps], o.base, o.C, T, B * nseg_map, o.groups)) return -1;
     map_base[nmaps] = o.base; map_c[nmaps] = o.C; map_g[nmaps] = o.groups;
     return nmaps++;
   };
@@ -370,46 +318,45 @@ int wgrad_tc_blocks(const WgBlock* blocks, int nblocks, const WgOperand* b_ops, 
   p.n_split = (opts && opts->n_split > 1) ? opts->n_split : 1;
   p.nseg = (opts && opts->nseg > 1) ? opts->nseg : 1;
   if (p.nseg > 1) {
-    if (p.nseg > kMaxSeg || p.n_split > 1 || 2 * N * nblocks > 512 || !opts->seg_shift) {
-      set_error("wgrad_tc: bad segment configuration (nseg=%d, %d accumulator columns)", p.nseg, N * nblocks);
+    if (p.nseg > kMaxSeg || p.n_split > 1 || !opts->seg_shift) {
+      set_error("wgrad_tc: bad segment configuration (nseg=%d)", p.nseg);
       return WNB_ERR_INVALID;
     }
     for (int i = 0; i < p.nseg; i++) p.seg_shift[i] = opts->seg_shift[i];
     p.c_seg_stride = opts->c_seg_stride;
     p.db_seg_stride = opts->db_seg_stride;
   }
-  p.vec4 = (ldc % 4 == 0) ? 1 : 0;
-  for (int i = 0; i < nblocks; i++)
-    if (reinterpret_cast<uintptr_t>(blocks[i].c) & 15) p.vec4 = 0;
   p.T = T; p.B = B;
-  p.tiles_per_b = (T + tk - 1) / tk;
+  p.tiles_per_b = (T + kTK - 1) / kTK;
   p.ntiles = B * p.tiles_per_b;
-  const size_t smem = (size_t)nst * stage_bytes + 1024 + 256;   // barriers: 2*nst + 4 (+ TMEM slot) <= 21 words
-  WNB_CUDA(ensure_dynamic_smem(reinterpret_cast<const void*>(wgrad_tc_kernel<false>), smem));
-  WNB_CUDA(ensure_dynamic_smem(reinterpret_cast<const void*>(wgrad_tc_kernel<true>), smem));
+  const size_t smem = (size_t)2 * N * 128 + (size_t)nst * stage_bytes + 1024 + 256;
   const int sms = device_sms();
-  int grid = p.ntiles < sms ? p.ntiles : sms;
-  if (p.n_split > 1) {
-    if (p.n_split > sms) { set_error("wgrad_tc: n_split exceeds the SM count"); return WNB_ERR_INVALID; }
-    grid = (sms / p.n_split) * p.n_split;
+  const int sets = p.nMB * p.n_split * p.nseg;
+  int ksplit = sms / sets;
+  if (ksplit < 1) ksplit = 1;
+  if (ksplit > p.ntiles) ksplit = p.ntiles;
+  p.ksplit = ksplit;
+  p.ncols = N;
+  const int grid = sets * ksplit;
+  p.part = static_cast<float*>(scratch_buffer(st, SCRATCH_WGRAD, (size_t)grid * 128 * N * sizeof(float)));
+  if (!p.part) { set_error("wgrad_tc: cannot allocate the partial-sum scratch"); return WNB_ERR_CUDA; }
+  cudaError_t le;
+  switch (N) {
+    case 32: le = launch_n<32>(grid, smem, st, p); break;
+    case 64: le = launch_n<64>(grid, smem, st, p); break;
+    case 96: le = launch_n<96>(grid, smem, st, p); break;
+    case 128: le = launch_n<128>(grid, smem, st, p); break;
+    case 160: le = launch_n<160>(grid, smem, st, p); break;
+    case 192: le = launch_n<192>(grid, smem, st, p); break;
+    case 224: le = launch_n<224>(grid, smem, st, p); break;
+    default: le = launch_n<256>(grid, smem, st, p); break;
   }
-  static int prof = -1;
-  if (prof < 0) { const char* e = getenv("WNB_PROF"); prof = (e && e[0] == '1') ? 1 : 0; }
-  if (prof) {
-    unsigned long long zero[WP_COUNT] = {}, h[WP_COUNT];
-    zero[WP_MIN] = ~0ull;
-    WNB_CUDA(cudaMemcpyToSymbol(g_wg_prof, zero, sizeof(zero)));
-    wgrad_tc_kernel<true><<<grid, kThreadsW, smem, st>>>(p);
-    WNB_CHECK_LAUNCH("wgrad_tc");
-    WNB_CUDA(cudaStreamSynchronize(st));
-    WNB_CUDA(cudaMemcpyFromSymbol(h, g_wg_prof, sizeof(h)));
-    fprintf(stderr, "wnb200 wgrad prof nMB=%d nB=%d tk=%d stages=%d stage=%dKB (kcycles/CTA): P:empty=%.1f M:full=%.1f "
-            "M:total=%.1f E:flush=%.1f cta min=%.1f max=%.1f\n", p.nMB, p.nB, p.tk, p.nstages, stage_bytes / 1024,
-            h[0] / 1e3 / grid, h[1] / 1e3 / grid, h[2] / 1e3 / grid, h[3] / 1e3 / grid, h[4] / 1e3, h[5] / 1e3);
-    return WNB_OK;
-  }
-  if (launch_pdl(wgrad_tc_kernel<false>, grid, kThreadsW, smem, st, p) != cudaSuccess) { /* reported below */ }
+  if (le != cudaSuccess) { set_error("wgrad_tc: launch failed: %s", cudaGetErrorString(le)); return WNB_ERR_CUDA; }
   WNB_CHECK_LAUNCH("wgrad_tc");
+  const int64_t total = (int64_t)p.nseg * p.n_split * p.nMB * 128 * (32 * p.nB + p.use_ones);
+  const int64_t rblocks = (total + 255) / 256;
+  wgrad_reduce_kernel<<<(int)(rblocks < sms * 8 ? rblocks : sms * 8), 256, 0, st>>>(p);
+  WNB_CHECK_LAUNCH("wgrad_reduce");
   return WNB_OK;
 }
 

@@ -1,9 +1,9 @@
 # -*- coding: utf-8 -*-
-"""B200-native mirror of ``wavenet_vocoder/nets/wavenet.py`` (reference v0.1.1).
+"""H100-native mirror of ``wavenet_vocoder/nets/wavenet.py`` (reference v0.1.1).
 
 Same import surface, constructor arguments, attributes, method signatures, ``state_dict`` keys and
 error behaviour as the reference module (SURVEY.md 8b), but every hot-path computation is a
-hand-written sm_100a kernel reached through the C ABI in ``include/wnb200.h``:
+hand-written sm_90a kernel reached through the C ABI in ``include/wnb200.h``:
 
 * ``WaveNet.forward``  (reference wavenet.py:212-241)  -> front gather, aux up-sampling, ONE fused
   kernel per residual block, post network; backward through ``torch.autograd.Function``.
@@ -34,7 +34,7 @@ PROFILE_EVENTS = None
 
 
 def tc_supported(cfg):
-    """True when the tcgen05 (tf32) fused-block kernel covers WaveNet(*cfg)."""
+    """True when the tf32 tensor-core path covers WaveNet(*cfg)."""
     lib = _lib.load()
     Q, A, R, S, depth, repeat, ks, U = cfg
     return bool(lib.wnb_resblock_fwd_supported(R, S, _round_up(A, 32), ks, MATH_TF32))
@@ -42,7 +42,7 @@ def tc_supported(cfg):
 
 def _device():
     if not torch.cuda.is_available():
-        raise _lib.WnbError("no CUDA device: the wnb200 kernels need a B200 (there is no CPU fallback)")
+        raise _lib.WnbError("no CUDA device: the wnb200 kernels need a CUDA GPU (there is no CPU fallback)")
     return torch.device("cuda", torch.cuda.current_device())
 
 
@@ -199,7 +199,7 @@ class _WaveNetFn(torch.autograd.Function):
         xs = torch.empty(nbuf, B, T, R, device=dev, dtype=torch.float32)
         check(lib.wnb_front_embed_fwd(ptr(x), ptr(wf), ptr(bf), ptr(xs[0]), B, T, Q, R, ks, st), "front_embed_fwd")
         skip = torch.empty(B, T, S, device=dev, dtype=torch.float32)
-        # shapes outside the fused tcgen05 kernel run the composed tcgen05 path, which needs a z scratch
+        # the composed tensor-core path needs a z scratch
         zbuf = None
         if math_mode == MATH_TF32 and lib.wnb_resblock_fwd_supported(R, S, Ap, ks, MATH_TF32) == 2:
             zbuf = torch.empty(B, T, R, device=dev, dtype=torch.float32)
@@ -511,11 +511,11 @@ class CausalConv1d(nn.Module):
         if torch.is_grad_enabled() and (x.requires_grad or self.conv.weight.requires_grad):
             # the reference module is a differentiable Conv1d; this standalone helper has no backward kernel, and a
             # silently detached result would train nothing -- say so instead
-            raise RuntimeError("CausalConv1d.forward is inference-only in the B200 build (no standalone backward): "
+            raise RuntimeError("CausalConv1d.forward is inference-only in this build (no standalone backward): "
                                "call it under torch.no_grad(); training goes through WaveNet.forward")
         lib = _lib.load()
         if not x.is_cuda:
-            raise _lib.WnbError("CausalConv1d.forward needs CUDA tensors: the B200 build has no CPU fallback")
+            raise _lib.WnbError("CausalConv1d.forward needs CUDA tensors: this build has no CPU fallback")
         B, C, T = x.shape
         xl = x.detach().float().transpose(1, 2).contiguous()                                   # (B, T, C)
         w = self.conv.weight.detach().float().permute(0, 2, 1).reshape(self.out_channels, -1).contiguous()  # [o][j*C+c]
@@ -579,8 +579,8 @@ class WaveNet(nn.Module):
         self.dilations = [2 ** i for i in range(self.dilation_depth)] * self.dilation_repeat
         self.receptive_field = (self.kernel_size - 1) * sum(self.dilations) + 1
 
-        # B200 build: contraction precision of the training forward. "fp32" = FFMA parity path,
-        # "tf32" = tcgen05 tensor-core path (fp32 storage and accumulation). Decode is always fp32.
+        # contraction precision of the training forward. "fp32" = FFMA parity path,
+        # "tf32" = wgmma tensor-core path (fp32 storage and accumulation). Decode is always fp32.
         self.math_mode = "fp32"
 
         # for preprocessing
@@ -684,13 +684,13 @@ class WaveNet(nn.Module):
         return plan
 
     def forward_loss(self, x, h, t, start=None):
-        """Training entry of the B200 build: mean cross entropy of ``forward(x, h)[:, start:]`` against ``t[:, start:]``
+        """Training entry of this build: mean cross entropy of ``forward(x, h)[:, start:]`` against ``t[:, start:]``
         (reference bin/train.py:533-536 with ``start = receptive_field``) as ONE autograd node -- the post network's
         logits never make a round trip through a separate loss kernel's gradient multiply.  Same value and gradients as
         ``cross_entropy(self(x, h), t, start)``."""
         start = self.receptive_field if start is None else int(start)
         if not x.is_cuda:
-            raise _lib.WnbError("WaveNet.forward_loss needs CUDA tensors: the B200 build has no CPU fallback")
+            raise _lib.WnbError("WaveNet.forward_loss needs CUDA tensors: this build has no CPU fallback")
         plan = self._stack_plan(x.device)
         if plan is None:
             return cross_entropy(self._forward_impl(x, h), t, start)
@@ -698,7 +698,7 @@ class WaveNet(nn.Module):
 
     def _forward_impl(self, x, h, upsample=True):
         if not x.is_cuda:
-            raise _lib.WnbError("WaveNet.forward needs CUDA tensors: the B200 build has no CPU fallback")
+            raise _lib.WnbError("WaveNet.forward needs CUDA tensors: this build has no CPU fallback")
         if upsample and PROFILE_EVENTS is None:
             plan = self._stack_plan(x.device)
             if plan is not None:
@@ -824,7 +824,7 @@ class WaveNet(nn.Module):
             logging.error("mode should be sampling or argmax")
             sys.exit(1)
         if not h.is_cuda:
-            raise _lib.WnbError("generation needs CUDA tensors: the B200 build has no CPU fallback")
+            raise _lib.WnbError("generation needs CUDA tensors: this build has no CPU fallback")
         dev = h.device
         B, T0 = x.shape
         n_list = [int(n) for n in n_samples_list]

@@ -2,7 +2,7 @@
 """Data-parallel plumbing: one process per GPU, NCCL over NVLink.
 
 The reference trains with single-process ``nn.DataParallel`` (bin/train.py:449-454: scatter batch,
-replicate params, gather logits on GPU 0, reduce grads).  The B200 build shards the minibatch across
+replicate params, gather logits on GPU 0, reduce grads).  This build shards the minibatch across
 ranks instead; the only exchange on the data path is ONE flat all-reduce of the gradients per step
 (8.6 MB fp32 at 64/512).  Each rank computes the mean loss over its own windows, so averaging the
 gradients reproduces DataParallel's global mean for equal per-rank batches (SURVEY.md 8e).

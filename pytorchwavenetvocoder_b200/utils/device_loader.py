@@ -2,7 +2,7 @@
 """``train_generator`` (reference bin/train.py:67-312, mini-batch modes) with the per-batch work on the GPU.
 
 The reference builds every batch on the host -- window slicing, mu-law over the whole window, StandardScaler,
-transpose, stack, three ``.cuda()`` copies per batch (train.py:157-185) -- in a Python prefetch thread.  At B200 step
+transpose, stack, three ``.cuda()`` copies per batch (train.py:157-185) -- in a Python prefetch thread.  At the step
 times (milliseconds) that thread is the wall.  Here
 
 * a loader thread only READS files (wav + feature frames) into pinned staging slots;

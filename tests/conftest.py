@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA GPU (an H100, sm_90a)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -2,11 +2,11 @@
 # -*- coding: utf-8 -*-
 """Generate the golden vectors under tests/golden/ from the LIVE reference.
 
-Run in the build container only (needs /root/reference, which does not exist on the GPU box):
+Needs a checkout of the original PytorchWaveNetVocoder (v0.1.1); the tests only read the stored vectors:
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py /path/to/PytorchWaveNetVocoder
 
-It imports ``wavenet_vocoder.nets`` from /root/reference (never copied into this repo), loads
+It imports ``wavenet_vocoder.nets`` from that checkout (never copied into this repo), loads
 seeded synthetic parameters (``oracle.wavenet_oracle.make_params``; numpy RandomState, so the
 same arrays are rebuilt bit-for-bit by the tests on any machine) into the reference modules and
 records their outputs: mu-law tables, forward logits, CE loss, every parameter gradient, and
@@ -21,7 +21,9 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference")
+if len(sys.argv) != 2:
+    sys.exit(__doc__)
+sys.path.insert(0, os.path.abspath(sys.argv[1]))
 
 from oracle import wavenet_oracle as O  # noqa: E402
 from tests.golden.cases import FORWARD_CASES, GEN_CASES, make_inputs, make_gen_inputs, mulaw_inputs, mulaw_pcm16_domain  # noqa: E402

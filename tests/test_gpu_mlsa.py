@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""B200 tier: wnb_mlsa_filter (csrc/mlsa.cu, SURVEY.md 8 row f4) against the CPU oracle (oracle/mlsa_oracle.c) -- bit exact
+"""GPU tier: wnb_mlsa_filter (csrc/mlsa.cu, SURVEY.md 8 row f4) against the CPU oracle (oracle/mlsa_oracle.c) -- bit exact
 in float64 and through the int16 wav path, ragged batches, both Pade orders, the inverse filter, a full-length batch
 (64 x 160 000 samples) checked exactly on a subset and through the shaping -> restoring round trip, and the CLI mirror
 of reference bin/noise_shaping.py end to end."""

@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""B200 tier: pytorchwavenetvocoder_b200.optim.Adam (one wnb_adam_flat launch per step) against torch.optim.Adam -- the
+"""GPU tier: pytorchwavenetvocoder_b200.optim.Adam (one wnb_adam_flat launch per step) against torch.optim.Adam -- the
 reference's optimizer (bin/train.py:457-460) -- on identical gradients, through the real training step, and through a
 checkpoint round trip in torch's own state_dict format."""
 import copy

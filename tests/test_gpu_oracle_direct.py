@@ -4,10 +4,9 @@
 * tf32 deferred-skip stack (csrc/stack.cu, the bench path) at the BASELINE configs[1] architecture
   ``WaveNet(256,28,64,512,10,3,2,80)``, B=2, T=4160 (time tiles well past the receptive field 3070): loss and
   EVERY parameter gradient vs ``oracle.backward`` in float64 (reference bin/train.py:530-538 over
-  nets/wavenet.py:212-241).  The observed error of every tensor is written to
-  ``gpurun_out/r2_parity_*.json`` (and printed) so that the asserted tolerances are the measured ones x ~2,
-  not a guess.
-* the composed tcgen05 path at the ljspeech-melspc architecture ``(256,80,512,256,10,3,3,256)`` on a short window
+  nets/wavenet.py:212-241).  The observed error of every tensor is printed (and written as parity_*.json into the
+  directory named by $WNB_PARITY_OUT, when set) so that the asserted tolerances are the measured ones x ~2, not a guess.
+* the composed tensor-core path at the ljspeech-melspc architecture ``(256,80,512,256,10,3,3,256)`` on a short window
   (reference egs/ljspeech/sd-melspc/run.sh:28-33).
 * long free-running argmax decode (>= 10 000 samples, all three kernels) vs ``oracle.batch_fast_generate`` with the
   first-divergence / top-2-margin protocol of SURVEY.md 8c-4(iii) (reference nets/wavenet.py:309-395).
@@ -24,11 +23,10 @@ from tests.util import our_model
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
 def _dump(name, obj):
-    d = os.path.join(ROOT, "gpurun_out")
+    d = os.environ.get("WNB_PARITY_OUT")
+    if not d:
+        return
     try:
         os.makedirs(d, exist_ok=True)
         with open(os.path.join(d, name), "w") as f:
@@ -135,13 +133,13 @@ def _summarise(rep):
 def test_tf32_stack_every_gradient_vs_fp64_oracle_arctic30():
     """The bench path: 30 blocks, 64 res / 512 skip, kernel 2, U = 80; all 184 gradient tensors vs the fp64 oracle.
 
-    Tolerances (asserted) = about twice the error observed on B200 (profiles/r2_parity_stack_arctic_tf32.json):
+    Tolerances (asserted) = about twice the error observed (see the note above TOL_TF32):
     tf32 rounds both operands of every contraction to 10 mantissa bits (2^-11 relative), the gate uses
     tanh.approx.f32 (2^-10.987 max relative error); the gradients at the bottom of the stack carry the rounding of
     every block above them."""
     cfg = O.Config(256, 28, 64, 512, 10, 3, 2, 80)
     rep = _summarise(_train_step_vs_oracle(cfg, 3, 2, 4160, cfg.receptive_field, "tf32", True))
-    _dump("r2_parity_stack_arctic_tf32.json", rep)
+    _dump("parity_stack_arctic_tf32.json", rep)
     print("tf32 stack vs fp64 oracle: loss err %.2e, logits max err %.2e, worst weight %s %.3e, worst bias %s %.3e"
           % (rep["loss_abs_err"], rep["logits_max_abs_err"], rep["worst_weight"][0], rep["worst_weight"][1],
              rep["worst_bias"][0], rep["worst_bias"][1]))
@@ -166,7 +164,7 @@ def test_fp32_path_every_gradient_vs_fp64_oracle_arctic30():
     """Same comparison for math_mode="fp32" (FFMA kernels): the parity path, errors at fp32 rounding level."""
     cfg = O.Config(256, 28, 64, 512, 10, 3, 2, 80)
     rep = _summarise(_train_step_vs_oracle(cfg, 3, 2, 4160, cfg.receptive_field, "fp32", None))
-    _dump("r2_parity_stack_arctic_fp32.json", rep)
+    _dump("parity_stack_arctic_fp32.json", rep)
     print("fp32 path vs fp64 oracle: loss err %.2e, logits max err %.2e, worst weight %s %.3e, worst bias %s %.3e"
           % (rep["loss_abs_err"], rep["logits_max_abs_err"], rep["worst_weight"][0], rep["worst_weight"][1],
              rep["worst_bias"][0], rep["worst_bias"][1]))
@@ -180,10 +178,10 @@ def test_fp32_path_every_gradient_vs_fp64_oracle_arctic30():
 
 def test_composed_tf32_path_vs_fp64_oracle_ljspeech_melspc():
     """configs[2] architecture (512 res / 256 skip, kernel 3, 80-dim mel aux, U = 256) on a short window: the
-    composed tcgen05 path (per-block GEMMs) vs the fp64 oracle, loss + every gradient."""
+    composed tensor-core path (per-block GEMMs) vs the fp64 oracle, loss + every gradient."""
     cfg = O.Config(256, 80, 512, 256, 10, 3, 3, 256)
     rep = _summarise(_train_step_vs_oracle(cfg, 5, 1, 768, 128, "tf32", False))
-    _dump("r2_parity_composed_ljspeech_tf32.json", rep)
+    _dump("parity_composed_ljspeech_tf32.json", rep)
     print("composed tf32 vs fp64 oracle: loss err %.2e, logits max err %.2e, worst weight %s %.3e, worst bias %s %.3e"
           % (rep["loss_abs_err"], rep["logits_max_abs_err"], rep["worst_weight"][0], rep["worst_weight"][1],
              rep["worst_bias"][0], rep["worst_bias"][1]))
@@ -196,14 +194,13 @@ def test_composed_tf32_path_vs_fp64_oracle_ljspeech_melspc():
         assert v["rel_fro"] <= tol, (k, v)
 
 
-# Asserted tolerances: ~2x the errors observed on B200 (see profiles/r2_parity_*.json for the per-tensor numbers)
-# Observed (B200, round 2): loss 1.1e-3, logits 1.4e-2 (max |logit| 3.2), every weight gradient 4.5-5.7 %, biases
-# 2.6-6.1 % -- UNIFORM over the 30 blocks and already 2.5 % at conv_post_1: it is not rounding accumulated through the
-# stack but the two ReLU masks of the post network flipping where a pre-activation is within tf32 rounding of zero.
+# Asserted tolerances: ~2x the errors observed.  Observed on an H100: loss 1.1e-3, logits 1.4e-2 (max |logit| 3.2),
+# weight gradients up to 5.7 %, biases up to 6.5 % -- already 2.5 % at conv_post_1: it is not rounding accumulated through
+# the stack but the two ReLU masks of the post network flipping where a pre-activation is within tf32 rounding of zero.
 # With the masks shared the same gradients agree to the second set of bounds.
 TOL_TF32 = {"loss": 2.5e-3, "logits": 3e-2, "weight": 0.08, "bias": 0.09}
-# observed with shared masks: weights 0.35-0.90 % (growing gently from the top block to the bottom one: tf32 rounding
-# accumulated through the stack), biases <= 0.82 %; mask flip fraction 7e-4 per ReLU
+# observed with shared masks: weights 0.35-0.90 % (tf32 rounding accumulated through the stack), biases <= 0.85 %; mask
+# flip fraction 7e-4 per ReLU
 TOL_TF32_SAME_MASKS = {"weight": 0.018, "bias": 0.018}
 # composed path at the ljspeech-melspc shape (observed: loss 5.1e-3, logits 2.4e-2 at max |logit| 5.3, weights <= 5.2 %,
 # biases <= 2.8 %; the same ReLU-mask effect, K = 512..1616 contractions)
@@ -238,7 +235,7 @@ def test_decode_long_run_first_divergence_protocol(kernel):
         rep.append({"utt": b, "identical": False, "first_divergence": i, "oracle_margin_there": float(ref["margin"][b, i]),
                     "ours": int(gen[b, i]), "oracle": int(ref["samples"][b, i]),
                     "oracle_top2": [int(v) for v in ref["top2"][b, i]]})
-    _dump("r2_decode_long_run_%s.json" % kernel, rep)
+    _dump("decode_long_run_%s.json" % kernel, rep)
     print("decode long run (%s): %s" % (kernel, rep))
     for r in rep:
         if not r["identical"]:

@@ -18,7 +18,7 @@ def test_two_streams_two_threads_concurrent_forward():
     cfg = O.Config(256, 28, 64, 512, 6, 2, 2, 16)
     nets = [our_model(cfg, O.make_params(cfg, 30 + i), math_mode="tf32").eval() for i in range(2)]
     rng = np.random.RandomState(0)
-    B, T = 4, 8192           # 256 tiles per launch > 148 SMs: the dynamic scheduler is exercised
+    B, T = 4, 8192           # more tiles per launch than SMs: the dynamic scheduler is exercised
     xs = [torch.from_numpy(rng.randint(0, 256, size=(B, T)).astype(np.int64)).cuda() for _ in range(2)]
     hs = [torch.from_numpy(rng.standard_normal((B, 28, T // 16)).astype(np.float32)).cuda() for _ in range(2)]
     with torch.no_grad():

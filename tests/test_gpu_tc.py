@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""GPU tier: the tcgen05/TMA fused residual-block kernel (math_mode="tf32") against the fp32 FFMA kernel
+"""GPU tier: the wgmma/TMA tensor-core residual-block paths (math_mode="tf32") against the fp32 FFMA kernel
 and the fp64 oracle.
 
 Stated tolerance for the tf32 path (tf32 multiplies = 10-bit mantissa operands, fp32 accumulate,
@@ -105,7 +105,7 @@ def test_training_step_tf32_close_to_fp32():
 
 
 def test_block_backward_tf32_vs_fp32_single_layer():
-    """wnb_resblock_bwd in tf32 mode (tcgen05 weight gradients) vs the all-FFMA path, one block."""
+    """wnb_resblock_bwd in tf32 mode (tensor-core weight gradients) vs the all-FFMA path, one block."""
     from pytorchwavenetvocoder_b200 import _lib
     lib = _lib.load()
     torch.manual_seed(5)
@@ -226,7 +226,7 @@ def test_composed_block_fwd_bwd_tf32_vs_fp32(R, S, Ap, ks, d, T, last, init):
 
 
 def test_composed_full_model_step_tf32_vs_fp32():
-    """ljspeech-like small model (80-dim aux, kernel_size 3, R=128/S=64): tf32 (composed tcgen05 path) vs fp32."""
+    """ljspeech-like small model (80-dim aux, kernel_size 3, R=128/S=64): tf32 (composed tensor-core path) vs fp32."""
     from pytorchwavenetvocoder_b200.nets import cross_entropy
     from pytorchwavenetvocoder_b200.nets.wavenet import tc_supported
     cfg_t = (256, 80, 128, 64, 4, 2, 3, 8)

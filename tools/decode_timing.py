@@ -1,4 +1,4 @@
-"""Debug helper: per-phase cycle breakdown of the warp-tiled decode kernel (run on the GPU box)."""
+"""Debug helper: per-phase cycle breakdown of the warp-tiled decode kernel (needs a GPU)."""
 import sys, ctypes, torch, numpy as np
 sys.path.insert(0, '.'); sys.path.insert(0, '..')
 from bench import make_model
