@@ -109,6 +109,13 @@ WNB_API int wnb_stack_fwd(float* xs, int nxs, const float* haux, const float* w1
 // dpre / dx of ALL blocks are kept so that the weight gradients dW1_l, dW2res_l of the whole stack are two launches at
 // the end instead of 2L small ones inside the block loop (each of those spent a third of its time on launch, set-up
 // and the atomic flush).
+// On return wnb_stack_bwd leaves in it, in this order (floats):
+//   dZ_all    B*T*L*R      dskip Wskip; columns l*R .. l*R+R-1 are block l's skip part of dz
+//   slack     L*R          never written
+//   dpre      L*B*T*2R     block l: [d pre-sigmoid | d pre-tanh] of its gate, the A operand of dW1_l
+//   dx        L*B*T*R      block l >= 1: gradient of xs[l] (block l-1's dout, the A operand of dW2res_{l-1});
+//                          slot 0 is never written (block 0's goes to dx0)
+// tests/test_gpu_tc_stages.py reads these to check every stage from the kernels' own inputs.
 WNB_API size_t wnb_stack_bwd_workspace(int L, int B, int T, int R, int S, int Ap, int ks) {
   (void)S; (void)Ap; (void)ks;
   const size_t bt = (size_t)B * T;

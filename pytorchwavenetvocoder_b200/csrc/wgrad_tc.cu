@@ -317,12 +317,20 @@ int wgrad_tc_blocks(const WgBlock* blocks, int nblocks, const WgOperand* b_ops, 
   p.ldc = ldc;
   p.n_split = (opts && opts->n_split > 1) ? opts->n_split : 1;
   p.nseg = (opts && opts->nseg > 1) ? opts->nseg : 1;
-  if (p.nseg > 1) {
-    if (p.nseg > kMaxSeg || p.n_split > 1 || !opts->seg_shift) {
-      set_error("wgrad_tc: bad segment configuration (nseg=%d)", p.nseg);
-      return WNB_ERR_INVALID;
-    }
+  if (p.nseg > 1 && (p.nseg > kMaxSeg || p.n_split > 1 || !opts->seg_shift)) {
+    set_error("wgrad_tc: bad segment configuration (nseg=%d)", p.nseg);
+    return WNB_ERR_INVALID;
+  }
+  // a WG_SEG_SHIFT operand takes its shift from the table also when there is one segment (a one-block stack)
+  bool seg_shift_used = false;
+  for (int i = 0; i < p.nops; i++) seg_shift_used |= (p.ops[i].flags & WG_SEG_SHIFT) != 0;
+  if (seg_shift_used && !(opts && opts->seg_shift)) {
+    set_error("wgrad_tc: a segment-shifted operand needs WgOpts::seg_shift");
+    return WNB_ERR_INVALID;
+  }
+  if (opts && opts->seg_shift)
     for (int i = 0; i < p.nseg; i++) p.seg_shift[i] = opts->seg_shift[i];
+  if (p.nseg > 1) {
     p.c_seg_stride = opts->c_seg_stride;
     p.db_seg_stride = opts->db_seg_stride;
   }
