@@ -51,6 +51,12 @@ extern "C" {
 
 #define WNB_MATH_FP32 0        /* SIMT FFMA, fp32 throughout (parity mode) */
 #define WNB_MATH_TF32 1        /* wgmma tf32 contractions, fp32 accumulate */
+/* wgmma bf16 contractions: both operands of every product rounded to bf16 (nearest even), fp32 accumulate; activations,
+ * weights and gradients stay fp32 in memory (the weights a call uses are rounded into a library scratch per call).
+ * Covered: wnb_resblock_fwd / wnb_resblock_bwd on the composed path's shapes (wnb_resblock_fwd_supported() == 2) and
+ * wnb_post_fwd / wnb_post_bwd with S, Q multiples of 32 up to 256 (or 512); any other shape is an error.  The
+ * deferred-skip stack and the fused per-block kernels are tf32 only. */
+#define WNB_MATH_BF16 2
 
 #define WNB_MODE_ARGMAX 0
 #define WNB_MODE_SAMPLING 1
@@ -97,7 +103,8 @@ WNB_API int wnb_resblock_fwd(const float* xin, const float* haux, const float* w
                      int math_mode, void* stream);
 
 /* tf32: 1 = fused per-block kernel (no zsave), 2 = composed tensor-core path (zsave optional), 0 = not covered;
-   fp32: 1 = covered, 0 = not */
+   bf16: 2 = composed tensor-core path (zsave optional), 0 = not covered; fp32: 1 = covered, 0 = not;
+   an unknown math_mode: 0 */
 WNB_API int wnb_resblock_fwd_supported(int R, int S, int Ap, int ks, int math_mode);
 
 /* ---- a5 standalone: CausalConv1d.forward (wavenet.py:95-121), channels-last, fp32 FFMA, forward only.
@@ -188,7 +195,8 @@ WNB_API int wnb_profile_read(int kind, double* total_ms, int* launches);
  *     skip = [z_0 | ... | z_{L-1}] Wskip^T + bskip,   Wskip[s][l*R+c] = skip_1x1_l.weight[s][c],  bskip = sum_l skip bias_l
  * so a block only writes z_l into Z_all (B,T,L*R) and its residual output (no read-modify-write of skip per block),
  * and the backward hoists dZ_all = dskip Wskip and dWskip = dskip^T Z_all out of the block loop the same way.
- * WNB_MATH_TF32 only; wnb_stack_supported() says whether the shape is covered (else use the per-block entries). */
+ * WNB_MATH_TF32 only (0 for any other math_mode); wnb_stack_supported() says whether the shape is covered (else use the
+ * per-block entries). */
 WNB_API int wnb_stack_supported(int R, int S, int Ap, int ks, int L, int math_mode);
 
 /* one block: xout (B,T,R) = xin + res_1x1(z) (NULL for the last block), z -> zall[:, :, zcol0:zcol0+R] (row pitch ldz).

@@ -15,6 +15,7 @@ LIB_PATH = os.path.join(_HERE, "libwnb200.so")
 
 MATH_FP32 = 0
 MATH_TF32 = 1
+MATH_BF16 = 2
 MODE_ARGMAX = 0
 MODE_SAMPLING = 1
 

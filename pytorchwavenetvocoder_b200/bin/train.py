@@ -7,7 +7,7 @@ Same command line (reference train.py:337-394), same ``model.conf`` / ``checkpoi
 What changes underneath: ``WaveNet`` is the sm_90a kernel build, the loss is the fused CE kernel, and
 ``--n_gpus N`` means N *processes* (the command re-launches itself under ``torch.distributed.run``; one rank per
 GPU, a single flat NCCL all-reduce of the gradients per step) instead of single-process ``nn.DataParallel``
-(:449-454).  ``--batch_size`` stays the GLOBAL batch: every rank trains on ``batch_size / n_gpus`` windows of it.  Extra, optional flags: ``--math_mode {tf32,fp32}``.
+(:449-454).  ``--batch_size`` stays the GLOBAL batch: every rank trains on ``batch_size / n_gpus`` windows of it.  Extra, optional flags: ``--math_mode {tf32,fp32,bf16}``.
 """
 from __future__ import division
 
@@ -205,8 +205,10 @@ def get_parser():
     parser.add_argument("--resume", default=None, nargs="?", type=str, help="model path to restart training")
     parser.add_argument("--n_gpus", default=1, type=int, help="number of gpus")
     parser.add_argument("--verbose", default=1, type=int, help="log level")
-    parser.add_argument("--math_mode", default="tf32", choices=["tf32", "fp32"], type=str,
-                        help="(H100 build) contraction precision of the training kernels")
+    parser.add_argument("--math_mode", default="tf32", choices=["tf32", "fp32", "bf16"], type=str,
+                        help="(H100 build) contraction precision of the training kernels; bf16 rounds the operands of "
+                             "every product to bf16 (fp32 accumulation and storage) and needs a shape the composed "
+                             "tensor-core path covers")
     parser.add_argument("--host_loader", default=False, type=_strtobool,
                         help="(H100 build) build the mini-batches on the host like the reference instead of on the GPU")
     return parser
@@ -286,10 +288,19 @@ def main():
     logging.info(model)
     model.apply(initialize)
     model.train()
-    from pytorchwavenetvocoder_b200.nets.wavenet import tc_supported
+    from pytorchwavenetvocoder_b200.nets.wavenet import bf16_supported, tc_supported
     cfg_t = (args.n_quantize, args.n_aux, args.n_resch, args.n_skipch, args.dilation_depth, args.dilation_repeat,
              args.kernel_size, upsampling_factor)
-    model.math_mode = args.math_mode if (args.math_mode == "fp32" or tc_supported(cfg_t)) else "fp32"
+    if args.math_mode == "bf16":
+        if not bf16_supported(cfg_t):   # asked for explicitly: an error, not a quiet change of precision
+            logging.error("--math_mode bf16 does not cover n_resch=%d n_skipch=%d n_aux=%d kernel_size=%d n_quantize=%d "
+                          "(needs n_resch a multiple of 64, n_skipch / n_quantize multiples of 32 up to 256 or 512, "
+                          "n_aux <= 256, kernel_size <= 3); use --math_mode tf32 or fp32"
+                          % (args.n_resch, args.n_skipch, args.n_aux, args.kernel_size, args.n_quantize))
+            sys.exit(1)
+        model.math_mode = "bf16"
+    else:
+        model.math_mode = args.math_mode if (args.math_mode == "fp32" or tc_supported(cfg_t)) else "fp32"
     logging.info("math_mode = %s" % model.math_mode)
 
     model.cuda()   # before the optimizer: the fused (single multi-tensor kernel) Adam needs CUDA parameters

@@ -4,6 +4,10 @@
 // causal / anti-causal padding), W is a row-major [N][K] weight matrix (K-major operand).  Hopper wgmma
 // m64nNk8 tf32, fp32 accumulate in registers of one consumer warpgroup; one producer warp streams
 // [64 x 32] activation boxes and [N x 32] weight boxes through an mbarrier ring with TMA.
+// bf16 operands (W = __nv_bfloat16): the weights arrive as bf16 [N x 32] boxes (a bf16 copy made by the caller, 64B
+// swizzle); the activation box is still fp32, and the consumers read two adjacent k per shared-memory load, round them
+// to bf16 (cvt.rn.bf16x2) into the register A fragment of wgmma m64nNk16 (bf16, fp32 accumulate).  The epilogues are
+// the same: the accumulator is fp32 either way.
 // Epilogue: the accumulator is written to shared memory column-major, then each consumer thread owns one time row
 // and 32-column chunks (warp w: rows 32 (w & 1) .., chunks w >> 1, (w >> 1) + 2, ...): + bias, ReLU, * (mask > 0),
 // + residual, then a swizzled per-warp staging box and a TMA store or TMA reduce-add (.add.f32) into the (B,T,N)
@@ -16,6 +20,9 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+
+#include <cuda_bf16.h>
+#include <type_traits>
 
 #include "common.cuh"
 #include "tc_host.h"
@@ -69,11 +76,18 @@ __device__ __forceinline__ void acc_ld16(const float* acc, int col, int row, flo
   for (int i = 0; i < 16; i++) v[i] = acc[(col + i) * kAccLd + row];
 }
 
-template <int N, int EPI>
+// bytes of one weight row of a stage (32 k): fp32 (read as tf32) or bf16
+template <typename W>
+__host__ __device__ constexpr int w_row_bytes() { return std::is_same<W, __nv_bfloat16>::value ? 64 : 128; }
+
+// W: element type of the weight operand, float (the tensor cores read it as tf32) or __nv_bfloat16
+template <int N, int EPI, typename W>
 __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_constant__ Params p) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr int stage_bytes = kASub + N * 128;
+  constexpr bool kBf16 = std::is_same<W, __nv_bfloat16>::value;
+  constexpr int kWRow = w_row_bytes<W>();
+  constexpr int stage_bytes = kASub + N * kWRow;
   unsigned char* ring = smem;
   float* accs = reinterpret_cast<float*>(ring + (size_t)p.nstages * stage_bytes);
   unsigned char* stg_base = reinterpret_cast<unsigned char*>(accs) + acc_bytes(N);
@@ -117,7 +131,7 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
             ptx::tma_load_3d(dst, &p.maps[sg.amap], &full[st], kc * 32, t0 + sg.shift, b);
             if (sg.b_n1 >= 0) {   // N = two row ranges of N/2 each (sigmoid rows, tanh rows)
               ptx::tma_load_2d(dst + kASub, &p.maps[sg.bmap], &full[st], sg.b_k0 + kc * 32, sg.b_n0);
-              ptx::tma_load_2d(dst + kASub + (N / 2) * 128, &p.maps[sg.bmap], &full[st], sg.b_k0 + kc * 32, sg.b_n1);
+              ptx::tma_load_2d(dst + kASub + (N / 2) * kWRow, &p.maps[sg.bmap], &full[st], sg.b_k0 + kc * 32, sg.b_n1);
             } else {
               ptx::tma_load_2d(dst + kASub, &p.maps[sg.bmap], &full[st], sg.b_k0 + kc * 32, sg.b_n0 + ncol0);
             }
@@ -144,18 +158,49 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
 #pragma unroll
     for (int i = 0; i < N / 2; i++) d[i] = 0.f;
     uint32_t prev = 0xFFFFFFFFu;
-    for (int kc = 0; kc < kchunks; kc++) {
-      ptx::mbar_wait(&full[st], ph);
-      ptx::wg_fence();
-      const uint32_t a_addr = ring_u32 + st * stage_bytes, b_addr = a_addr + kASub;
+    if constexpr (!kBf16) {
+      for (int kc = 0; kc < kchunks; kc++) {
+        ptx::mbar_wait(&full[st], ph);
+        ptx::wg_fence();
+        const uint32_t a_addr = ring_u32 + st * stage_bytes, b_addr = a_addr + kASub;
 #pragma unroll
-      for (int k = 0; k < 4; k++)
-        ptx::wgmma_ss<N>(d, ptx::gmma_desc_k_sw128(a_addr + 32 * k), ptx::gmma_desc_k_sw128(b_addr + 32 * k), 1);
-      ptx::wg_commit();
-      ptx::wg_wait<1>();                   // the previous chunk's MMAs are done: its stage can be refilled
-      if (prev != 0xFFFFFFFFu) ptx::mbar_arrive(&empty[prev]);
-      prev = st;
-      if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
+        for (int k = 0; k < 4; k++)
+          ptx::wgmma_ss<N>(d, ptx::gmma_desc_k_sw128(a_addr + 32 * k), ptx::gmma_desc_k_sw128(b_addr + 32 * k), 1);
+        ptx::wg_commit();
+        ptx::wg_wait<1>();                   // the previous chunk's MMAs are done: its stage can be refilled
+        if (prev != 0xFFFFFFFFu) ptx::mbar_arrive(&empty[prev]);
+        prev = st;
+        if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
+      }
+    } else {
+      // A fragments (rows 16 warp + lane/4 (+ 8), k pairs 2 (lane % 4) (+ 8)) converted from the fp32 box into one of two
+      // register sets: wgmma reads them asynchronously, so a set is refilled only after the chunk that used it is done
+      const int fr = 16 * warp + (lane >> 2), fk = 2 * (lane & 3);
+      uint32_t a0[2][4], a1[2][4];
+      auto chunk = [&](uint32_t (&a)[2][4]) {
+        ptx::mbar_wait(&full[st], ph);
+        const unsigned char* as = ring + (size_t)st * stage_bytes;
+#pragma unroll
+        for (int k = 0; k < 2; k++)
+#pragma unroll
+          for (int h = 0; h < 4; h++) {
+            const float2 v = *reinterpret_cast<const float2*>(as + ptx::sw128_off(fr + 8 * (h & 1), 16 * k + fk + 8 * (h >> 1)));
+            a[k][h] = ptx::cvt_bf16x2(v.x, v.y);
+          }
+        ptx::wg_fence();
+        const uint32_t b_addr = ring_u32 + st * stage_bytes + kASub;
+#pragma unroll
+        for (int k = 0; k < 2; k++) ptx::wgmma_rs_bf16<N>(d, a[k], ptx::gmma_desc_k_sw64(b_addr + 32 * k), 1);
+        ptx::wg_commit();
+        ptx::wg_wait<1>();                 // the previous chunk's MMAs are done: its stage can be refilled
+        if (prev != 0xFFFFFFFFu) ptx::mbar_arrive(&empty[prev]);
+        prev = st;
+        if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
+      };
+      for (int kc = 0; kc < kchunks; kc += 2) {
+        chunk(a0);
+        if (kc + 1 < kchunks) chunk(a1);
+      }
     }
     ptx::wg_wait<0>();
     ptx::wg_touch(d);
@@ -390,25 +435,36 @@ static bool map2(CUtensorMap* m, const float* base, int K, int Nrows, int box_ro
              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
-
-template <int N, int EPI>
-static cudaError_t launch_n(int grid, size_t smem, cudaStream_t st, const Params& p) {
-  cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(gemm_nt_tc_kernel<N, EPI>), smem);
-  if (e != cudaSuccess) return e;
-  return launch_pdl(gemm_nt_tc_kernel<N, EPI>, grid, kThreadsN, smem, st, p);
+// the bf16 weight matrix: [box_rows x 32] boxes of 64-byte rows, 64B swizzle (the layout gmma_desc_k_sw64 describes)
+static bool map2_bf16(CUtensorMap* m, const __nv_bfloat16* base, int K, int Nrows, int box_rows) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) return false;
+  cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)Nrows};
+  cuuint64_t gstr[1] = {(cuuint64_t)K * 2};
+  cuuint32_t box[2] = {32, (cuuint32_t)box_rows}, es[2] = {1, 1};
+  return enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<__nv_bfloat16*>(base), gdim, gstr, box, es,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int EPI>
+template <int N, int EPI, typename W>
+static cudaError_t launch_n(int grid, size_t smem, cudaStream_t st, const Params& p) {
+  cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(gemm_nt_tc_kernel<N, EPI, W>), smem);
+  if (e != cudaSuccess) return e;
+  return launch_pdl(gemm_nt_tc_kernel<N, EPI, W>, grid, kThreadsN, smem, st, p);
+}
+
+template <int EPI, typename W>
 static cudaError_t launch_epi(int N, int grid, size_t smem, cudaStream_t st, const Params& p) {
   switch (N) {
-    case 32: return launch_n<32, EPI>(grid, smem, st, p);
-    case 64: return launch_n<64, EPI>(grid, smem, st, p);
-    case 96: return launch_n<96, EPI>(grid, smem, st, p);
-    case 128: return launch_n<128, EPI>(grid, smem, st, p);
-    case 160: return launch_n<160, EPI>(grid, smem, st, p);
-    case 192: return launch_n<192, EPI>(grid, smem, st, p);
-    case 224: return launch_n<224, EPI>(grid, smem, st, p);
-    default: return launch_n<256, EPI>(grid, smem, st, p);
+    case 32: return launch_n<32, EPI, W>(grid, smem, st, p);
+    case 64: return launch_n<64, EPI, W>(grid, smem, st, p);
+    case 96: return launch_n<96, EPI, W>(grid, smem, st, p);
+    case 128: return launch_n<128, EPI, W>(grid, smem, st, p);
+    case 160: return launch_n<160, EPI, W>(grid, smem, st, p);
+    case 192: return launch_n<192, EPI, W>(grid, smem, st, p);
+    case 224: return launch_n<224, EPI, W>(grid, smem, st, p);
+    default: return launch_n<256, EPI, W>(grid, smem, st, p);
   }
 }
 
@@ -435,10 +491,20 @@ int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, con
     p.nblk = 2;
   }
   const int nbox = gate ? N / 2 : N;   // (gate: two boxes of GC = N/2 rows, sigmoid rows and tanh rows)
+  const bool bf16 = segs[0].wb != nullptr;
   for (int s = 0; s < nseg; s++) {
     if (segs[s].K % 32 != 0) { set_error("gemm_nt_tc: K must be a multiple of 32"); return WNB_ERR_INVALID; }
+    if ((segs[s].wb != nullptr) != bf16) {
+      set_error("gemm_nt_tc: either every segment or none has a bf16 weight copy");
+      return WNB_ERR_INVALID;
+    }
+    if (bf16 && (segs[s].w_cols % 8 != 0 || (reinterpret_cast<uintptr_t>(segs[s].wb) & 15))) {
+      set_error("gemm_nt_tc: a bf16 weight matrix needs a row pitch of 8k elements and a 16-byte aligned base");
+      return WNB_ERR_INVALID;
+    }
     if (!map3(&p.maps[s], segs[s].a, segs[s].CA, T, B, kTM) ||
-        !map2(&p.maps[4 + s], segs[s].w, segs[s].w_cols, segs[s].w_rows, nbox)) {
+        !(bf16 ? map2_bf16(&p.maps[4 + s], segs[s].wb, segs[s].w_cols, segs[s].w_rows, nbox)
+               : map2(&p.maps[4 + s], segs[s].w, segs[s].w_cols, segs[s].w_rows, nbox))) {
       set_error("gemm_nt_tc: tensor map creation failed");
       return WNB_ERR_CUDA;
     }
@@ -497,7 +563,7 @@ int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, con
   }
   // shared memory: ring stages (A box + weight box) | accumulator copy | 4 warps x 2 staging boxes | barriers.  When three
   // stages fit in half of the SM, two CTAs share it and one's epilogue overlaps the other's mainloop.
-  const int stage_bytes = kASub + N * 128;
+  const int stage_bytes = kASub + N * (bf16 ? w_row_bytes<__nv_bfloat16>() : w_row_bytes<float>());
   const int fixed = acc_bytes(N) + 4 * 2 * kStg + 1024 + 256;
   const int sm_bytes = 227 * 1024, half = 113 * 1024;
   const int ctas = fixed + 3 * stage_bytes <= half ? 2 : 1;
@@ -510,9 +576,13 @@ int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, con
   const int ntiles = B * ((T + kTM - 1) / kTM) * p.nblk;
   const int grid = ntiles < sms * ctas ? ntiles : sms * ctas;
   cudaError_t le;
-  if (epi == EPI_PLAIN) le = launch_epi<EPI_PLAIN>(N, grid, smem, st, p);
-  else if (epi == EPI_GATE) le = launch_epi<EPI_GATE>(N, grid, smem, st, p);
-  else le = launch_epi<EPI_GATE_BWD_NOZ>(N, grid, smem, st, p);
+  if (bf16) {   // (the gate backward without z belongs to the tf32 stack only)
+    if (epi == EPI_PLAIN) le = launch_epi<EPI_PLAIN, __nv_bfloat16>(N, grid, smem, st, p);
+    else if (epi == EPI_GATE) le = launch_epi<EPI_GATE, __nv_bfloat16>(N, grid, smem, st, p);
+    else { set_error("gemm_nt_tc: no bf16 variant of the gate backward without z"); return WNB_ERR_INVALID; }
+  } else if (epi == EPI_PLAIN) le = launch_epi<EPI_PLAIN, float>(N, grid, smem, st, p);
+  else if (epi == EPI_GATE) le = launch_epi<EPI_GATE, float>(N, grid, smem, st, p);
+  else le = launch_epi<EPI_GATE_BWD_NOZ, float>(N, grid, smem, st, p);
   if (le != cudaSuccess) { set_error("gemm_nt_tc: launch failed: %s", cudaGetErrorString(le)); return WNB_ERR_CUDA; }
   WNB_CHECK_LAUNCH("gemm_nt_tc");
   return WNB_OK;

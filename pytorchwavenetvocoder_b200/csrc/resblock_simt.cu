@@ -14,6 +14,9 @@
 // the fallback for shapes the tensor-core paths do not cover.
 #include <stdlib.h>
 
+#include <initializer_list>
+#include <utility>
+
 #include "gemm_simt.cuh"
 #include "tc_host.h"
 
@@ -369,6 +372,63 @@ __global__ void relu_inplace_kernel(float4* __restrict__ x, int64_t n4) {
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// bf16 operand path (WNB_MATH_BF16): the weights an entry call multiplies with, rounded to bf16
+// ------------------------------------------------------------------------------------------------
+// The ABI keeps fp32 master weights.  A bf16 entry call first rounds the matrices it uses (nearest even) into the
+// per-stream SCRATCH_BF16 buffer with ONE launch; every copy starts on a 256-byte boundary.  The copies are rewritten by
+// the next bf16 call on the same stream, which is ordered after every kernel of this one.
+constexpr int kMaxBf16Mats = 4;
+struct Bf16Job { const float* src[kMaxBf16Mats]; __nv_bfloat16* dst[kMaxBf16Mats]; int64_t n[kMaxBf16Mats]; int count; };
+
+__global__ void to_bf16_kernel(const __grid_constant__ Bf16Job j) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int m = 0; m < j.count; m++)
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < j.n[m]; i += stride)
+      j.dst[m][i] = __float2bfloat16_rn(j.src[m][i]);
+}
+
+// fp32 matrix -> its bf16 copy, looked up by the fp32 pointer the GEMM segments carry
+struct Bf16Weights {
+  const float* src[kMaxBf16Mats] = {};
+  const __nv_bfloat16* dst[kMaxBf16Mats] = {};
+  int count = 0;
+  const __nv_bfloat16* of(const float* w) const {
+    for (int i = 0; i < count; i++)
+      if (src[i] == w) return dst[i];
+    return nullptr;
+  }
+  // the segments' bf16 weights (no-op for a null table: the tf32 path)
+  static void apply(const Bf16Weights* bw, NtTcSeg* segs, int n) {
+    if (bw)
+      for (int i = 0; i < n; i++) segs[i].wb = bw->of(segs[i].w);
+  }
+};
+
+// mats: (fp32 matrix, element count)
+static int to_bf16_weights(Bf16Weights& bw, std::initializer_list<std::pair<const float*, int64_t>> mats, cudaStream_t st) {
+  Bf16Job j{};
+  size_t off[kMaxBf16Mats], bytes = 0;
+  for (const auto& m : mats) {
+    off[j.count] = bytes;
+    bytes += ((size_t)m.second * sizeof(__nv_bfloat16) + 255) & ~(size_t)255;
+    j.src[j.count] = m.first;
+    j.n[j.count] = m.second;
+    j.count++;
+  }
+  unsigned char* base = static_cast<unsigned char*>(scratch_buffer(st, SCRATCH_BF16, bytes));
+  if (!base) { set_error("bf16: cannot allocate the weight scratch"); return WNB_ERR_CUDA; }
+  bw.count = j.count;
+  for (int i = 0; i < j.count; i++) {
+    j.dst[i] = reinterpret_cast<__nv_bfloat16*>(base + off[i]);
+    bw.src[i] = j.src[i];
+    bw.dst[i] = j.dst[i];
+  }
+  to_bf16_kernel<<<device_sms() * 4, 256, 0, st>>>(j);
+  WNB_CHECK_LAUNCH("to_bf16");
+  return WNB_OK;
+}
+
 // weight gradient C (M x N) += A^T B for arbitrary M (blocks of 128 rows, TMA zero fill past the tensor) and
 // N (chunks of <= 7 groups of 32), optional bias gradient db (M) = column sums of A
 static int wgrad_tc_full(const float* a, int CA, int M, const float* b, int CB, int N, float* c, int ldc, float* db,
@@ -420,7 +480,7 @@ static int wgrad_tc_split(const float* a, int CA, int M, const float* b, int CB,
 // B = channels [0, N) of tensor b (CB channels) read at time t + shift:  C (M x N, ldc) += A^T B, db (M) += colsum A.
 // M-blocks of 128 rows are batched per launch (up to 5); N goes in chunks of <= 224 columns.
 static int wgrad_tc_concat(const float* a0, int C0, const float* a1, int C1, int M, const float* b, int CB, int N,
-                           int shift, float* c, int ldc, float* db, int B, int T, cudaStream_t st) {
+                           int shift, float* c, int ldc, float* db, int B, int T, cudaStream_t st, bool bf16 = false) {
   // The N axis is split into column groups handled by different CTAs of ONE launch (WgOpts::n_split, as wgrad_tc_split
   // does): every launch then streams its M-blocks of A once and B once, with the B columns shared through L2 -- instead
   // of one launch per (<= 224-column chunk) x (M-block pair) that re-reads the A tensor for every chunk (the recipes'
@@ -439,7 +499,8 @@ static int wgrad_tc_concat(const float* a0, int C0, const float* a1, int C1, int
   }
   const int n_split = groups / nB;
   const WgOperand bo[1] = {{b, CB, 0, nB, shift}};
-  const WgOpts o{n_split};
+  WgOpts o{n_split};
+  o.bf16 = bf16 ? 1 : 0;
   WgBlock blk[5];
   int nblk = 0;
   for (int m0 = 0; m0 < M; m0 += 128) {
@@ -461,7 +522,8 @@ static int wgrad_tc_concat(const float* a0, int C0, const float* a1, int C1, int
       bk.ops[1] = WgOperand{a1, C1, 0, 4 - g0, 0};
     }
     if (++nblk == per_launch || m0 + 128 >= M) {
-      if ((rc = wgrad_tc_blocks(blk, nblk, bo, 1, ldc, B, T, st, n_split > 1 ? &o : nullptr)) != WNB_OK) return rc;
+      if ((rc = wgrad_tc_blocks(blk, nblk, bo, 1, ldc, B, T, st, (n_split > 1 || bf16) ? &o : nullptr)) != WNB_OK)
+        return rc;
       nblk = 0;
     }
   }
@@ -483,13 +545,15 @@ static NtTcOpts plain_opts(int N) {
 
 // Forward of one residual block for shapes outside the fused kernel: R/64 gate GEMMs (N = 128: 64 sigmoid + 64
 // tanh rows of W1, K = ks*R + Ap streamed) with the gate epilogue writing z, then the res GEMM (+bias, +x) and the
-// skip GEMM (+bias, store or reduce-add).  z (B,T,R) goes through p.zsave.
-static int resblock_fwd_composed(const FwdParams& p, cudaStream_t st) {
+// skip GEMM (+bias, store or reduce-add).  z (B,T,R) goes through p.zsave.  bw: bf16 copies of w1 / w2 (bf16 operand
+// path), or null (tf32).
+static int resblock_fwd_composed(const FwdParams& p, cudaStream_t st, const Bf16Weights* bw = nullptr) {
   const int R = p.R, S = p.S, Ap = p.Ap, ks = p.ks, K1 = ks * R + Ap;
   NtTcSeg segs[4];
   int ns = 0, rc;
   for (int j = 0; j < ks; j++) segs[ns++] = NtTcSeg{p.xin, R, -(ks - 1 - j) * p.d, R, p.w1, 2 * R, K1, j * R, 0};
   segs[ns++] = NtTcSeg{p.haux, Ap, 0, Ap, p.w1, 2 * R, K1, ks * R, 0};
+  Bf16Weights::apply(bw, segs, ns);
   // 128 gate channels (N = 256) and two time tiles per CTA tile when R allows: the activation tile [x taps | aux] is
   // re-read R/128 instead of R/64 times and every weight chunk serves 256 rows (these GEMMs are L2 -> SM bound)
   const int GC = composed_gc(R);
@@ -500,13 +564,15 @@ static int resblock_fwd_composed(const FwdParams& p, cudaStream_t st) {
       return rc;
   }
   if (p.xout) {
-    const NtTcSeg sr[1] = {{p.zsave, R, 0, R, p.w2, R + S, R, 0, 0}};
+    NtTcSeg sr[1] = {{p.zsave, R, 0, R, p.w2, R + S, R, 0, 0}};
+    Bf16Weights::apply(bw, sr, 1);
     const NtTcOpts o = plain_opts(R);
     if ((rc = gemm_nt_tc(sr, 1, R / o.n_blocks, p.xout, R, p.b2, nullptr, 0, p.xin, R, 0, 0, p.B, p.T, st, nullptr, nullptr,
                          nullptr, 0, 0, nullptr, &o)) != WNB_OK)
       return rc;
   }
-  const NtTcSeg ss[1] = {{p.zsave, R, 0, R, p.w2, R + S, R, 0, R}};
+  NtTcSeg ss[1] = {{p.zsave, R, 0, R, p.w2, R + S, R, 0, R}};
+  Bf16Weights::apply(bw, ss, 1);
   const NtTcOpts o = plain_opts(S);
   return gemm_nt_tc(ss, 1, S / o.n_blocks, p.skip, S, p.b2 + R, nullptr, 0, nullptr, 0, 0, p.skip_init ? 0 : 1, p.B, p.T, st,
                     nullptr, nullptr, nullptr, 0, 0, nullptr, &o);
@@ -524,6 +590,22 @@ WNB_API int wnb_resblock_fwd(const float* xin, const float* haux, const float* w
   WNB_REQUIRE(B > 0 && T > 0 && R > 0 && S > 0 && Ap > 0 && ks >= 1 && dilation >= 1, "resblock_fwd: bad shape");
   WNB_REQUIRE(xin && haux && w1 && b1 && w2 && b2 && skip, "resblock_fwd: null pointer");
   FwdParams p{xin, haux, w1, b1, w2, b2, xout, skip, zsave, B, T, R, S, Ap, ks, dilation, skip_init};
+  if (math_mode == WNB_MATH_BF16) {
+    // bf16 operands: the composed path for every shape it covers (the fused kernel is tf32 only)
+    WNB_REQUIRE(composed_tc_supported(R, S, Ap, ks), "resblock_fwd: shape R=%d S=%d Ap=%d ks=%d not supported by the "
+                "bf16 tensor-core path (use WNB_MATH_TF32 or WNB_MATH_FP32)", R, S, Ap, ks);
+    cudaStream_t st = (cudaStream_t)stream;
+    Bf16Weights bw;
+    int rc = to_bf16_weights(bw, {{w1, (int64_t)2 * R * (ks * R + Ap)}, {w2, (int64_t)(R + S) * R}}, st);
+    if (rc != WNB_OK) return rc;
+    if (zsave) return resblock_fwd_composed(p, st, &bw);
+    float* z = nullptr;
+    WNB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&z), (size_t)B * T * R * sizeof(float), st));
+    p.zsave = z;
+    rc = resblock_fwd_composed(p, st, &bw);
+    WNB_CUDA(cudaFreeAsync(z, st));
+    return rc;
+  }
   if (math_mode == WNB_MATH_TF32) {
     if (resblock_fwd_skip_supported(R, S, Ap, ks)) {
       WNB_REQUIRE(!zsave, "resblock_fwd: the fused per-block kernel keeps z on chip (pass no zsave)");
@@ -568,6 +650,8 @@ WNB_API int wnb_resblock_fwd_supported(int R, int S, int Ap, int ks, int math_mo
   if (R <= 0 || S <= 0 || Ap <= 0 || ks < 1) return 0;
   if (math_mode == WNB_MATH_TF32)   // 1 = fused per-block kernel, 2 = composed tensor-core path (zsave scratch)
     return resblock_fwd_skip_supported(R, S, Ap, ks) ? 1 : (composed_tc_supported(R, S, Ap, ks) ? 2 : 0);
+  if (math_mode == WNB_MATH_BF16) return composed_tc_supported(R, S, Ap, ks) ? 2 : 0;
+  if (math_mode != WNB_MATH_FP32) return 0;
   return (sizeof(TileSmem<8>) + (size_t)R * kBsLd * sizeof(float)) <= 227 * 1024 ? 1 : 0;
 }
 
@@ -583,24 +667,38 @@ WNB_API int wnb_resblock_bwd(const float* xin, const float* haux, const float* d
   WNB_REQUIRE(B > 0 && T > 0 && R > 0 && S > 0 && Ap > 0 && ks >= 1 && dilation >= 1, "resblock_bwd: bad shape");
   WNB_REQUIRE(xin && haux && dskip && w1 && b1 && w1t && w2t && dxin && dw1 && db1 && dw2 && db2 && workspace,
               "resblock_bwd: null pointer");
-  (void)math_mode;  // backward is fp32 SIMT in this round for both math modes
+  WNB_REQUIRE(math_mode == WNB_MATH_FP32 || math_mode == WNB_MATH_TF32 || math_mode == WNB_MATH_BF16,
+              "resblock_bwd: unknown math_mode %d", math_mode);
+  WNB_REQUIRE(math_mode != WNB_MATH_BF16 || composed_tc_supported(R, S, Ap, ks), "resblock_bwd: shape R=%d S=%d Ap=%d "
+              "ks=%d not supported by the bf16 tensor-core path (use WNB_MATH_TF32 or WNB_MATH_FP32)", R, S, Ap, ks);
   cudaStream_t st = (cudaStream_t)stream;
   float* z = (float*)workspace;
   float* dpre = z + (size_t)B * T * R;
   const int K1 = ks * R + Ap, M2 = R + S;
   int rc;
   const bool tc_fused_shape = math_mode == WNB_MATH_TF32 && R == 64 && ks == 2 && Ap == 32 && S % 32 == 0;
-  if (math_mode == WNB_MATH_TF32 && !tc_fused_shape && composed_tc_supported(R, S, Ap, ks)) {
-    // ---------------- composed tensor-core backward for general shapes ----------------
+  const bool bf16 = math_mode == WNB_MATH_BF16;
+  if (bf16 || (math_mode == WNB_MATH_TF32 && !tc_fused_shape && composed_tc_supported(R, S, Ap, ks))) {
+    // ---------------- composed tensor-core backward for general shapes (tf32, or bf16 operands) ----------------
+    Bf16Weights bwt;
+    const Bf16Weights* bw = nullptr;
+    if (bf16) {
+      if ((rc = to_bf16_weights(bwt, {{w1, (int64_t)2 * R * K1}, {w1t, (int64_t)K1 * 2 * R}, {w2t, (int64_t)R * M2}}, st)) !=
+          WNB_OK)
+        return rc;
+      bw = &bwt;
+    }
     float* dz = dxin;   // (B,T,R) scratch until the dX GEMM overwrites it
     const NtTcOpts opl = plain_opts(R);
     if (dout) {
-      const NtTcSeg sz[2] = {{dout, R, 0, R, w2t, R, R + S, 0, 0}, {dskip, S, 0, S, w2t, R, R + S, R, 0}};
+      NtTcSeg sz[2] = {{dout, R, 0, R, w2t, R, R + S, 0, 0}, {dskip, S, 0, S, w2t, R, R + S, R, 0}};
+      Bf16Weights::apply(bw, sz, 2);
       if ((rc = gemm_nt_tc(sz, 2, R / opl.n_blocks, dz, R, nullptr, nullptr, 0, nullptr, 0, 0, 0, B, T, st, nullptr, nullptr,
                            nullptr, 0, 0, nullptr, &opl)) != WNB_OK)
         return rc;
     } else {
-      const NtTcSeg sz[1] = {{dskip, S, 0, S, w2t, R, R + S, R, 0}};
+      NtTcSeg sz[1] = {{dskip, S, 0, S, w2t, R, R + S, R, 0}};
+      Bf16Weights::apply(bw, sz, 1);
       if ((rc = gemm_nt_tc(sz, 1, R / opl.n_blocks, dz, R, nullptr, nullptr, 0, nullptr, 0, 0, 0, B, T, st, nullptr, nullptr,
                            nullptr, 0, 0, nullptr, &opl)) != WNB_OK)
         return rc;
@@ -609,6 +707,7 @@ WNB_API int wnb_resblock_bwd(const float* xin, const float* haux, const float* d
     int ns = 0;
     for (int j = 0; j < ks; j++) sg[ns++] = NtTcSeg{xin, R, -(ks - 1 - j) * dilation, R, w1, 2 * R, K1, j * R, 0};
     sg[ns++] = NtTcSeg{haux, Ap, 0, Ap, w1, 2 * R, K1, ks * R, 0};
+    Bf16Weights::apply(bw, sg, ns);
     const int GC = composed_gc(R);
         for (int c0 = 0; c0 < R; c0 += GC) {   // gate recompute + z + dpre, GC gate channels per launch
       const NtTcGate g{2, c0, R, b1 + c0, b1 + R + c0, dz, dpre};
@@ -619,23 +718,26 @@ WNB_API int wnb_resblock_bwd(const float* xin, const float* haux, const float* d
     {  // dxin = dout + sum_j dpre(t + (ks-1-j)d) W1[:, tap j]
       NtTcSeg sx[3];
       for (int j = 0; j < ks; j++) sx[j] = NtTcSeg{dpre, 2 * R, (ks - 1 - j) * dilation, 2 * R, w1t, K1, 2 * R, 0, j * R};
+      Bf16Weights::apply(bw, sx, ks);
       if ((rc = gemm_nt_tc(sx, ks, R / opl.n_blocks, dxin, R, nullptr, nullptr, 0, dout, R, 0, 0, B, T, st, nullptr, nullptr,
                            nullptr, 0, 0, nullptr, &opl)) != WNB_OK)
         return rc;
     }
     if (dhaux) {
-      const NtTcSeg sh[1] = {{dpre, 2 * R, 0, 2 * R, w1t, K1, 2 * R, 0, ks * R}};
+      NtTcSeg sh[1] = {{dpre, 2 * R, 0, 2 * R, w1t, K1, 2 * R, 0, ks * R}};
+      Bf16Weights::apply(bw, sh, 1);
       if ((rc = gemm_nt_tc(sh, 1, Ap, dhaux, Ap, nullptr, nullptr, 0, nullptr, 0, 0, 1, B, T, st)) != WNB_OK) return rc;
     }
     // dW1 = dpre^T [x taps | aux]  (+ db1), dW2 = [dout | dskip]^T z  (+ db2)
     for (int j = 0; j < ks; j++)
       if ((rc = wgrad_tc_concat(dpre, 2 * R, nullptr, 0, 2 * R, xin, R, R, -(ks - 1 - j) * dilation, dw1 + j * R, K1,
-                                j == 0 ? db1 : nullptr, B, T, st)) != WNB_OK)
+                                j == 0 ? db1 : nullptr, B, T, st, bf16)) != WNB_OK)
         return rc;
-    if ((rc = wgrad_tc_concat(dpre, 2 * R, nullptr, 0, 2 * R, haux, Ap, Ap, 0, dw1 + ks * R, K1, nullptr, B, T, st)) != WNB_OK)
+    if ((rc = wgrad_tc_concat(dpre, 2 * R, nullptr, 0, 2 * R, haux, Ap, Ap, 0, dw1 + ks * R, K1, nullptr, B, T, st, bf16)) !=
+        WNB_OK)
       return rc;
-    if (dout) return wgrad_tc_concat(dout, R, dskip, S, R + S, z, R, R, 0, dw2, R, db2, B, T, st);
-    return wgrad_tc_concat(dskip, S, nullptr, 0, S, z, R, R, 0, dw2 + (size_t)R * R, R, db2 + R, B, T, st);
+    if (dout) return wgrad_tc_concat(dout, R, dskip, S, R + S, z, R, R, 0, dw2, R, db2, B, T, st, bf16);
+    return wgrad_tc_concat(dskip, S, nullptr, 0, S, z, R, R, 0, dw2 + (size_t)R * R, R, db2 + R, B, T, st, bf16);
   }
   const bool tc_bwd = tc_fused_shape;
   if (tc_bwd) {
@@ -759,24 +861,36 @@ WNB_API int wnb_post_fwd(float* skip, const float* wp1, const float* bp1, const 
                  void* stream) {
   WNB_REQUIRE(B > 0 && T > 0 && S > 0 && Q > 0, "post_fwd: bad shape");
   WNB_REQUIRE(skip && wp1 && bp1 && wp2 && bp2 && r1 && logits, "post_fwd: null pointer (r1 scratch is required)");
+  WNB_REQUIRE(math_mode == WNB_MATH_FP32 || math_mode == WNB_MATH_TF32 || math_mode == WNB_MATH_BF16,
+              "post_fwd: unknown math_mode %d", math_mode);
+  WNB_REQUIRE(math_mode != WNB_MATH_BF16 || (nt_tc_n_ok(S) && nt_tc_n_ok(Q)),
+              "post_fwd: S=%d Q=%d not supported by the bf16 tensor-core path", S, Q);
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
-  if (math_mode == WNB_MATH_TF32 && nt_tc_n_ok(S) && nt_tc_n_ok(Q)) {
+  if ((math_mode == WNB_MATH_TF32 || math_mode == WNB_MATH_BF16) && nt_tc_n_ok(S) && nt_tc_n_ok(Q)) {
     // rectify the skip sum in place (its sign pattern, all the backward needs, is unchanged), then two
     // tensor-core GEMMs with fused bias / ReLU epilogues
+    Bf16Weights bwt;
+    const Bf16Weights* bw = nullptr;
+    if (math_mode == WNB_MATH_BF16) {
+      if ((rc = to_bf16_weights(bwt, {{wp1, (int64_t)S * S}, {wp2, (int64_t)Q * S}}, st)) != WNB_OK) return rc;
+      bw = &bwt;
+    }
     const int64_t n4 = (int64_t)B * T * S / 4;
     if (!skip_rectified) {
       relu_inplace_kernel<<<device_sms() * 8, 256, 0, st>>>(reinterpret_cast<float4*>(skip), n4);
       WNB_CHECK_LAUNCH("relu_inplace");
     }
-    const NtTcSeg s1[1] = {{skip, S, 0, S, wp1, S, S, 0, 0}};
+    NtTcSeg s1[1] = {{skip, S, 0, S, wp1, S, S, 0, 0}};
+    Bf16Weights::apply(bw, s1, 1);
     if (post_split(S)) {   // two 256-column blocks: double-buffered accumulators, epilogue overlapped with the next tile
       const NtTcOpts o{2};
       if ((rc = gemm_nt_tc(s1, 1, S / 2, r1, S, bp1, nullptr, 0, nullptr, 0, 1, 0, B, T, st, nullptr, nullptr, nullptr, 0, 0,
                            nullptr, &o)) != WNB_OK)
         return rc;
     } else if ((rc = gemm_nt_tc(s1, 1, S, r1, S, bp1, nullptr, 0, nullptr, 0, 1, 0, B, T, st)) != WNB_OK) return rc;
-    const NtTcSeg s2[1] = {{r1, S, 0, S, wp2, Q, S, 0, 0}};
+    NtTcSeg s2[1] = {{r1, S, 0, S, wp2, Q, S, 0, 0}};
+    Bf16Weights::apply(bw, s2, 1);
     const NtTcOpts o2{1};
     return gemm_nt_tc(s2, 1, Q, logits, Q, bp2, nullptr, 0, nullptr, 0, 0, 0, B, T, st, nullptr, nullptr, nullptr, 0, 0,
                       nullptr, &o2);
@@ -804,12 +918,25 @@ WNB_API int wnb_post_bwd(const float* skip, const float* r1, const float* dlogit
   WNB_REQUIRE(skip && r1 && dlogits && wp1t && wp2t && dskip && dwp1 && dbp1 && dwp2 && dbp2 && workspace,
               "post_bwd: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
+  WNB_REQUIRE(math_mode == WNB_MATH_FP32 || math_mode == WNB_MATH_TF32 || math_mode == WNB_MATH_BF16,
+              "post_bwd: unknown math_mode %d", math_mode);
+  WNB_REQUIRE(math_mode != WNB_MATH_BF16 || (nt_tc_n_ok(S) && nt_tc_n_ok(Q)),
+              "post_bwd: S=%d Q=%d not supported by the bf16 tensor-core path", S, Q);
   float* dh1 = workspace;  // (B,T,S)
   int rc;
-  if (math_mode == WNB_MATH_TF32 && nt_tc_n_ok(S) && nt_tc_n_ok(Q)) {
-    // (skip was rectified in place by the tf32 forward, so it doubles as relu(skip) and as the sign mask)
-    const NtTcSeg s1[1] = {{dlogits, Q, 0, Q, wp2t, S, Q, 0, 0}};
-    const NtTcSeg s2[1] = {{dh1, S, 0, S, wp1t, S, S, 0, 0}};
+  const bool bf16 = math_mode == WNB_MATH_BF16;
+  if ((math_mode == WNB_MATH_TF32 || bf16) && nt_tc_n_ok(S) && nt_tc_n_ok(Q)) {
+    // (skip was rectified in place by the tensor-core forward, so it doubles as relu(skip) and as the sign mask)
+    Bf16Weights bwt;
+    const Bf16Weights* bw = nullptr;
+    if (bf16) {
+      if ((rc = to_bf16_weights(bwt, {{wp2t, (int64_t)S * Q}, {wp1t, (int64_t)S * S}}, st)) != WNB_OK) return rc;
+      bw = &bwt;
+    }
+    NtTcSeg s1[1] = {{dlogits, Q, 0, Q, wp2t, S, Q, 0, 0}};
+    NtTcSeg s2[1] = {{dh1, S, 0, S, wp1t, S, S, 0, 0}};
+    Bf16Weights::apply(bw, s1, 1);
+    Bf16Weights::apply(bw, s2, 1);
     if (post_split(S)) {
       const NtTcOpts o{2};
       if ((rc = gemm_nt_tc(s1, 1, S / 2, dh1, S, nullptr, r1, S, nullptr, 0, 0, 0, B, T, st, nullptr, nullptr, nullptr, 0, 0,
@@ -825,6 +952,10 @@ WNB_API int wnb_post_bwd(const float* skip, const float* r1, const float* dlogit
     // 2 launches of (2 M-blocks x 128-column groups) for dWp1: a squarer tile than 4 M-blocks x 64 columns; same-box
     // A/B (two repetitions each): 8.90 / 8.95 ms per step against 8.97 / 8.97 (WNB_POST_WG_OLD=1 selects the old split)
     static const bool old_split = [] { const char* e = getenv("WNB_POST_WG_OLD"); return e && e[0] == '1'; }();
+    if (bf16) {
+      if ((rc = wgrad_tc_concat(dlogits, Q, nullptr, 0, Q, r1, S, S, 0, dwp2, S, dbp2, B, T, st, true)) != WNB_OK) return rc;
+      return wgrad_tc_concat(dh1, S, nullptr, 0, S, skip, S, S, 0, dwp1, S, dbp1, B, T, st, true);
+    }
     if (old_split) {
       if ((rc = wgrad_tc_split(dlogits, Q, Q, r1, S, S, dwp2, S, dbp2, B, T, st)) != WNB_OK) return rc;
       return wgrad_tc_split(dh1, S, S, skip, S, S, dwp1, S, dbp1, B, T, st);

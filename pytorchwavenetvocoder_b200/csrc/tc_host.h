@@ -1,5 +1,6 @@
 // tc_host.h -- host-side entry points of the tensor-core (wgmma) kernels (internal; the C ABI is include/wnb200.h).
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
 namespace wnb {
@@ -18,7 +19,8 @@ struct WgBlock { WgOperand ops[2]; int nops; float* c; int m_valid; float* db; }
 // nseg > 1: nseg independent problems of identical structure in one launch (every residual block's dW1, say):
 // operands pick their per-segment batch / shift / channel offsets with the WG_* flags, block i's C and db are at
 // c + i*c_seg_stride, db + i*db_seg_stride; CTAs split the flattened (segment, time tile) space evenly.
-struct WgOpts { int n_split; int nseg; const int* seg_shift; int c_seg_stride; int db_seg_stride; };
+// bf16: both operands are rounded to bf16 (nearest even) and multiplied by bf16 wgmma, fp32 accumulate.
+struct WgOpts { int n_split; int nseg; const int* seg_shift; int c_seg_stride; int db_seg_stride; int bf16; };
 int wgrad_tc_blocks(const WgBlock* blocks, int nblocks, const WgOperand* b_ops, int nb_ops, int ldc, int B, int T,
                     cudaStream_t st, const WgOpts* opts = nullptr);
 int wgrad_tc(const WgOperand* a_ops, int na_ops, const WgOperand* b_ops, int nb_ops, float* c, int ldc, int m_valid,
@@ -26,8 +28,12 @@ int wgrad_tc(const WgOperand* a_ops, int na_ops, const WgOperand* b_ops, int nb_
 
 // ---- NT GEMM (gemm_nt_tc.cu):  out[b,t,n] = sum_seg sum_k A_seg[b,t+shift,k] W_seg[n0+n][k0+k]  (+ epilogues) ----
 // One segment: activation tensor (B,T,CA) read at rows t+shift, channels [0,K); weight matrix w (rows x ldw,
-// K-contiguous) rows [n0, n0+N), columns [k0, k0+K).
-struct NtTcSeg { const float* a; int CA; int shift; int K; const float* w; int w_rows; int w_cols; int k0; int n0; };
+// K-contiguous) rows [n0, n0+N), columns [k0, k0+K).  wb: null, or a bf16 copy of w (same layout): then both operands
+// are rounded to bf16 (nearest even) and multiplied by bf16 wgmma; every segment of a call has one or none has.
+struct NtTcSeg {
+  const float* a; int CA; int shift; int K; const float* w; int w_rows; int w_cols; int k0; int n0;
+  const __nv_bfloat16* wb;
+};
 // gate epilogue request: mode 1 = forward (z out), 2 = backward (dz in, z + dpre out); channels c0..c0+63 of R
 struct NtTcGate { int mode; int c0; int R; const float* bias_sig; const float* bias_tanh; const float* dz; float* dpre; };
 struct NtTcOpts {

@@ -1,11 +1,12 @@
 // tc_ptx.cuh -- thin inline-PTX wrappers for the Hopper (sm_90a) async machinery of the tensor-core kernels:
 // mbarrier, TMA (cp.async.bulk.tensor load / store / reduce-add), wgmma (fences, commit / wait groups, shared-memory
-// matrix descriptors; the MMA wrappers themselves are in wgmma_tf32.cuh), named barriers.
+// matrix descriptors; the MMA wrappers themselves are in wgmma_tf32.cuh and wgmma_bf16.cuh), named barriers.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "wgmma_bf16.cuh"
 #include "wgmma_tf32.cuh"
 
 namespace wnb {
@@ -152,6 +153,11 @@ __device__ __forceinline__ void bulk_wait() {
 __device__ __forceinline__ uint64_t gmma_desc_k_sw128(uint32_t saddr) {
   return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
+// The same for a K-major bf16 tile in the 64B-swizzled layout (CU_TENSOR_MAP_SWIZZLE_64B): rows of 32 bf16 (64 B),
+// 8-row groups 512 B apart, tile start on a 512-byte boundary; the k-th group of 16 bf16 is at +32 k bytes.
+__device__ __forceinline__ uint64_t gmma_desc_k_sw64(uint32_t saddr) {
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (32ull << 32) | (2ull << 62);
+}
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -173,6 +179,16 @@ __device__ __forceinline__ uint32_t sw128_off(int r, int c) {
   return (uint32_t)(r * 128 + ((((c >> 2) ^ r) & 7) << 4) + ((c & 3) << 2));
 }
 
+// byte offset of element (row n, column k < 32) in a [rows x 32 bf16] tile in the 64B-swizzled layout
+__device__ __forceinline__ uint32_t sw64_off(int n, int k) {
+  return (uint32_t)(n * 64 + ((((k >> 3) ^ (n >> 1)) & 3) << 4) + ((k & 7) << 1));
+}
+// two fp32 -> one register of two bf16, each rounded to nearest even; lo goes to the lower half
+__device__ __forceinline__ uint32_t cvt_bf16x2(float lo, float hi) {
+  uint32_t r;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
+}
 __device__ __forceinline__ float tanh_approx(float x) {
   float y;
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));

@@ -17,6 +17,11 @@
 // each group = (tensor map, channel offset, time shift); dilated taps are just shifted groups, zero filled
 // out of range by TMA.  An optional extra all-ones B group turns column 0 of that group into the bias
 // gradient sum_t A[t][m] (replaces colsum_kernel).
+//
+// bf16 operands (BF16 = true, WgOpts::bf16): the transpose writes B rounded to bf16 (cvt.rn.bf16x2 of two time rows)
+// into a 64B-swizzled K-major [N x 32] bf16 tile, the A fragments are rounded the same way from the fp32 sub-tiles, and
+// the MMAs are bf16 wgmma m64nNk16 with fp32 accumulation.  The all-ones rows are exact in bf16; slots and their
+// reduction are unchanged.
 #include <cuda.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -56,13 +61,18 @@ struct alignas(64) Params {
   int seg_shift[kMaxSeg];
 };
 
-template <int N>
+// bytes of one row (32 time steps) of the transposed B tile
+template <bool BF16>
+__host__ __device__ constexpr int bt_row_bytes() { return BF16 ? 64 : 128; }
+
+template <int N, bool BF16>
 __global__ void __launch_bounds__(kThreadsW, 1) wgrad_tc_kernel(const __grid_constant__ Params p) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  constexpr int kBtRow = bt_row_bytes<BF16>();
   const int stage_bytes = (4 + p.nB) * kSub;
   unsigned char* bT = smem;                                   // 2 x K-major [N x 32] B tile (+ the ones rows)
-  unsigned char* ring = smem + 2 * N * 128;
+  unsigned char* ring = smem + 2 * N * kBtRow;
   uint64_t* bars = reinterpret_cast<uint64_t*>(ring + (size_t)p.nstages * stage_bytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + p.nstages;
@@ -89,8 +99,13 @@ __global__ void __launch_bounds__(kThreadsW, 1) wgrad_tc_kernel(const __grid_con
   }
   if (p.use_ones) {   // the ones rows of both transposed B tiles: filled once, never overwritten
     for (int h = 0; h < 2; h++) {
-      float4* o = reinterpret_cast<float4*>(bT + h * N * 128 + p.nB * 32 * 128);
-      for (int i = threadIdx.x; i < 32 * 128 / 16; i += kThreadsW) o[i] = make_float4(1.f, 1.f, 1.f, 1.f);
+      if constexpr (BF16) {
+        uint4* o = reinterpret_cast<uint4*>(bT + h * N * kBtRow + p.nB * 32 * kBtRow);
+        for (int i = threadIdx.x; i < 32 * kBtRow / 16; i += kThreadsW) o[i] = make_uint4(0x3F803F80u, 0x3F803F80u, 0x3F803F80u, 0x3F803F80u);
+      } else {
+        float4* o = reinterpret_cast<float4*>(bT + h * N * 128 + p.nB * 32 * 128);
+        for (int i = threadIdx.x; i < 32 * 128 / 16; i += kThreadsW) o[i] = make_float4(1.f, 1.f, 1.f, 1.f);
+      }
     }
   }
   __syncthreads();
@@ -152,6 +167,55 @@ __global__ void __launch_bounds__(kThreadsW, 1) wgrad_tc_kernel(const __grid_con
   // Stage i: B transposed into bT[i & 1], A fragments into register set i & 1, the ring stage released, then the MMAs of
   // stage i are issued and those of stage i - 1 waited for -- so the transpose of stage i + 1 overlaps the MMAs of stage i.
   // (wgmma reads its A registers asynchronously: the set of stage i is not touched again before stage i + 2.)
+  if constexpr (BF16) {
+    // as below with bf16 operands: each transpose step rounds two time rows of 4 channels into 4 bf16 pairs; the A
+    // fragment of k16 step kk holds rows m, m + 8 at time rows 16 kk + 2 (lane % 4) (+ 8), each with its successor
+    uint32_t a0[2][4], a1[2][4];
+    const int nvec2 = p.nB * 32 * 32 / 8;
+    auto stage = [&](uint32_t (&a)[2][4], unsigned char* bTh) {
+      ptx::mbar_wait(&full[s], ph);
+      const unsigned char* st = ring + (size_t)s * stage_bytes;
+      ptx::named_bar(1, kConsumers);
+      for (int idx = threadIdx.x; idx < nvec2; idx += kConsumers) {
+        const int grp = idx >> 7, r = ((idx >> 3) & 15) * 2, c4 = idx & 7;   // B group, time row pair, 4-channel piece
+        const unsigned char* src = st + (4 + grp) * kSub + ((c4 ^ (r & 7)) << 4);
+        const float4 v0 = *reinterpret_cast<const float4*>(src + r * 128);
+        const float4 v1 = *reinterpret_cast<const float4*>(st + (4 + grp) * kSub + (r + 1) * 128 + ((c4 ^ ((r + 1) & 7)) << 4));
+        const float lo[4] = {v0.x, v0.y, v0.z, v0.w}, hi[4] = {v1.x, v1.y, v1.z, v1.w};
+#pragma unroll
+        for (int j = 0; j < 4; j++)
+          *reinterpret_cast<uint32_t*>(bTh + ptx::sw64_off(grp * 32 + c4 * 4 + j, r)) = ptx::cvt_bf16x2(lo[j], hi[j]);
+      }
+#pragma unroll
+      for (int kk = 0; kk < 2; kk++) {
+#pragma unroll
+        for (int h = 0; h < 4; h++) {
+          const int m = m0 + 8 * (h & 1), kr = 16 * kk + 2 * tq + 8 * (h >> 1);
+          const unsigned char* sub = st + (m >> 5) * kSub;
+          a[kk][h] = ptx::cvt_bf16x2(*reinterpret_cast<const float*>(sub + ptx::sw128_off(kr, m & 31)),
+                                     *reinterpret_cast<const float*>(sub + ptx::sw128_off(kr + 1, m & 31)));
+        }
+      }
+      ptx::mbar_arrive(&empty[s]);
+      if (++s == (uint32_t)p.nstages) { s = 0; ph ^= 1; }
+      ptx::fence_proxy_async();
+      ptx::named_bar(1, kConsumers);
+      ptx::wg_fence();
+      const uint32_t b_u32 = ptx::smem_u32(bTh);
+#pragma unroll
+      for (int kk = 0; kk < 2; kk++) ptx::wgmma_rs_bf16<N>(d, a[kk], ptx::gmma_desc_k_sw64(b_u32 + 32 * kk), 1);
+      ptx::wg_commit();
+      ptx::wg_wait<1>();
+    };
+    for (int f = tile_begin; f < tile_end; f += 2) {
+      stage(a0, bT);
+      if (f + 1 < tile_end) stage(a1, bT + N * kBtRow);
+    }
+    ptx::wg_wait<0>();
+    ptx::wg_touch(d);
+    write_slot();
+    return;
+  }
   uint32_t a0[4][4], a1[4][4];
   auto stage = [&](uint32_t (&a)[4][4], unsigned char* bTh) {
     ptx::mbar_wait(&full[s], ph);
@@ -248,11 +312,25 @@ static bool make_act_map(CUtensorMap* m, const float* base, int C, int T, int B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int N>
+template <int N, bool BF16>
 static cudaError_t launch_n(int grid, size_t smem, cudaStream_t st, const Params& p) {
-  cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(wgrad_tc_kernel<N>), smem);
+  cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(wgrad_tc_kernel<N, BF16>), smem);
   if (e != cudaSuccess) return e;
-  return launch_pdl(wgrad_tc_kernel<N>, grid, kThreadsW, smem, st, p);
+  return launch_pdl(wgrad_tc_kernel<N, BF16>, grid, kThreadsW, smem, st, p);
+}
+
+template <bool BF16>
+static cudaError_t launch_bf(int N, int grid, size_t smem, cudaStream_t st, const Params& p) {
+  switch (N) {
+    case 32: return launch_n<32, BF16>(grid, smem, st, p);
+    case 64: return launch_n<64, BF16>(grid, smem, st, p);
+    case 96: return launch_n<96, BF16>(grid, smem, st, p);
+    case 128: return launch_n<128, BF16>(grid, smem, st, p);
+    case 160: return launch_n<160, BF16>(grid, smem, st, p);
+    case 192: return launch_n<192, BF16>(grid, smem, st, p);
+    case 224: return launch_n<224, BF16>(grid, smem, st, p);
+    default: return launch_n<256, BF16>(grid, smem, st, p);
+  }
 }
 
 }  // namespace wg
@@ -272,8 +350,10 @@ int wgrad_tc_blocks(const WgBlock* blocks, int nblocks, const WgOperand* b_ops, 
   p.use_ones = any_db ? 1 : 0;
   if (p.nB < 1 || p.nB > kMaxB - 1) { set_error("wgrad_tc: 1..7 B groups"); return WNB_ERR_INVALID; }
   const int N = 32 * (p.nB + p.use_ones);
+  const bool bf16 = opts && opts->bf16;
+  const int bt_bytes = 2 * N * (bf16 ? bt_row_bytes<true>() : bt_row_bytes<false>());   // the two transposed B tiles
   const int stage_bytes = (4 + p.nB) * kSub;
-  int nst = (227 * 1024 - 1024 - 256 - 2 * N * 128) / stage_bytes;
+  int nst = (227 * 1024 - 1024 - 256 - bt_bytes) / stage_bytes;
   if (nst > 8) nst = 8;
   if (nst < 2) { set_error("wgrad_tc: stage too large"); return WNB_ERR_INVALID; }
   p.nstages = nst;
@@ -337,7 +417,7 @@ int wgrad_tc_blocks(const WgBlock* blocks, int nblocks, const WgOperand* b_ops, 
   p.T = T; p.B = B;
   p.tiles_per_b = (T + kTK - 1) / kTK;
   p.ntiles = B * p.tiles_per_b;
-  const size_t smem = (size_t)2 * N * 128 + (size_t)nst * stage_bytes + 1024 + 256;
+  const size_t smem = (size_t)bt_bytes + (size_t)nst * stage_bytes + 1024 + 256;
   const int sms = device_sms();
   const int sets = p.nMB * p.n_split * p.nseg;
   int ksplit = sms / sets;
@@ -348,17 +428,7 @@ int wgrad_tc_blocks(const WgBlock* blocks, int nblocks, const WgOperand* b_ops, 
   const int grid = sets * ksplit;
   p.part = static_cast<float*>(scratch_buffer(st, SCRATCH_WGRAD, (size_t)grid * 128 * N * sizeof(float)));
   if (!p.part) { set_error("wgrad_tc: cannot allocate the partial-sum scratch"); return WNB_ERR_CUDA; }
-  cudaError_t le;
-  switch (N) {
-    case 32: le = launch_n<32>(grid, smem, st, p); break;
-    case 64: le = launch_n<64>(grid, smem, st, p); break;
-    case 96: le = launch_n<96>(grid, smem, st, p); break;
-    case 128: le = launch_n<128>(grid, smem, st, p); break;
-    case 160: le = launch_n<160>(grid, smem, st, p); break;
-    case 192: le = launch_n<192>(grid, smem, st, p); break;
-    case 224: le = launch_n<224>(grid, smem, st, p); break;
-    default: le = launch_n<256>(grid, smem, st, p); break;
-  }
+  const cudaError_t le = bf16 ? launch_bf<true>(N, grid, smem, st, p) : launch_bf<false>(N, grid, smem, st, p);
   if (le != cudaSuccess) { set_error("wgrad_tc: launch failed: %s", cudaGetErrorString(le)); return WNB_ERR_CUDA; }
   WNB_CHECK_LAUNCH("wgrad_tc");
   const int64_t total = (int64_t)p.nseg * p.n_split * p.nMB * 128 * (32 * p.nB + p.use_ones);

@@ -24,7 +24,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from .. import _lib
-from .._lib import MATH_FP32, MATH_TF32, MODE_ARGMAX, MODE_SAMPLING, check, ptr, stream
+from .._lib import MATH_BF16, MATH_FP32, MATH_TF32, MODE_ARGMAX, MODE_SAMPLING, check, ptr, stream
 
 __all__ = ["encode_mu_law", "decode_mu_law", "initialize", "OneHot", "CausalConv1d", "UpSampling",
            "WaveNet", "cross_entropy", "mulaw_pcm16_table", "codes_to_pcm16"]
@@ -38,6 +38,15 @@ def tc_supported(cfg):
     lib = _lib.load()
     Q, A, R, S, depth, repeat, ks, U = cfg
     return bool(lib.wnb_resblock_fwd_supported(R, S, _round_up(A, 32), ks, MATH_TF32))
+
+
+def bf16_supported(cfg):
+    """True when the bf16 tensor-core path (math_mode="bf16": the composed per-block GEMMs and the post network)
+    covers WaveNet(*cfg)."""
+    lib = _lib.load()
+    Q, A, R, S, depth, repeat, ks, U = cfg
+    ok = S % 32 == 0 and Q % 32 == 0 and (S <= 256 or S == 512) and (Q <= 256 or Q == 512)
+    return ok and lib.wnb_resblock_fwd_supported(R, S, _round_up(A, 32), ks, MATH_BF16) == 2
 
 
 def _device():
@@ -199,9 +208,9 @@ class _WaveNetFn(torch.autograd.Function):
         xs = torch.empty(nbuf, B, T, R, device=dev, dtype=torch.float32)
         check(lib.wnb_front_embed_fwd(ptr(x), ptr(wf), ptr(bf), ptr(xs[0]), B, T, Q, R, ks, st), "front_embed_fwd")
         skip = torch.empty(B, T, S, device=dev, dtype=torch.float32)
-        # the composed tensor-core path needs a z scratch
+        # the composed tensor-core path (tf32 or bf16) needs a z scratch
         zbuf = None
-        if math_mode == MATH_TF32 and lib.wnb_resblock_fwd_supported(R, S, Ap, ks, MATH_TF32) == 2:
+        if math_mode in (MATH_TF32, MATH_BF16) and lib.wnb_resblock_fwd_supported(R, S, Ap, ks, math_mode) == 2:
             zbuf = torch.empty(B, T, R, device=dev, dtype=torch.float32)
         prof = PROFILE_EVENTS
         for l, d in enumerate(dilations):
@@ -579,8 +588,11 @@ class WaveNet(nn.Module):
         self.dilations = [2 ** i for i in range(self.dilation_depth)] * self.dilation_repeat
         self.receptive_field = (self.kernel_size - 1) * sum(self.dilations) + 1
 
-        # contraction precision of the training forward. "fp32" = FFMA parity path,
-        # "tf32" = wgmma tensor-core path (fp32 storage and accumulation). Decode is always fp32.
+        # contraction precision of training (forward and backward). "fp32" = FFMA parity path, "tf32" = wgmma
+        # tensor-core path, "bf16" = wgmma with both operands of every product rounded to bf16 on the per-block
+        # composed path (bf16_supported(); the deferred-skip stack is tf32 only). Storage, accumulation, gradients
+        # and optimizer state stay fp32 in every mode. Decode (fast_generate / batch_fast_generate) is always fp32,
+        # whatever math_mode says, so that argmax decoding keeps its parity with the reference.
         self.math_mode = "fp32"
 
         # for preprocessing
@@ -621,7 +633,9 @@ class WaveNet(nn.Module):
             return MATH_FP32
         if self.math_mode == "tf32":
             return MATH_TF32
-        raise ValueError("math_mode should be fp32 or tf32")
+        if self.math_mode == "bf16":
+            return MATH_BF16
+        raise ValueError("math_mode should be fp32, tf32 or bf16, got %r" % (self.math_mode,))
 
     def _pack(self):
         R, A, Ap, ks = self.n_resch, self.n_aux, self.n_aux_pad, self.kernel_size
@@ -893,7 +907,8 @@ class WaveNet(nn.Module):
     def fast_generate(self, x, h, n_samples, intervals=None, mode="sampling"):
         """GENERATE WAVEFORM WITH FAST ALGORITHM (reference wavenet.py:309-395).
 
-        One persistent kernel launch; ``intervals`` only controls the summary log line."""
+        One persistent kernel launch; ``intervals`` only controls the summary log line.  Decoding is fp32 whatever
+        ``math_mode`` is (argmax parity with the reference)."""
         start = time.time()
         gen = self._decode(x[:1], h[:1], [n_samples], mode)
         out = gen[0, :n_samples].cpu().numpy().astype(np.int64)
@@ -916,7 +931,8 @@ class WaveNet(nn.Module):
         """GENERATE WAVEFORM WITH FAST ALGORITHM IN BATCH MODE (reference wavenet.py:397-511).
 
         Returns the utterances in COMPLETION order (ascending length, ties by batch index) exactly
-        like the reference's retirement loop (:487-509).  The caller's list is not mutated."""
+        like the reference's retirement loop (:487-509).  The caller's list is not mutated.  Decoding is fp32 whatever
+        ``math_mode`` is (argmax parity with the reference)."""
         start = time.time()
         n_list = [int(n) for n in n_samples_list]
         gen = self._decode(x, h, n_list, mode).cpu().numpy().astype(np.int64)

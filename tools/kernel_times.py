@@ -1,11 +1,14 @@
 #!/usr/bin/env python
 """Per-kernel GPU time of one training step of the bench workload (bench.py's model and batch), from torch.profiler.
 
-    python tools/kernel_times.py [--steps N] [--match SUBSTRING ...]
+    python tools/kernel_times.py [--steps N] [--match SUBSTRING ...] [--math {tf32,bf16,fp32}]
+                                 [--cfg Q,A,R,S,depth,repeat,ks,U --batch B --length T]
 
 Prints one line per kernel name: total microseconds per step and launches per step, sorted by time; with --match only
 the kernels whose name contains one of the substrings (e.g. the fixed-order reductions: --match front_embed token_kernel
-sum_rows sum_loss wgrad_reduce aux_upsample_bwd).
+sum_rows sum_loss wgrad_reduce aux_upsample_bwd).  --math picks the model's math_mode, --cfg another architecture (e.g.
+the recipe shapes 256,28,512,256,10,3,2,80 --length 23040 or 256,80,512,256,10,3,3,256 --length 20992) on random
+weights and a random batch of --batch windows.
 """
 import argparse
 import os
@@ -21,13 +24,30 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--match", nargs="*", default=None)
+    ap.add_argument("--math", default="tf32", choices=["tf32", "bf16", "fp32"])
+    ap.add_argument("--cfg", default=None, help="Q,A,R,S,depth,repeat,ks,U (default: bench.py's model and batch)")
+    ap.add_argument("--batch", type=int, default=bench.BATCH)
+    ap.add_argument("--length", type=int, default=None, help="samples per window with --cfg (a multiple of U)")
     args = ap.parse_args()
     from pytorchwavenetvocoder_b200.optim import Adam
     dev = torch.device("cuda", 0)
-    cfg, net = bench.make_model(dev, "tf32")
+    if args.cfg is None:
+        cfg, net = bench.make_model(dev, args.math)
+        x, h, t = (a.to(dev) for a in bench.synth_batch(cfg, 0, args.batch, pinned=False))
+    else:
+        sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+        from math_mode_times import make
+        c = tuple(int(v) for v in args.cfg.split(","))
+        if args.length is None:
+            raise SystemExit("--length is required with --cfg")
+        net, _ = make(c, args.math, dev)
+        cfg = bench._Cfg(c)
+        g = torch.Generator().manual_seed(20260924)
+        xfull = torch.randint(0, c[0], (args.batch, args.length + 1), generator=g, dtype=torch.int64)
+        x, t = xfull[:, :-1].contiguous().to(dev), xfull[:, 1:].contiguous().to(dev)
+        h = torch.randn(args.batch, c[1], args.length // max(c[7], 1), generator=g).to(dev)
     net.train()
     opt = Adam(net.parameters(), lr=1e-4, module=net)
-    x, h, t = (a.to(dev) for a in bench.synth_batch(cfg, 0, bench.BATCH, pinned=False))
 
     def step():
         loss = net.forward_loss(x, h, t, cfg.receptive_field)
