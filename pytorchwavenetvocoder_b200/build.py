@@ -6,6 +6,10 @@
 The library is a plain C-ABI shared object (no torch headers); cudart is linked statically and the
 driver API (TMA descriptor encoding) is resolved at run time through cudaGetDriverEntryPoint, so the
 .so loads on a machine without a GPU (CPU test tier).
+
+Debugging builds: adding "-DWNB_WAIT_PRINTF" to NVCC_FLAGS makes a bounded mbarrier wait that times out (csrc/tc_ptx.cuh)
+print its block and thread before it traps.  It is off by default because the printf call serialises every wgmma of the
+tensor-core kernels (ptxas note C7510; tests/test_wgmma_pipeline.py checks that the default build has none).
 """
 import os
 import subprocess

@@ -21,21 +21,26 @@ struct ProfScope {
 
 // Launch with programmatic stream serialization (PDL): the kernel may become resident while its predecessor in the
 // stream drains; it must call ptx::pdl_wait() before touching global memory (all kernels launched this way do).
-// WNB_PDL=0 in the environment turns the attribute off.
+// WNB_PDL=0 in the environment turns the attribute off.  cluster > 1: thread-block clusters of `cluster` CTAs along x
+// (grid a multiple of it).
 bool pdl_enabled();
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), unsigned grid, unsigned block, size_t smem, cudaStream_t st,
-                              Args&&... args) {
+                              unsigned cluster, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(block);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute attr[1];
+  cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+  attr[1].id = cudaLaunchAttributeClusterDimension;
+  attr[1].val.clusterDim.x = cluster;
+  attr[1].val.clusterDim.y = 1;
+  attr[1].val.clusterDim.z = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = 1;
+  cfg.numAttrs = cluster > 1 ? 2 : 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 

@@ -14,6 +14,13 @@
 // output; gate forward / backward epilogues for the residual blocks.  The kernel is instantiated per (N, epilogue
 // kind) so each variant gets its own register allocation.  Column blocks (tiles ordered block-fastest so the A tile
 // is shared through L2), split output and programmatic dependent launch as options.
+// Thread-block clusters (Params::cm = CM in {1, 2, 4} CTAs along x; 1 unless forced, see pick_cm for the measurements):
+// the CTAs of a cluster take CM consecutive time tiles (flattened over the batch) of the same column block, and each
+// weight box is read from L2 once per cluster: CTA r loads rows [r N/CM, (r+1) N/CM) of it (of each half, for the gate's
+// two half boxes) and multicasts them into the same ring offset of every CTA.  A stage is refilled only when the
+// consumers of every CTA have released it (one arrive per consumer warp on each CTA's empty barrier).  A CTA whose tile
+// lies past the last one still loads its weight slice and releases the stages, without MMAs or stores.  Each tile's
+// arithmetic is the same for every CM.
 // Used for: the post network forward (wavenet.py:518-523) and backward, the hoisted skip GEMMs, the gate backward,
 // the residual-stream data gradient dX (two time-shifted segments) with the aux gradient dhaux (reduce-add).
 #include <cuda.h>
@@ -22,6 +29,9 @@
 #include <string.h>
 
 #include <cuda_bf16.h>
+#include <map>
+#include <mutex>
+#include <tuple>
 #include <type_traits>
 
 #include "common.cuh"
@@ -64,6 +74,7 @@ struct alignas(64) Params {
   // column blocks (NtTcOpts::n_blocks), dz row pitch and z suppression of the gate-backward epilogue
   int nblk, gate_ld_dz, gate_skip_z;
   int rev;   // NtTcOpts::reverse
+  int cm;    // CTAs per cluster (1, 2, 4): the weight box of a stage is multicast from CM slices of N / CM rows
 };
 
 // EPI selects the epilogue at compile time so that each variant gets its own register allocation: 0 plain (bias / add /
@@ -96,18 +107,23 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
   uint64_t* empty = bars + p.nstages;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_b = (p.T + kTM - 1) / kTM;
-  const int ntiles = p.B * tiles_per_b * p.nblk;   // column block fastest: the blocks of one time tile share A via L2
+  const int ntt = p.B * tiles_per_b;   // time tiles
+  // a group = CM consecutive time tiles x one column block, column block fastest: the blocks of one time tile share A via L2
+  const int cm = p.cm, rank = blockIdx.x % cm, cluster = blockIdx.x / cm, nclusters = gridDim.x / cm;
+  const int ngroups = (ntt + cm - 1) / cm * p.nblk;
   int kchunks = 0;
   for (int s = 0; s < p.nseg; s++) kchunks += p.seg[s].K / 32;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < p.nstages; i++) {
       ptx::mbar_init(&full[i], 1);
-      ptx::mbar_init(&empty[i], kConsumers);
+      ptx::mbar_init(&empty[i], (kConsumers / 32) * cm);   // one arrive per consumer warp of every CTA of the cluster
     }
     ptx::fence_barrier_init();
   }
-  __syncthreads();
+  // the peers multicast into this CTA's ring and arrive on its barriers: all of them must see the initialised barriers
+  if (cm > 1) ptx::cluster_sync();
+  else __syncthreads();
   // programmatic dependent launch: the set-up above overlapped the previous kernel's tail; from here on this
   // kernel reads / writes memory that kernel may have produced
   ptx::pdl_launch_dependents();
@@ -117,29 +133,41 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
     // =============================== TMA producer ===============================
     if (ptx::elect_one()) {
       for (int i = 0; i < 10; i++) ptx::prefetch_tmap(&p.maps[i]);
+      const uint16_t cta_mask = (uint16_t)((1u << cm) - 1);
+      // this CTA's slice of a weight box (rows wr * rank .. of each half box) -> every CTA of the cluster
+      auto load_w = [&](unsigned char* box, const Seg& sg, int k, int n, int box_rows, uint64_t* bar) {
+        const int wr = box_rows / cm;
+        if (cm == 1) ptx::tma_load_2d(box, &p.maps[sg.bmap], bar, k, n);
+        else ptx::tma_load_2d_multicast(box + rank * wr * kWRow, &p.maps[sg.bmap], bar, k, n + rank * wr, cta_mask);
+      };
       uint32_t st = 0, ph = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const int te = p.rev ? ntiles - 1 - tile : tile;
-        const int tt = te / p.nblk, ncol0 = (te - tt * p.nblk) * N;
+      for (int grp = cluster; grp < ngroups; grp += nclusters) {
+        const int ge = p.rev ? ngroups - 1 - grp : grp;
+        const int tg = ge / p.nblk, ncol0 = (ge - tg * p.nblk) * N;
+        const int tt = tg * cm + rank;
+        const bool has_tile = tt < ntt;
         const int b = tt / tiles_per_b, t0 = (tt - b * tiles_per_b) * kTM;
         for (int s = 0; s < p.nseg; s++) {
           const Seg sg = p.seg[s];
           for (int kc = 0; kc < sg.K / 32; kc++) {
             ptx::mbar_wait(&empty[st], ph ^ 1);
-            ptx::mbar_arrive_expect_tx(&full[st], stage_bytes);
+            ptx::mbar_arrive_expect_tx(&full[st], has_tile ? stage_bytes : stage_bytes - kASub);
             unsigned char* dst = ring + (size_t)st * stage_bytes;
-            ptx::tma_load_3d(dst, &p.maps[sg.amap], &full[st], kc * 32, t0 + sg.shift, b);
+            if (has_tile) ptx::tma_load_3d(dst, &p.maps[sg.amap], &full[st], kc * 32, t0 + sg.shift, b);
             if (sg.b_n1 >= 0) {   // N = two row ranges of N/2 each (sigmoid rows, tanh rows)
-              ptx::tma_load_2d(dst + kASub, &p.maps[sg.bmap], &full[st], sg.b_k0 + kc * 32, sg.b_n0);
-              ptx::tma_load_2d(dst + kASub + (N / 2) * kWRow, &p.maps[sg.bmap], &full[st], sg.b_k0 + kc * 32, sg.b_n1);
+              load_w(dst + kASub, sg, sg.b_k0 + kc * 32, sg.b_n0, N / 2, &full[st]);
+              load_w(dst + kASub + (N / 2) * kWRow, sg, sg.b_k0 + kc * 32, sg.b_n1, N / 2, &full[st]);
             } else {
-              ptx::tma_load_2d(dst + kASub, &p.maps[sg.bmap], &full[st], sg.b_k0 + kc * 32, sg.b_n0 + ncol0);
+              load_w(dst + kASub, sg, sg.b_k0 + kc * 32, sg.b_n0 + ncol0, N, &full[st]);
             }
             if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
           }
         }
       }
     }
+    // no CTA may exit while a peer can still multicast into its ring or arrive on its barriers
+    __syncwarp();
+    if (cm > 1) ptx::cluster_sync();
     return;
   }
 
@@ -150,10 +178,28 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
   unsigned char* stg = stg_base + warp * 2 * kStg;
   const uint32_t ring_u32 = ptx::smem_u32(ring);
   uint32_t st = 0, ph = 0, nstore = 0;
-  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const int te = p.rev ? ntiles - 1 - tile : tile;
-    const int tt = te / p.nblk, ncol0 = (te - tt * p.nblk) * N;
+  // stage s may be refilled as far as this warp is concerned: one arrive on the empty barrier of every CTA of the cluster
+  auto release = [&](uint32_t s) {
+    __syncwarp();
+    if (lane == 0) {
+      if (cm == 1) ptx::mbar_arrive(&empty[s]);
+      else
+        for (int r = 0; r < cm; r++) ptx::mbar_arrive_cluster(&empty[s], (uint32_t)r);
+    }
+  };
+  for (int grp = cluster; grp < ngroups; grp += nclusters) {
+    const int ge = p.rev ? ngroups - 1 - grp : grp;
+    const int tg = ge / p.nblk, ncol0 = (ge - tg * p.nblk) * N;
+    const int tt = tg * cm + rank;
     const int b = tt / tiles_per_b, t0 = (tt - b * tiles_per_b) * kTM;
+    if (tt >= ntt) {   // past the last tile (partial last group): only keep the stages moving for the peers
+      for (int kc = 0; kc < kchunks; kc++) {
+        ptx::mbar_wait(&full[st], ph);
+        release(st);
+        if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
+      }
+      continue;
+    }
     float d[N / 2];
 #pragma unroll
     for (int i = 0; i < N / 2; i++) d[i] = 0.f;
@@ -168,7 +214,7 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
           ptx::wgmma_ss<N>(d, ptx::gmma_desc_k_sw128(a_addr + 32 * k), ptx::gmma_desc_k_sw128(b_addr + 32 * k), 1);
         ptx::wg_commit();
         ptx::wg_wait<1>();                   // the previous chunk's MMAs are done: its stage can be refilled
-        if (prev != 0xFFFFFFFFu) ptx::mbar_arrive(&empty[prev]);
+        if (prev != 0xFFFFFFFFu) release(prev);
         prev = st;
         if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
       }
@@ -193,7 +239,7 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
         for (int k = 0; k < 2; k++) ptx::wgmma_rs_bf16<N>(d, a[k], ptx::gmma_desc_k_sw64(b_addr + 32 * k), 1);
         ptx::wg_commit();
         ptx::wg_wait<1>();                 // the previous chunk's MMAs are done: its stage can be refilled
-        if (prev != 0xFFFFFFFFu) ptx::mbar_arrive(&empty[prev]);
+        if (prev != 0xFFFFFFFFu) release(prev);
         prev = st;
         if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
       };
@@ -204,7 +250,7 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
     }
     ptx::wg_wait<0>();
     ptx::wg_touch(d);
-    if (prev != 0xFFFFFFFFu) ptx::mbar_arrive(&empty[prev]);
+    if (prev != 0xFFFFFFFFu) release(prev);
     // accumulator -> shared memory (column-major), after every thread is done reading the previous tile's copy
     ptx::named_bar(1, kConsumers);
     {
@@ -399,6 +445,8 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
     }
   }
   if (lane == 0) ptx::bulk_wait<0>();
+  __syncwarp();
+  if (cm > 1) ptx::cluster_sync();
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -447,25 +495,76 @@ static bool map2_bf16(CUtensorMap* m, const __nv_bfloat16* base, int K, int Nrow
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// Clusters of cm CTAs of `kernel` that can be resident at once on the current device (a cluster lives in one GPC, so this
+// can be less than SMs x CTAs per SM / cm), cached per (device, kernel, shared memory, cm); 0 if the query fails.
+template <typename K>
+static int max_active_clusters(K kernel, size_t smem, int cm) {
+  static std::mutex mu;
+  static std::map<std::tuple<int, const void*, size_t, int>, int> fit;
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
+  const auto key = std::make_tuple(dev, reinterpret_cast<const void*>(kernel), smem, cm);
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = fit.find(key);
+  if (it != fit.end()) return it->second;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(cm);
+  cfg.blockDim = dim3(kThreadsN);
+  cfg.dynamicSmemBytes = smem;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = cm;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess) n = 0;
+  return fit[key] = n;
+}
+
+// ngroups: cluster work items (p.cm time tiles x one column block); ctas: CTAs per SM the shared memory allows
 template <int N, int EPI, typename W>
-static cudaError_t launch_n(int grid, size_t smem, cudaStream_t st, const Params& p) {
+static cudaError_t launch_n(int ngroups, int ctas, size_t smem, cudaStream_t st, const Params& p) {
   cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(gemm_nt_tc_kernel<N, EPI, W>), smem);
   if (e != cudaSuccess) return e;
-  return launch_pdl(gemm_nt_tc_kernel<N, EPI, W>, grid, kThreadsN, smem, st, p);
+  int slots = device_sms() * ctas;
+  if (p.cm > 1) {
+    slots = max_active_clusters(gemm_nt_tc_kernel<N, EPI, W>, smem, p.cm);
+    if (slots < 1) return cudaErrorInvalidConfiguration;
+  }
+  const int grid = (ngroups < slots ? ngroups : slots) * p.cm;
+  return launch_pdl(gemm_nt_tc_kernel<N, EPI, W>, grid, kThreadsN, smem, st, p.cm, p);
 }
 
 template <int EPI, typename W>
-static cudaError_t launch_epi(int N, int grid, size_t smem, cudaStream_t st, const Params& p) {
+static cudaError_t launch_epi(int N, int ngroups, int ctas, size_t smem, cudaStream_t st, const Params& p) {
   switch (N) {
-    case 32: return launch_n<32, EPI, W>(grid, smem, st, p);
-    case 64: return launch_n<64, EPI, W>(grid, smem, st, p);
-    case 96: return launch_n<96, EPI, W>(grid, smem, st, p);
-    case 128: return launch_n<128, EPI, W>(grid, smem, st, p);
-    case 160: return launch_n<160, EPI, W>(grid, smem, st, p);
-    case 192: return launch_n<192, EPI, W>(grid, smem, st, p);
-    case 224: return launch_n<224, EPI, W>(grid, smem, st, p);
-    default: return launch_n<256, EPI, W>(grid, smem, st, p);
+    case 32: return launch_n<32, EPI, W>(ngroups, ctas, smem, st, p);
+    case 64: return launch_n<64, EPI, W>(ngroups, ctas, smem, st, p);
+    case 96: return launch_n<96, EPI, W>(ngroups, ctas, smem, st, p);
+    case 128: return launch_n<128, EPI, W>(ngroups, ctas, smem, st, p);
+    case 160: return launch_n<160, EPI, W>(ngroups, ctas, smem, st, p);
+    case 192: return launch_n<192, EPI, W>(ngroups, ctas, smem, st, p);
+    case 224: return launch_n<224, EPI, W>(ngroups, ctas, smem, st, p);
+    default: return launch_n<256, EPI, W>(ngroups, ctas, smem, st, p);
   }
+}
+
+// CTAs per cluster for a launch whose weight boxes have box_rows rows (each half box, for the gate's two).
+// The default is 1 for every launch.  Measured on an H100 80GB HBM3 (power limit not reported), bench.py's step
+// (8 x 23 040, ms per step for the kind, CM = 1 / 2 / 4): skip GEMM 1.94 / 2.19 / 2.40, dZ_all 1.84 / 1.78 / 2.10, gate backward 4.62 / 4.77 /
+// 5.24, dx 3.97 / 4.28 / 4.68; whole step 24.9 / 25.5 / 27.2 ms.  Halving the weight bytes pulled from L2 does not pay
+// for the cluster-wide coupling of the ring while a tile's epilogue still runs after its mainloop in the same warpgroup.
+// WNB_NT_CLUSTER=1, 2 or 4 in the environment forces CM (tests, A/B timing); it is read on every call.  Either way CM is
+// halved until each CTA's slice of a box is a whole number of 8-row swizzle atoms (1024 B tf32, 512 B bf16), the
+// alignment at which a slice lands in the same swizzled layout as the whole box.
+static int pick_cm(int box_rows) {
+  const char* e = getenv("WNB_NT_CLUSTER");
+  int cm = 1;
+  if (e && (e[0] == '1' || e[0] == '2' || e[0] == '4') && e[1] == 0) cm = e[0] - '0';
+  while (cm > 1 && box_rows % (8 * cm) != 0) cm /= 2;
+  return cm;
 }
 
 }  // namespace nt
@@ -491,6 +590,7 @@ int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, con
     p.nblk = 2;
   }
   const int nbox = gate ? N / 2 : N;   // (gate: two boxes of GC = N/2 rows, sigmoid rows and tanh rows)
+  p.cm = pick_cm(nbox);                // (each CTA of a cluster loads nbox / cm rows of each box)
   const bool bf16 = segs[0].wb != nullptr;
   for (int s = 0; s < nseg; s++) {
     if (segs[s].K % 32 != 0) { set_error("gemm_nt_tc: K must be a multiple of 32"); return WNB_ERR_INVALID; }
@@ -503,8 +603,8 @@ int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, con
       return WNB_ERR_INVALID;
     }
     if (!map3(&p.maps[s], segs[s].a, segs[s].CA, T, B, kTM) ||
-        !(bf16 ? map2_bf16(&p.maps[4 + s], segs[s].wb, segs[s].w_cols, segs[s].w_rows, nbox)
-               : map2(&p.maps[4 + s], segs[s].w, segs[s].w_cols, segs[s].w_rows, nbox))) {
+        !(bf16 ? map2_bf16(&p.maps[4 + s], segs[s].wb, segs[s].w_cols, segs[s].w_rows, nbox / p.cm)
+               : map2(&p.maps[4 + s], segs[s].w, segs[s].w_cols, segs[s].w_rows, nbox / p.cm))) {
       set_error("gemm_nt_tc: tensor map creation failed");
       return WNB_ERR_CUDA;
     }
@@ -572,17 +672,15 @@ int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, con
   if (nst < 2) { set_error("gemm_nt_tc: N too large"); return WNB_ERR_INVALID; }
   p.nstages = nst;
   const size_t smem = (size_t)fixed + (size_t)nst * stage_bytes;
-  const int sms = device_sms();
-  const int ntiles = B * ((T + kTM - 1) / kTM) * p.nblk;
-  const int grid = ntiles < sms * ctas ? ntiles : sms * ctas;
+  const int ngroups = cdiv(B * cdiv(T, kTM), p.cm) * p.nblk;
   cudaError_t le;
   if (bf16) {   // (the gate backward without z belongs to the tf32 stack only)
-    if (epi == EPI_PLAIN) le = launch_epi<EPI_PLAIN, __nv_bfloat16>(N, grid, smem, st, p);
-    else if (epi == EPI_GATE) le = launch_epi<EPI_GATE, __nv_bfloat16>(N, grid, smem, st, p);
+    if (epi == EPI_PLAIN) le = launch_epi<EPI_PLAIN, __nv_bfloat16>(N, ngroups, ctas, smem, st, p);
+    else if (epi == EPI_GATE) le = launch_epi<EPI_GATE, __nv_bfloat16>(N, ngroups, ctas, smem, st, p);
     else { set_error("gemm_nt_tc: no bf16 variant of the gate backward without z"); return WNB_ERR_INVALID; }
-  } else if (epi == EPI_PLAIN) le = launch_epi<EPI_PLAIN, float>(N, grid, smem, st, p);
-  else if (epi == EPI_GATE) le = launch_epi<EPI_GATE, float>(N, grid, smem, st, p);
-  else le = launch_epi<EPI_GATE_BWD_NOZ, float>(N, grid, smem, st, p);
+  } else if (epi == EPI_PLAIN) le = launch_epi<EPI_PLAIN, float>(N, ngroups, ctas, smem, st, p);
+  else if (epi == EPI_GATE) le = launch_epi<EPI_GATE, float>(N, ngroups, ctas, smem, st, p);
+  else le = launch_epi<EPI_GATE_BWD_NOZ, float>(N, ngroups, ctas, smem, st, p);
   if (le != cudaSuccess) { set_error("gemm_nt_tc: launch failed: %s", cudaGetErrorString(le)); return WNB_ERR_CUDA; }
   WNB_CHECK_LAUNCH("gemm_nt_tc");
   return WNB_OK;

@@ -487,7 +487,7 @@ int resblock_fwd_z(const float* xin, const float* haux, const float* w1, const f
   if (!sched) { set_error("resblock_fwd_z: cannot allocate the scheduler words"); return WNB_ERR_CUDA; }
   const int ntiles = B * ((T + kTM - 1) / kTM);
   const int grid = ntiles < sms ? ntiles : sms;
-  if (launch_pdl(resblock_fwd_z_kernel, grid, kThreadsZ, kSmemBytes, st, maps, b1, b2res ? b2res : b1, B, T, d,
+  if (launch_pdl(resblock_fwd_z_kernel, grid, kThreadsZ, kSmemBytes, st, 1, maps, b1, b2res ? b2res : b1, B, T, d,
                  xout ? 1 : 0, zcol0, sched, reverse ? 1 : 0) != cudaSuccess) { /* reported below */ }
   WNB_CHECK_LAUNCH("resblock_fwd_z");
   return WNB_OK;
@@ -520,7 +520,7 @@ int resblock_fwd_skip(const float* xin, const float* haux, const float* w1, cons
   if (!sched) { set_error("resblock_fwd: cannot allocate the scheduler words"); return WNB_ERR_CUDA; }
   const int ntiles = B * ((T + kTM - 1) / kTM);
   const int grid = ntiles < sms ? ntiles : sms;
-  if (launch_pdl(resblock_fwd_skip_kernel, grid, tcs::kSThreads, tcs::kSSmemBytes, st, maps, b1, b2, B, T, S, d,
+  if (launch_pdl(resblock_fwd_skip_kernel, grid, tcs::kSThreads, tcs::kSSmemBytes, st, 1, maps, b1, b2, B, T, S, d,
                  xout ? 1 : 0, skip_init, sched) != cudaSuccess) { /* reported below */ }
   WNB_CHECK_LAUNCH("resblock_fwd_skip");
   return WNB_OK;

@@ -43,6 +43,18 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// arrive on the barrier at the same shared-memory offset as `bar` in CTA `rank` of the cluster.  Default (.release.cta)
+// semantics: this releases a stage whose shared-memory reads are already complete (wgmma wait_group), so no cluster-scope
+// release is needed -- .release.cluster would put a MEMBAR.ALL.GPU in front of every arrive.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
+// every thread of every CTA of the cluster; makes barrier initialisation and shared-memory writes visible cluster-wide
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
@@ -62,6 +74,9 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 // Bounded waits: a protocol bug must trap (error returned to the host) instead of hanging the GPU -- but the bound is
 // WALL-CLOCK time (20 s on %globaltimer, looked at every 64 K polls), not a poll count: under a profiler's kernel
 // replay, time slicing or preemption a healthy kernel can sit on a barrier for many millions of polls.
+// The time-out path makes no function call unless WNB_WAIT_PRINTF is defined (a debugging build that prints the block
+// and thread of the time-out): a call (printf) inside a wgmma pipeline makes ptxas serialise every wgmma.mma_async of
+// the kernel (note C7510), which is what the tensor-core kernels would pay for the message in every build.
 __device__ __forceinline__ uint64_t globaltimer_ns() {
   uint64_t t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -82,7 +97,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   SpinGuard guard;
   while (!mbar_try_wait(bar, parity)) {
     if (guard.expired()) {
+#ifdef WNB_WAIT_PRINTF
       printf("wnb200: mbarrier wait timed out after 20 s (block %d thread %d)\n", blockIdx.x, threadIdx.x);
+#endif
       __trap();
     }
   }
@@ -96,6 +113,16 @@ __device__ __forceinline__ void tma_load_2d(void* smem, const CUtensorMap* m, ui
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(smem)), "l"((uint64_t)m), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+// the same box written to the same shared-memory offset of every CTA of the cluster in `cta_mask`; each destination's
+// barrier at `bar`'s offset receives the box's bytes
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                      uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(smem)), "l"((uint64_t)m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(void* smem, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {

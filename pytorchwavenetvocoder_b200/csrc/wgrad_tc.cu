@@ -316,7 +316,7 @@ template <int N, bool BF16>
 static cudaError_t launch_n(int grid, size_t smem, cudaStream_t st, const Params& p) {
   cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(wgrad_tc_kernel<N, BF16>), smem);
   if (e != cudaSuccess) return e;
-  return launch_pdl(wgrad_tc_kernel<N, BF16>, grid, kThreadsW, smem, st, p);
+  return launch_pdl(wgrad_tc_kernel<N, BF16>, grid, kThreadsW, smem, st, 1, p);
 }
 
 template <bool BF16>
