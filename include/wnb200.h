@@ -322,6 +322,10 @@ WNB_API int wnb_decode_warp(int32_t* xs, const float* h, const float* up_w, cons
  * on both */
 WNB_API int wnb_decode_warp_plan(int B);
 WNB_API int wnb_decode_warp_cluster(int B);
+/* the kernel instantiation decode_warp_kernel<NU, W, BIG, CL> that wnb_decode_warp runs for B utterances of L layers,
+ * under the current WNB_DECODE_BIG: form[0..3] = NU (utterances per CTA), W (consumer warps), CL (CTAs per cluster),
+ * BIG (1: three 64 KB ring slots, 0: up to six 32 KB slots).  WNB_ERR_UNSUPPORTED when no ring fits. */
+WNB_API int wnb_decode_warp_form(int B, int L, int32_t* form);
 
 #ifdef __cplusplus
 }

@@ -322,11 +322,15 @@ def _pick(logits_row, mode, u):
         # inverse-CDF categorical draw from softmax(logits) with the supplied uniform u
         # (the reference uses torch.distributions.Categorical, wavenet.py:377-379, whose RNG
         #  stream cannot be reproduced outside torch; distribution is what is pinned)
+        # A target below the total lands on a class whose cumulative sum rises past it, so of nonzero probability; a
+        # target at or past the total (u >= 1) takes the last class of nonzero probability, like the kernels.
         m = logits_row.max()
         e = np.exp((logits_row - m).astype(np.float32))
         c = np.cumsum(e, dtype=np.float32)
         k = int(np.searchsorted(c, np.float32(u) * c[-1], side="right"))
-        return min(k, logits_row.shape[0] - 1)
+        if k >= logits_row.shape[0]:
+            k = int(np.nonzero(e > 0)[0][-1])
+        return k
     raise ValueError("mode should be sampling or argmax")
 
 

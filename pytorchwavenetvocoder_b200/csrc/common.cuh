@@ -103,4 +103,41 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// Inverse-CDF pick of the three decode kernels, called by all 32 lanes of a warp.  Each lane owns consecutive classes
+// (lane order = class order) with e_q = expf(l_q - max) summing to `lsum`; `incl` is the inclusive shuffle scan of the
+// lanes' lsum, `lnz` the lane's last class with e_q > 0 (-1 if none), `uni` in [0, 1).  `walk(start, target)` returns
+// the lane's first class with e_q > 0 whose running sum from start passes target, or -1.
+// A lane claims target = uni * total when excl <= target < incl, with excl = the previous lane's incl (0 on lane 0):
+// bit-equal neighbours, so no target below the total falls between two lanes.  The scan's sums are not monotone in
+// the lane (a lane of zero mass can end a rounding step above its predecessor), but the first lane whose incl exceeds
+// the target always claims it, and overlapping claims take the lowest class.  The walk starts from incl - lsum, which
+// can differ from excl by rounding: every target that lane's own interval [incl - lsum, incl) held before the claim
+// test used excl picks what it picked then.  A walk that never passes the target picks the last class with e_q > 0 at
+// or before its lane; a target no lane claims (>= total), the row's last such class.  So the pick always has nonzero
+// probability.
+template <class Walk>
+__device__ __forceinline__ int sample_pick(float incl, float lsum, int lnz, float uni, int lane, Walk walk) {
+  float excl = __shfl_up_sync(0xffffffffu, incl, 1);
+  if (lane == 0) excl = 0.f;
+  const float total = __shfl_sync(0xffffffffu, incl, 31);
+  const float target = uni * total;
+  const bool claim = target >= excl && target < incl;
+  int cand = claim ? walk(incl - lsum, target) : 0x7fffffff;
+  const bool fell = cand < 0;
+  const unsigned claims = __ballot_sync(0xffffffffu, claim);
+  if (claims == 0u || __any_sync(0xffffffffu, fell)) {   // rare: a target within rounding of a lane's upper end
+    int pl = lnz;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, pl, o);
+      if (lane >= o) pl = max(pl, v);
+    }
+    if (fell) cand = pl;
+    if (claims == 0u) cand = __shfl_sync(0xffffffffu, pl, 31);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) cand = min(cand, __shfl_xor_sync(0xffffffffu, cand, o));
+  return cand;
+}
+
 }  // namespace wnb

@@ -363,28 +363,27 @@ __global__ void __launch_bounds__(kStreamThreads, 1) decode_stream_kernel(const 
             uni = (float)(rr[0] >> 8) * (1.0f / 16777216.0f);
           }
           float lsum = 0.f;
-          for (int q = q0; q < q1; q++) lsum += expf(lg[q] - best);
+          int lnz = -1;
+          for (int q = q0; q < q1; q++) {
+            const float e = expf(lg[q] - best);
+            lsum += e;
+            if (e > 0.f) lnz = q;
+          }
           float incl = lsum;
 #pragma unroll
           for (int o = 1; o < 32; o <<= 1) {
             const float v = __shfl_up_sync(0xffffffffu, incl, o);
             if (lane >= o) incl += v;
           }
-          const float total = __shfl_sync(0xffffffffu, incl, 31);
-          const float target = uni * total;
-          const float excl = incl - lsum;
-          int cand = 0x7fffffff;
-          if (q0 < Q && target < incl && target >= excl) {
-            float c = excl;
-            cand = q1 - 1;
+          pick = sample_pick(incl, lsum, lnz, uni, lane, [&](float start, float target) {   // (common.cuh)
+            float c = start;
             for (int q = q0; q < q1; q++) {
-              c += expf(lg[q] - best);
-              if (c > target) { cand = q; break; }
+              const float e = expf(lg[q] - best);
+              c += e;
+              if (c > target && e > 0.f) return q;
             }
-          }
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) cand = min(cand, __shfl_xor_sync(0xffffffffu, cand, o));
-          pick = (cand == 0x7fffffff) ? Q - 1 : cand;
+            return -1;
+          });
         }
         if (lane == 0 && u0 + u < p.B && i < s_n[u]) p.xs[(size_t)(u0 + u) * stride_xs + pos + 1] = pick;
       }

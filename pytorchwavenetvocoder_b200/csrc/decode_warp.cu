@@ -760,33 +760,30 @@ __global__ void __launch_bounds__((W / CL) * 32 + 64, 1) decode_warp_kernel(cons
           }
           float ex[8];
           float lsum = 0.f;
+          int lnz = -1;                         // this lane's last class of nonzero probability
 #pragma unroll
-          for (int k = 0; k < 8; k++) { ex[k] = expf(lg8[k] - best); lsum += ex[k]; }
+          for (int k = 0; k < 8; k++) {
+            ex[k] = expf(lg8[k] - best);
+            lsum += ex[k];
+            if (ex[k] > 0.f) lnz = q0 + k;
+          }
           float incl = lsum;
 #pragma unroll
           for (int o = 1; o < 32; o <<= 1) {
             const float v = __shfl_up_sync(0xffffffffu, incl, o);
             if (lane >= o) incl += v;
           }
-          const float total = __shfl_sync(0xffffffffu, incl, 31);
-          const float target = uni * total;
-          const float excl = incl - lsum;
-          int cand = 0x7fffffff;
-          if (target < incl && target >= excl) {
-            float c = excl;
-            cand = q1 - 1;
+          pick = sample_pick(incl, lsum, lnz, uni, lane, [&](float start, float target) {   // (common.cuh)
+            int c = -1;
 #pragma unroll
-            for (int k = 7; k >= 0; k--) {      // first k (ascending) whose running sum passes the target
-              float ck = excl;
+            for (int k = 7; k >= 0; k--) {      // first k (ascending) with e > 0 whose running sum passes the target
+              float ck = start;
 #pragma unroll
               for (int m = 0; m <= k; m++) ck += ex[m];
-              if (ck > target) cand = q0 + k;
+              if (ck > target && ex[k] > 0.f) c = q0 + k;
             }
-            (void)c;
-          }
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) cand = min(cand, __shfl_xor_sync(0xffffffffu, cand, o));
-          pick = (cand == 0x7fffffff) ? kQ - 1 : cand;
+            return c;
+          });
         }
         // (CL == 2: both CTAs hold the same 256 logits and make the same pick; each writes it -- same value -- so
         //  that its own next prologue reads what it wrote, no cross-CTA dependency on global memory)
@@ -827,6 +824,21 @@ static void decode_warp_plan(int B, int* NU, int* W, int* CL) {
   *CL = (cl_on && B <= device_sms() / 2) ? 2 : 1;
 }
 
+// ring slots for NU utterances per CTA and L layers, given the per-CTA work space: three 64 KB slots (half as many
+// mbarrier round trips per step) when they fit and WNB_DECODE_BIG is not 0, else up to six 32 KB slots.  False when
+// fewer than three fit.  Shared by the launcher and wnb_decode_warp_form.
+static bool decode_warp_slots(int NU, int L, int* nslot, bool* big, size_t* work) {
+  using namespace dw;
+  *work = ((size_t)NU * (kR * 3 + kAp + 2 * kS + kQ + (size_t)L * kR) + 128 * NU) * sizeof(float);
+  const long avail = 227L * 1024 - 256 - (long)*work - 16 * 16;
+  const char* eb = getenv("WNB_DECODE_BIG");
+  *big = avail >= 3L * 2 * kSlot && !(eb && atoi(eb) == 0);
+  int n = *big ? 3 : (int)(avail / kSlot);
+  if (n > 6) n = 6;
+  *nslot = n;
+  return n >= 3;
+}
+
 int decode_warp_launch(dw::Params& p, int W_packed, int CL_packed, cudaStream_t st) {
   using namespace dw;
   int NU, W, CL;
@@ -838,14 +850,10 @@ int decode_warp_launch(dw::Params& p, int W_packed, int CL_packed, cudaStream_t 
   }
   p.rank_stride = (long long)((size_t)p.L * (kLayerFloats - (CL - 1) * (kW1Floats / 2 + kWresFloats / 2 + kWskipFloats / 2)) +
                               kPBiasFloats + (kP1Floats + kP2Floats) / CL);
-  const size_t work = ((size_t)NU * (kR * 3 + kAp + 2 * kS + kQ + (size_t)p.L * kR) + 128 * NU) * sizeof(float);
-  const long avail = 227L * 1024 - 256 - (long)work - 16 * 16;
-  // three 64 KB slots (half as many mbarrier round trips per step) when they fit, else up to six 32 KB slots
-  const char* eb = getenv("WNB_DECODE_BIG");
-  const bool big = avail >= 3L * 2 * kSlot && !(eb && atoi(eb) == 0);
-  int nslot = big ? 3 : (int)(avail / kSlot);
-  if (nslot > 6) nslot = 6;
-  if (nslot < 3) return WNB_ERR_UNSUPPORTED;
+  int nslot;
+  bool big;
+  size_t work;
+  if (!decode_warp_slots(NU, p.L, &nslot, &big, &work)) return WNB_ERR_UNSUPPORTED;
   p.nslot = nslot;
   p.big = big ? 1 : 0;
   {
@@ -924,6 +932,23 @@ WNB_API int wnb_decode_warp_cluster(int B) {
   int NU, W, CL;
   decode_warp_plan(B, &NU, &W, &CL);
   return CL;
+}
+
+// the decode_warp_kernel<NU, W, BIG, CL> instantiation the launcher would run for B utterances and L layers, under the
+// current WNB_DECODE_BIG: form[0..3] = NU, W, CL, BIG (0 / 1).  WNB_ERR_UNSUPPORTED when no ring fits.
+WNB_API int wnb_decode_warp_form(int B, int L, int32_t* form) {
+  WNB_REQUIRE(B > 0 && L >= 1 && L <= dw::kMaxL, "decode_warp_form: bad shape");
+  WNB_REQUIRE(form, "decode_warp_form: null pointer");
+  int NU, W, CL, nslot;
+  bool big;
+  size_t work;
+  decode_warp_plan(B, &NU, &W, &CL);
+  if (!decode_warp_slots(NU, L, &nslot, &big, &work)) {
+    set_error("decode_warp_form: not enough shared memory for this depth");
+    return WNB_ERR_UNSUPPORTED;
+  }
+  form[0] = NU; form[1] = W; form[2] = CL; form[3] = big ? 1 : 0;
+  return WNB_OK;
 }
 
 WNB_API int wnb_decode_warp(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
