@@ -2,25 +2,33 @@
 //     D[t][n] = epi( sum_seg sum_k A_seg[t + shift_seg][k] * W_seg[n][k] )          n < N <= 256 per tile
 // A rows are time steps (K-major operand straight from the (B,T,C) tensor, TMA zero fill outside [0,T) =
 // causal / anti-causal padding), W is a row-major [N][K] weight matrix (K-major operand).  Hopper wgmma
-// m64nNk8 tf32, fp32 accumulate in registers of one consumer warpgroup; one producer warp streams
-// [64 x 32] activation boxes and [N x 32] weight boxes through an mbarrier ring with TMA.
+// m64nNk8 tf32, fp32 accumulate in registers.  A CTA has one producer warpgroup and two consumer warpgroups and works on
+// pairs of consecutive 64-row time tiles (flattened over the batch) of one column block: one producer thread streams,
+// per stage of an mbarrier ring, the two tiles' [64 x 32] activation boxes and ONE [N x 32] weight box with TMA, and each
+// consumer warpgroup multiplies its own activation box by the shared weight box.  So a weight box is pulled from L2 once
+// per 128 time rows.  A pair whose second tile lies past the last one leaves that warpgroup with nothing but releasing
+// the stages.  setmaxnreg gives the consumers 232 registers (N = 256: 128 accumulator registers) and the producer 40.
 // bf16 operands (W = __nv_bfloat16): the weights arrive as bf16 [N x 32] boxes (a bf16 copy made by the caller, 64B
 // swizzle); the activation box is still fp32, and the consumers read two adjacent k per shared-memory load, round them
 // to bf16 (cvt.rn.bf16x2) into the register A fragment of wgmma m64nNk16 (bf16, fp32 accumulate).  The epilogues are
 // the same: the accumulator is fp32 either way.
-// Epilogue: the accumulator is written to shared memory column-major, then each consumer thread owns one time row
-// and 32-column chunks (warp w: rows 32 (w & 1) .., chunks w >> 1, (w >> 1) + 2, ...): + bias, ReLU, * (mask > 0),
-// + residual, then a swizzled per-warp staging box and a TMA store or TMA reduce-add (.add.f32) into the (B,T,N)
-// output; gate forward / backward epilogues for the residual blocks.  The kernel is instantiated per (N, epilogue
-// kind) so each variant gets its own register allocation.  Column blocks (tiles ordered block-fastest so the A tile
-// is shared through L2), split output and programmatic dependent launch as options.
+// Epilogue, straight from the accumulator registers: in the m64nN fragment a thread holds rows 16 w + lane/4 (+ 8) and
+// column pairs 8 j + 2 (lane % 4) (+ 1), so the tanh partner of gate column c (c + GC) and the dz partial (c + 2 GC) sit
+// in the same thread.  + bias, + residual, ReLU, * (mask > 0), or the gate forward / backward, then each warp writes its
+// 16 rows x 32 columns into a swizzled staging box and one lane issues a TMA store or TMA reduce-add (.add.f32) into the
+// (B,T,N) output.  The epilogue operand read from memory per tile (the gate backward's dz, the residual added to the
+// plain epilogue when it is at most 64 columns wide) is loaded by TMA into a buffer per warpgroup when the tile's
+// mainloop starts, so its latency hides behind the MMAs; rows past T come back as zero fill.  Bias and mask are read
+// with __ldg.  The kernel is instantiated per (N, epilogue kind, operand type) so each variant gets its own register
+// allocation.  Column blocks (work items ordered block-fastest so the A tiles are shared through L2), split output and
+// programmatic dependent launch as options.
 // Thread-block clusters (Params::cm = CM in {1, 2, 4} CTAs along x; 1 unless forced, see pick_cm for the measurements):
-// the CTAs of a cluster take CM consecutive time tiles (flattened over the batch) of the same column block, and each
-// weight box is read from L2 once per cluster: CTA r loads rows [r N/CM, (r+1) N/CM) of it (of each half, for the gate's
-// two half boxes) and multicasts them into the same ring offset of every CTA.  A stage is refilled only when the
-// consumers of every CTA have released it (one arrive per consumer warp on each CTA's empty barrier).  A CTA whose tile
-// lies past the last one still loads its weight slice and releases the stages, without MMAs or stores.  Each tile's
-// arithmetic is the same for every CM.
+// the CTAs of a cluster take CM consecutive tile pairs of the same column block, and each weight box is read from L2
+// once per cluster: CTA r loads rows [r N/CM, (r+1) N/CM) of it (of each half, for the gate's two half boxes) and
+// multicasts them into the same ring offset of every CTA.  A stage is refilled only when the consumers of both
+// warpgroups of every CTA have released it (one arrive per consumer warp on each CTA's empty barrier).  A CTA whose
+// pair lies past the last one still loads its weight slice and releases the stages, without MMAs or stores.  Each
+// tile's arithmetic is the same for every CM.
 // Used for: the post network forward (wavenet.py:518-523) and backward, the hoisted skip GEMMs, the gate backward,
 // the residual-stream data gradient dX (two time-shifted segments) with the aux gradient dhaux (reduce-add).
 #include <cuda.h>
@@ -42,19 +50,20 @@ namespace wnb {
 namespace nt {
 
 constexpr int kTM = 64;                  // time rows per tile (wgmma M)
-constexpr int kASub = kTM * 32 * 4;      // 8 KB
-constexpr int kStg = 32 * 32 * 4;        // 4 KB
-constexpr int kConsumers = 128;          // one warpgroup: MMA + epilogue
-constexpr int kThreadsN = kConsumers + 32;
-constexpr int kAccLd = kTM + 4;          // column pitch (floats) of the shared-memory accumulator: conflict-free both ways
-// bytes of the accumulator copy, rounded up so that the staging boxes behind it keep the 1024-byte alignment the
-// 128B-swizzled TMA stores need
-__host__ __device__ constexpr int acc_bytes(int N) { return (N * kAccLd * 4 + 1023) & ~1023; }
+constexpr int kASub = kTM * 32 * 4;      // 8 KB: one tile's activation box of a stage
+constexpr int kStgRows = 16;             // rows of a staging box: one warp's share of the fragment
+constexpr int kStg = kStgRows * 32 * 4;  // 2 KB
+constexpr int kStgBytes = 8 * 2 * kStg;  // 8 consumer warps x 2 staging boxes
+constexpr int kEopBox = kTM * 32 * 4;    // 8 KB: [64 x 32] box of the epilogue operand
+constexpr int kMaxEop = 2;               // epilogue operand boxes per warpgroup (64 columns)
+constexpr int kWG = 128;
+constexpr int kConsumers = 2 * kWG;      // two warpgroups: MMA + epilogue, one tile each
+constexpr int kThreadsN = kConsumers + kWG;   // + the producer warpgroup (one thread issues TMA)
 constexpr int kMaxSeg = 4;
 
 struct Seg { int amap; int shift; int K; int bmap; int b_k0; int b_n0; int b_n1; };   // b_n1 >= 0: rows of the 2nd half of N
 struct alignas(64) Params {
-  CUtensorMap maps[10];   // [0..3] A tensors, [4..7] weight matrices, [8] output, [9] second output
+  CUtensorMap maps[11];   // [0..3] A tensors, [4..7] weight matrices, [8] output, [9] second output, [10] epilogue operand
   Seg seg[kMaxSeg];
   int nseg, N, T, B, nstages;
   const float* bias; const float* mask; int ldmask; const float* add; int ldadd;
@@ -75,17 +84,14 @@ struct alignas(64) Params {
   int nblk, gate_ld_dz, gate_skip_z;
   int rev;   // NtTcOpts::reverse
   int cm;    // CTAs per cluster (1, 2, 4): the weight box of a stage is multicast from CM slices of N / CM rows
+  // [64 x 32] boxes of the epilogue operand (gate dz, or the plain epilogue's add) staged per tile through maps[10]
+  // (0: read with __ldg)
+  int neop;
 };
 
 // EPI selects the epilogue at compile time so that each variant gets its own register allocation: 0 plain (bias / add /
 // ReLU / mask / split output), 1 gate forward and gate backward with z output, 2 gate backward without z (the stack path).
 enum { EPI_PLAIN = 0, EPI_GATE = 1, EPI_GATE_BWD_NOZ = 2 };
-
-// 16 consecutive accumulator columns of one row out of the column-major shared-memory copy
-__device__ __forceinline__ void acc_ld16(const float* acc, int col, int row, float (&v)[16]) {
-#pragma unroll
-  for (int i = 0; i < 16; i++) v[i] = acc[(col + i) * kAccLd + row];
-}
 
 // bytes of one weight row of a stage (32 k): fp32 (read as tf32) or bf16
 template <typename W>
@@ -98,19 +104,21 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr bool kBf16 = std::is_same<W, __nv_bfloat16>::value;
   constexpr int kWRow = w_row_bytes<W>();
-  constexpr int stage_bytes = kASub + N * kWRow;
+  constexpr int stage_bytes = 2 * kASub + N * kWRow;   // [A box tile 0 | A box tile 1 | weight box]
   unsigned char* ring = smem;
-  float* accs = reinterpret_cast<float*>(ring + (size_t)p.nstages * stage_bytes);
-  unsigned char* stg_base = reinterpret_cast<unsigned char*>(accs) + acc_bytes(N);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(stg_base + 4 * 2 * kStg);
+  unsigned char* stg_base = ring + (size_t)p.nstages * stage_bytes;
+  unsigned char* eop_base = stg_base + kStgBytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(eop_base + 2 * p.neop * kEopBox);
   uint64_t* full = bars;
   uint64_t* empty = bars + p.nstages;
+  uint64_t* eop_full = bars + 2 * p.nstages;   // [2]: one per consumer warpgroup
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_b = (p.T + kTM - 1) / kTM;
   const int ntt = p.B * tiles_per_b;   // time tiles
-  // a group = CM consecutive time tiles x one column block, column block fastest: the blocks of one time tile share A via L2
+  const int npairs = (ntt + 1) / 2;
+  // a group = CM consecutive tile pairs x one column block, column block fastest: the blocks of one pair share A via L2
   const int cm = p.cm, rank = blockIdx.x % cm, cluster = blockIdx.x / cm, nclusters = gridDim.x / cm;
-  const int ngroups = (ntt + cm - 1) / cm * p.nblk;
+  const int ngroups = (npairs + cm - 1) / cm * p.nblk;
   int kchunks = 0;
   for (int s = 0; s < p.nseg; s++) kchunks += p.seg[s].K / 32;
 
@@ -119,6 +127,8 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
       ptx::mbar_init(&full[i], 1);
       ptx::mbar_init(&empty[i], (kConsumers / 32) * cm);   // one arrive per consumer warp of every CTA of the cluster
     }
+    ptx::mbar_init(&eop_full[0], 1);
+    ptx::mbar_init(&eop_full[1], 1);
     ptx::fence_barrier_init();
   }
   // the peers multicast into this CTA's ring and arrive on its barriers: all of them must see the initialised barriers
@@ -129,10 +139,11 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
   ptx::pdl_launch_dependents();
   ptx::pdl_wait();
 
-  if (warp == 4) {
-    // =============================== TMA producer ===============================
-    if (ptx::elect_one()) {
-      for (int i = 0; i < 10; i++) ptx::prefetch_tmap(&p.maps[i]);
+  if (warp >= kConsumers / 32) {
+    // =============================== TMA producer warpgroup ===============================
+    ptx::setmaxnreg_dec<40>();
+    if (warp == kConsumers / 32 && ptx::elect_one()) {
+      for (int i = 0; i < 11; i++) ptx::prefetch_tmap(&p.maps[i]);
       const uint16_t cta_mask = (uint16_t)((1u << cm) - 1);
       // this CTA's slice of a weight box (rows wr * rank .. of each half box) -> every CTA of the cluster
       auto load_w = [&](unsigned char* box, const Seg& sg, int k, int n, int box_rows, uint64_t* bar) {
@@ -144,21 +155,25 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
       for (int grp = cluster; grp < ngroups; grp += nclusters) {
         const int ge = p.rev ? ngroups - 1 - grp : grp;
         const int tg = ge / p.nblk, ncol0 = (ge - tg * p.nblk) * N;
-        const int tt = tg * cm + rank;
-        const bool has_tile = tt < ntt;
-        const int b = tt / tiles_per_b, t0 = (tt - b * tiles_per_b) * kTM;
+        const int tt0 = 2 * (tg * cm + rank);   // the pair's first tile; the second is tt0 + 1
+        const int ntiles = tt0 + 1 < ntt ? 2 : (tt0 < ntt ? 1 : 0);
+        int tb[2], tt[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++) { tb[h] = (tt0 + h) / tiles_per_b; tt[h] = (tt0 + h - tb[h] * tiles_per_b) * kTM; }
         for (int s = 0; s < p.nseg; s++) {
           const Seg sg = p.seg[s];
           for (int kc = 0; kc < sg.K / 32; kc++) {
-            ptx::mbar_wait(&empty[st], ph ^ 1);
-            ptx::mbar_arrive_expect_tx(&full[st], has_tile ? stage_bytes : stage_bytes - kASub);
+            ptx::mbar_wait<ptx::kStoreFault>(&empty[st], ph ^ 1);
+            ptx::mbar_arrive_expect_tx(&full[st], stage_bytes - (2 - ntiles) * kASub);
             unsigned char* dst = ring + (size_t)st * stage_bytes;
-            if (has_tile) ptx::tma_load_3d(dst, &p.maps[sg.amap], &full[st], kc * 32, t0 + sg.shift, b);
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+              if (h < ntiles) ptx::tma_load_3d(dst + h * kASub, &p.maps[sg.amap], &full[st], kc * 32, tt[h] + sg.shift, tb[h]);
             if (sg.b_n1 >= 0) {   // N = two row ranges of N/2 each (sigmoid rows, tanh rows)
-              load_w(dst + kASub, sg, sg.b_k0 + kc * 32, sg.b_n0, N / 2, &full[st]);
-              load_w(dst + kASub + (N / 2) * kWRow, sg, sg.b_k0 + kc * 32, sg.b_n1, N / 2, &full[st]);
+              load_w(dst + 2 * kASub, sg, sg.b_k0 + kc * 32, sg.b_n0, N / 2, &full[st]);
+              load_w(dst + 2 * kASub + (N / 2) * kWRow, sg, sg.b_k0 + kc * 32, sg.b_n1, N / 2, &full[st]);
             } else {
-              load_w(dst + kASub, sg, sg.b_k0 + kc * 32, sg.b_n0 + ncol0, N, &full[st]);
+              load_w(dst + 2 * kASub, sg, sg.b_k0 + kc * 32, sg.b_n0 + ncol0, N, &full[st]);
             }
             if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
           }
@@ -171,13 +186,15 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
     return;
   }
 
-  // =============================== consumer warpgroup: wgmma mainloop + epilogue ===============================
-  const int q = warp & 1;                 // rows 32 q .. 32 q + 31 of the tile in the epilogue
-  const int hf = warp >> 1;               // 0 / 1: this warp takes 32-column chunks hf, hf + 2, ...
-  const int row = q * 32 + lane;
+  // =============================== consumer warpgroups: wgmma mainloop + epilogue ===============================
+  ptx::setmaxnreg_inc<232>();
+  const int wg = warp >> 2;               // warpgroup: tile wg of each pair
+  const int wq = warp & 3;                // warp in the warpgroup: rows 16 wq .. 16 wq + 15 of the tile
+  const int rq = lane >> 2, cq = 2 * (lane & 3);   // fragment row (+ 8) and column pair (+ 8 j) of this thread
   unsigned char* stg = stg_base + warp * 2 * kStg;
+  unsigned char* eop = eop_base + wg * p.neop * kEopBox;
   const uint32_t ring_u32 = ptx::smem_u32(ring);
-  uint32_t st = 0, ph = 0, nstore = 0;
+  uint32_t st = 0, ph = 0, nstore = 0, eph = 0;
   // stage s may be refilled as far as this warp is concerned: one arrive on the empty barrier of every CTA of the cluster
   auto release = [&](uint32_t s) {
     __syncwarp();
@@ -190,15 +207,24 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
   for (int grp = cluster; grp < ngroups; grp += nclusters) {
     const int ge = p.rev ? ngroups - 1 - grp : grp;
     const int tg = ge / p.nblk, ncol0 = (ge - tg * p.nblk) * N;
-    const int tt = tg * cm + rank;
+    const int tt = 2 * (tg * cm + rank) + wg;
     const int b = tt / tiles_per_b, t0 = (tt - b * tiles_per_b) * kTM;
-    if (tt >= ntt) {   // past the last tile (partial last group): only keep the stages moving for the peers
+    if (tt >= ntt) {   // past the last tile (partial last pair or group): only keep the stages moving
       for (int kc = 0; kc < kchunks; kc++) {
-        ptx::mbar_wait(&full[st], ph);
+        ptx::mbar_wait<ptx::kStoreFault>(&full[st], ph);
         release(st);
         if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
       }
       continue;
+    }
+    if (p.neop) {
+      // this tile's epilogue operand -> the warpgroup's buffer, once every warp is done reading the previous tile's
+      ptx::named_bar(1 + wg, kWG);
+      if (wq == 0 && lane == 0) {
+        const int c0 = p.gate_mode ? p.gate_c0 : ncol0;
+        ptx::mbar_arrive_expect_tx(&eop_full[wg], p.neop * kEopBox);
+        for (int k = 0; k < p.neop; k++) ptx::tma_load_3d(eop + k * kEopBox, &p.maps[10], &eop_full[wg], c0 + 32 * k, t0, b);
+      }
     }
     float d[N / 2];
 #pragma unroll
@@ -206,9 +232,9 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
     uint32_t prev = 0xFFFFFFFFu;
     if constexpr (!kBf16) {
       for (int kc = 0; kc < kchunks; kc++) {
-        ptx::mbar_wait(&full[st], ph);
+        ptx::mbar_wait<ptx::kStoreFault>(&full[st], ph);
         ptx::wg_fence();
-        const uint32_t a_addr = ring_u32 + st * stage_bytes, b_addr = a_addr + kASub;
+        const uint32_t a_addr = ring_u32 + st * stage_bytes + wg * kASub, b_addr = ring_u32 + st * stage_bytes + 2 * kASub;
 #pragma unroll
         for (int k = 0; k < 4; k++)
           ptx::wgmma_ss<N>(d, ptx::gmma_desc_k_sw128(a_addr + 32 * k), ptx::gmma_desc_k_sw128(b_addr + 32 * k), 1);
@@ -219,13 +245,13 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
         if (++st == (uint32_t)p.nstages) { st = 0; ph ^= 1; }
       }
     } else {
-      // A fragments (rows 16 warp + lane/4 (+ 8), k pairs 2 (lane % 4) (+ 8)) converted from the fp32 box into one of two
+      // A fragments (rows 16 wq + lane/4 (+ 8), k pairs 2 (lane % 4) (+ 8)) converted from the fp32 box into one of two
       // register sets: wgmma reads them asynchronously, so a set is refilled only after the chunk that used it is done
-      const int fr = 16 * warp + (lane >> 2), fk = 2 * (lane & 3);
+      const int fr = 16 * wq + rq, fk = cq;
       uint32_t a0[2][4], a1[2][4];
       auto chunk = [&](uint32_t (&a)[2][4]) {
-        ptx::mbar_wait(&full[st], ph);
-        const unsigned char* as = ring + (size_t)st * stage_bytes;
+        ptx::mbar_wait<ptx::kStoreFault>(&full[st], ph);
+        const unsigned char* as = ring + (size_t)st * stage_bytes + wg * kASub;
 #pragma unroll
         for (int k = 0; k < 2; k++)
 #pragma unroll
@@ -234,7 +260,7 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
             a[k][h] = ptx::cvt_bf16x2(v.x, v.y);
           }
         ptx::wg_fence();
-        const uint32_t b_addr = ring_u32 + st * stage_bytes + kASub;
+        const uint32_t b_addr = ring_u32 + st * stage_bytes + 2 * kASub;
 #pragma unroll
         for (int k = 0; k < 2; k++) ptx::wgmma_rs_bf16<N>(d, a[k], ptx::gmma_desc_k_sw64(b_addr + 32 * k), 1);
         ptx::wg_commit();
@@ -251,196 +277,130 @@ __global__ void __launch_bounds__(kThreadsN, 1) gemm_nt_tc_kernel(const __grid_c
     ptx::wg_wait<0>();
     ptx::wg_touch(d);
     if (prev != 0xFFFFFFFFu) release(prev);
-    // accumulator -> shared memory (column-major), after every thread is done reading the previous tile's copy
-    ptx::named_bar(1, kConsumers);
-    {
-      const int r0 = 16 * warp + (lane >> 2), c0 = 2 * (lane & 3);
-#pragma unroll
-      for (int i = 0; i < N / 2; i++) accs[(8 * (i >> 2) + c0 + (i & 1)) * kAccLd + r0 + 8 * ((i >> 1) & 1)] = d[i];
-    }
-    ptx::named_bar(1, kConsumers);
 
-    const int t = t0 + row;
-    const bool row_ok = t < p.T;
-    const size_t grow = (size_t)b * p.T + (row_ok ? t : 0);
-    if constexpr (EPI == EPI_GATE_BWD_NOZ) {
-      // ---- gate backward without the z output (the stack path): two passes of 16 gate channels; the two dpre boxes
-      //      of this warp (d pre-sigmoid, d pre-tanh) are filled side by side and stored with one bulk group ----
-      const int c0 = hf * 32;
-      if (lane == 0) ptx::bulk_wait_read<0>();
+    // ---- epilogue from registers.  Value v[4 jj + 2 h + e] of a 32-column chunk cb is accumulator d[4 (4 cb + jj) + 2 h
+    //      + e]: row rq + 8 h of this warp's 16, column 32 cb + 8 jj + cq + e ----
+    const int r16 = 16 * wq;
+    bool row_ok[2];
+    size_t grow[2];
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int t = t0 + r16 + rq + 8 * h;
+      row_ok[h] = t < p.T;
+      grow[h] = (size_t)b * p.T + (row_ok[h] ? t : 0);
+    }
+    if (p.neop) {
+      ptx::mbar_wait<ptx::kStoreFault>(&eop_full[wg], eph);
+      eph ^= 1;
+    }
+    // two values of the epilogue operand at row rq + 8 h, column c (even): from the staged boxes, or from memory
+    auto operand = [&](const float* g, int ld, int col0, int c, int h) -> float2 {
+      if (p.neop) return *reinterpret_cast<const float2*>(eop + (c >> 5) * kEopBox + ptx::sw128_off(r16 + rq + 8 * h, c & 31));
+      return row_ok[h] ? __ldg(reinterpret_cast<const float2*>(g + grow[h] * ld + col0 + c)) : make_float2(0.f, 0.f);
+    };
+    // 16 values -> this warp's next staging box -> TMA store (or reduce-add) of [16 rows x 32 columns] at column col
+    auto store16 = [&](const float (&v)[16], const CUtensorMap* map, int col, bool reduce) {
+      unsigned char* sb = stg + (nstore & 1) * kStg;
+      if (lane == 0) ptx::bulk_wait_read<1>();
       __syncwarp();
-      const uint32_t sb0 = ptx::smem_u32(stg + lane * 128), sb1 = sb0 + kStg;
-      const float4* bsv = reinterpret_cast<const float4*>(p.bias + c0);
-      const float4* btv = reinterpret_cast<const float4*>(p.bias2 + c0);
-      const float4* dzr = reinterpret_cast<const float4*>(p.gate_dz + grow * p.gate_ld_dz + p.gate_c0 + c0);
 #pragma unroll
-      for (int h2 = 0; h2 < 2; h2++) {
-        const int cc = c0 + h2 * 16;
-        float a[16], g[16], dzp[16];
-        acc_ld16(accs, cc, row, a);
-        acc_ld16(accs, 64 + cc, row, g);
-        if (p.gate_mode == 3) acc_ld16(accs, 128 + cc, row, dzp);
+      for (int jj = 0; jj < 4; jj++)
 #pragma unroll
-        for (int jj = 0; jj < 4; jj++) {
-          const float4 d4 = row_ok ? __ldg(dzr + h2 * 4 + jj) : make_float4(0.f, 0.f, 0.f, 0.f);
-          const float4 bs = __ldg(bsv + h2 * 4 + jj), bt = __ldg(btv + h2 * 4 + jj);
-          const float dzs[4] = {d4.x, d4.y, d4.z, d4.w};
-          const float bsa[4] = {bs.x, bs.y, bs.z, bs.w}, bta[4] = {bt.x, bt.y, bt.z, bt.w};
-          float da[4], dg[4];
-#pragma unroll
-          for (int k = 0; k < 4; k++) {
-            const int i = 4 * jj + k;
-            float dz = dzs[k];
-            if (p.gate_mode == 3) dz += dzp[i];
-            const float sg = 0.5f * ptx::tanh_approx(0.5f * (a[i] + bsa[k])) + 0.5f;
-            const float th = ptx::tanh_approx(g[i] + bta[k]);
-            da[k] = dz * th * sg * (1.f - sg);      // d pre-sigmoid
-            dg[k] = dz * sg * (1.f - th * th);      // d pre-tanh
-          }
-          const uint32_t off = (uint32_t)(((h2 * 4 + jj) ^ (lane & 7)) << 4);
-          ptx::st_shared_v4(sb0 + off, da[0], da[1], da[2], da[3]);
-          ptx::st_shared_v4(sb1 + off, dg[0], dg[1], dg[2], dg[3]);
-        }
-      }
+        for (int h = 0; h < 2; h++)
+          *reinterpret_cast<float2*>(sb + ptx::sw128_off(rq + 8 * h, 8 * jj + cq)) = make_float2(v[4 * jj + 2 * h], v[4 * jj + 2 * h + 1]);
       ptx::fence_proxy_async();
       __syncwarp();
       if (lane == 0) {
-        ptx::tma_store_3d(&p.maps[9], stg, p.gate_c0 + c0, t0 + q * 32, b);
-        ptx::tma_store_3d(&p.maps[9], stg + kStg, p.gate_R + p.gate_c0 + c0, t0 + q * 32, b);
+        if (reduce) ptx::tma_reduce_add_3d(map, sb, col, t0 + r16, b);
+        else ptx::tma_store_3d(map, sb, col, t0 + r16, b);
         ptx::bulk_commit();
       }
-      continue;
-    }
-    if constexpr (EPI == EPI_GATE) {
-      // ---- gate epilogues: pair sigmoid column c with tanh column GC + c (GC = 64 or 128 gate channels per tile) ----
-      const int GC = p.gate_gc;
-      for (int c0 = hf * 32; c0 < GC; c0 += 64) {
-        float a[32], g[32], dzv[32], dzp[32];
-        acc_ld16(accs, c0, row, *reinterpret_cast<float(*)[16]>(a));
-        acc_ld16(accs, c0 + 16, row, *reinterpret_cast<float(*)[16]>(a + 16));
-        acc_ld16(accs, GC + c0, row, *reinterpret_cast<float(*)[16]>(g));
-        acc_ld16(accs, GC + c0 + 16, row, *reinterpret_cast<float(*)[16]>(g + 16));
-        if (p.gate_mode == 3) {
-          acc_ld16(accs, 2 * GC + c0, row, *reinterpret_cast<float(*)[16]>(dzp));
-          acc_ld16(accs, 2 * GC + c0 + 16, row, *reinterpret_cast<float(*)[16]>(dzp + 16));
-        }
-        if (p.gate_mode == 1) {
-          // forward: z only
+      nstore++;
+    };
+    if constexpr (EPI == EPI_GATE_BWD_NOZ || EPI == EPI_GATE) {
+      // ---- gate epilogues: sigmoid column c pairs with tanh column GC + c (d[i + GC/2]) and, in mode 3, the dz
+      //      partial at 2 GC + c (d[i + GC]); GC = 64, or 128 at N = 256.  Other N never take a gate epilogue. ----
+      if constexpr (N == 128 || N == 192 || N == 256) {
+        constexpr int GC = N == 256 ? 128 : 64;
+        const bool bwd = p.gate_mode >= 2;
 #pragma unroll
-          for (int i = 0; i < 32; i++) {
-            const float sg = 0.5f * ptx::tanh_approx(0.5f * (a[i] + __ldg(p.bias + c0 + i))) + 0.5f;
-            dzv[i] = sg * ptx::tanh_approx(g[i] + __ldg(p.bias2 + c0 + i));
+        for (int cb = 0; cb < GC / 32; cb++) {
+          float a[16], g[16], z[16];
+#pragma unroll
+          for (int jj = 0; jj < 4; jj++)
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+              const int c = 32 * cb + 8 * jj + cq, v = 4 * jj + 2 * h, i = 4 * (4 * cb + jj) + 2 * h;
+              float2 dz2 = make_float2(0.f, 0.f);
+              if (bwd) dz2 = operand(p.gate_dz, p.gate_ld_dz, p.gate_c0, c, h);
+              const float dzs[2] = {dz2.x, dz2.y};
+              const float bsa[2] = {__ldg(p.bias + c), __ldg(p.bias + c + 1)};
+              const float bta[2] = {__ldg(p.bias2 + c), __ldg(p.bias2 + c + 1)};
+#pragma unroll
+              for (int e = 0; e < 2; e++) {
+                const float sg = 0.5f * ptx::tanh_approx(0.5f * (d[i + e] + bsa[e])) + 0.5f;
+                const float th = ptx::tanh_approx(d[i + e + GC / 2] + bta[e]);
+                if (!bwd) { z[v + e] = sg * th; continue; }   // forward: z only
+                float dz = dzs[e];
+                if constexpr (N == 192)
+                  if (p.gate_mode == 3) dz += d[i + e + GC];
+                a[v + e] = dz * th * sg * (1.f - sg);      // d pre-sigmoid
+                g[v + e] = dz * sg * (1.f - th * th);      // d pre-tanh
+                z[v + e] = sg * th;                        // z
+              }
+            }
+          const int col = p.gate_c0 + 32 * cb;
+          if (EPI == EPI_GATE && !(bwd && p.gate_skip_z)) store16(z, &p.maps[8], col, false);
+          if (bwd) {
+            store16(a, &p.maps[9], col, false);
+            store16(g, &p.maps[9], p.gate_R + col, false);
           }
-          unsigned char* sb = stg + (nstore & 1) * kStg;
-          if (lane == 0) ptx::bulk_wait_read<1>();
-          __syncwarp();
-          float4* dstrow = reinterpret_cast<float4*>(sb + lane * 128);
-#pragma unroll
-          for (int j = 0; j < 8; j++)
-            dstrow[j ^ (lane & 7)] = make_float4(dzv[4 * j], dzv[4 * j + 1], dzv[4 * j + 2], dzv[4 * j + 3]);
-          ptx::fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            ptx::tma_store_3d(&p.maps[8], sb, p.gate_c0 + c0, t0 + q * 32, b);
-            ptx::bulk_commit();
-          }
-          nstore++;
-          continue;
-        }
-        if (row_ok) {
-          const float4* dr = reinterpret_cast<const float4*>(p.gate_dz + grow * p.gate_ld_dz + p.gate_c0 + c0);
-#pragma unroll
-          for (int j = 0; j < 8; j++) {
-            const float4 d4 = __ldg(dr + j);
-            dzv[4 * j] = d4.x; dzv[4 * j + 1] = d4.y; dzv[4 * j + 2] = d4.z; dzv[4 * j + 3] = d4.w;
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; i++) dzv[i] = 0.f;
-        }
-        if (p.gate_mode == 3) {
-#pragma unroll
-          for (int i = 0; i < 32; i++) dzv[i] += dzp[i];
-        }
-#pragma unroll
-        for (int i = 0; i < 32; i++) {
-          const float sg = 0.5f * ptx::tanh_approx(0.5f * (a[i] + __ldg(p.bias + c0 + i))) + 0.5f;
-          const float th = ptx::tanh_approx(g[i] + __ldg(p.bias2 + c0 + i));
-          const float dz = dzv[i];
-          a[i] = dz * th * sg * (1.f - sg);      // d pre-sigmoid
-          g[i] = dz * sg * (1.f - th * th);      // d pre-tanh
-          dzv[i] = sg * th;                      // z
-        }
-#pragma unroll
-        for (int which = 0; which < 3; which++) {
-          if (which == 0 && p.gate_skip_z) continue;
-          const float* src = which == 0 ? dzv : (which == 1 ? a : g);
-          unsigned char* sb = stg + (nstore & 1) * kStg;
-          if (lane == 0) ptx::bulk_wait_read<1>();
-          __syncwarp();
-          float4* dstrow = reinterpret_cast<float4*>(sb + lane * 128);
-#pragma unroll
-          for (int j = 0; j < 8; j++)
-            dstrow[j ^ (lane & 7)] = make_float4(src[4 * j], src[4 * j + 1], src[4 * j + 2], src[4 * j + 3]);
-          ptx::fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            if (which == 0) ptx::tma_store_3d(&p.maps[8], sb, p.gate_c0 + c0, t0 + q * 32, b);
-            else ptx::tma_store_3d(&p.maps[9], sb, (which == 1 ? 0 : p.gate_R) + p.gate_c0 + c0, t0 + q * 32, b);
-            ptx::bulk_commit();
-          }
-          nstore++;
         }
       }
-      continue;
     }
     if constexpr (EPI == EPI_PLAIN) {
-      for (int c0 = hf * 32; c0 < N; c0 += 64) {
-        float v[32];
-        acc_ld16(accs, c0, row, *reinterpret_cast<float(*)[16]>(v));
-        acc_ld16(accs, c0 + 16, row, *reinterpret_cast<float(*)[16]>(v + 16));
+#pragma unroll
+      for (int cb = 0; cb < N / 32; cb++) {
+        const int c0 = 32 * cb;
         const bool second = p.out2_col0 > 0 && c0 >= p.out2_col0;
+        float v[16];
+#pragma unroll
+        for (int i = 0; i < 16; i++) v[i] = d[16 * cb + i];
         if (p.bias && !second) {
 #pragma unroll
-          for (int i = 0; i < 32; i++) v[i] += __ldg(p.bias + ncol0 + c0 + i);
-        }
-        if (p.add && row_ok && !second) {
-          const float4* ar = reinterpret_cast<const float4*>(p.add + grow * p.ldadd + ncol0 + c0);
+          for (int jj = 0; jj < 4; jj++) {
+            const float b0 = __ldg(p.bias + ncol0 + c0 + 8 * jj + cq), b1 = __ldg(p.bias + ncol0 + c0 + 8 * jj + cq + 1);
 #pragma unroll
-          for (int j = 0; j < 8; j++) {
-            const float4 a = __ldg(ar + j);
-            v[4 * j] += a.x; v[4 * j + 1] += a.y; v[4 * j + 2] += a.z; v[4 * j + 3] += a.w;
+            for (int h = 0; h < 2; h++) { v[4 * jj + 2 * h] += b0; v[4 * jj + 2 * h + 1] += b1; }
           }
+        }
+        if (p.add && !second) {
+#pragma unroll
+          for (int jj = 0; jj < 4; jj++)
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+              if (p.neop || row_ok[h]) {
+                const float2 a = operand(p.add, p.ldadd, ncol0, c0 + 8 * jj + cq, h);
+                v[4 * jj + 2 * h] += a.x; v[4 * jj + 2 * h + 1] += a.y;
+              }
         }
         if (p.relu_out && !second) {
 #pragma unroll
-          for (int i = 0; i < 32; i++) v[i] = fmaxf(v[i], 0.f);
+          for (int i = 0; i < 16; i++) v[i] = fmaxf(v[i], 0.f);
         }
-        if (p.mask && row_ok && !second) {
-          const float4* mr = reinterpret_cast<const float4*>(p.mask + grow * p.ldmask + ncol0 + c0);
+        if (p.mask && !second) {
 #pragma unroll
-          for (int j = 0; j < 8; j++) {
-            const float4 m = __ldg(mr + j);
-            v[4 * j] = m.x > 0.f ? v[4 * j] : 0.f; v[4 * j + 1] = m.y > 0.f ? v[4 * j + 1] : 0.f;
-            v[4 * j + 2] = m.z > 0.f ? v[4 * j + 2] : 0.f; v[4 * j + 3] = m.w > 0.f ? v[4 * j + 3] : 0.f;
-          }
-        }
-        unsigned char* sb = stg + (nstore & 1) * kStg;
-        if (lane == 0) ptx::bulk_wait_read<1>();
-        __syncwarp();
-        float4* dstrow = reinterpret_cast<float4*>(sb + lane * 128);
+          for (int jj = 0; jj < 4; jj++)
 #pragma unroll
-        for (int j = 0; j < 8; j++)
-          dstrow[j ^ (lane & 7)] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-        ptx::fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          if (second) ptx::tma_reduce_add_3d(&p.maps[9], sb, c0 - p.out2_col0, t0 + q * 32, b);
-          else if (p.accumulate) ptx::tma_reduce_add_3d(&p.maps[8], sb, ncol0 + c0, t0 + q * 32, b);
-          else ptx::tma_store_3d(&p.maps[8], sb, ncol0 + c0, t0 + q * 32, b);
-          ptx::bulk_commit();
+            for (int h = 0; h < 2; h++)
+              if (row_ok[h]) {
+                const float2 m = __ldg(reinterpret_cast<const float2*>(p.mask + grow[h] * p.ldmask + ncol0 + c0 + 8 * jj + cq));
+                v[4 * jj + 2 * h] = m.x > 0.f ? v[4 * jj + 2 * h] : 0.f;
+                v[4 * jj + 2 * h + 1] = m.y > 0.f ? v[4 * jj + 2 * h + 1] : 0.f;
+              }
         }
-        nstore++;
+        if (second) store16(v, &p.maps[9], c0 - p.out2_col0, true);
+        else store16(v, &p.maps[8], ncol0 + c0, p.accumulate != 0);
       }
     }
   }
@@ -523,12 +483,13 @@ static int max_active_clusters(K kernel, size_t smem, int cm) {
   return fit[key] = n;
 }
 
-// ngroups: cluster work items (p.cm time tiles x one column block); ctas: CTAs per SM the shared memory allows
+// ngroups: cluster work items (p.cm tile pairs x one column block).  One CTA per SM: its three warpgroups take the whole
+// register file (setmaxnreg 40 / 232 / 232) and most of the shared memory.
 template <int N, int EPI, typename W>
-static cudaError_t launch_n(int ngroups, int ctas, size_t smem, cudaStream_t st, const Params& p) {
+static cudaError_t launch_n(int ngroups, size_t smem, cudaStream_t st, const Params& p) {
   cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(gemm_nt_tc_kernel<N, EPI, W>), smem);
   if (e != cudaSuccess) return e;
-  int slots = device_sms() * ctas;
+  int slots = device_sms();
   if (p.cm > 1) {
     slots = max_active_clusters(gemm_nt_tc_kernel<N, EPI, W>, smem, p.cm);
     if (slots < 1) return cudaErrorInvalidConfiguration;
@@ -538,24 +499,26 @@ static cudaError_t launch_n(int ngroups, int ctas, size_t smem, cudaStream_t st,
 }
 
 template <int EPI, typename W>
-static cudaError_t launch_epi(int N, int ngroups, int ctas, size_t smem, cudaStream_t st, const Params& p) {
+static cudaError_t launch_epi(int N, int ngroups, size_t smem, cudaStream_t st, const Params& p) {
   switch (N) {
-    case 32: return launch_n<32, EPI, W>(ngroups, ctas, smem, st, p);
-    case 64: return launch_n<64, EPI, W>(ngroups, ctas, smem, st, p);
-    case 96: return launch_n<96, EPI, W>(ngroups, ctas, smem, st, p);
-    case 128: return launch_n<128, EPI, W>(ngroups, ctas, smem, st, p);
-    case 160: return launch_n<160, EPI, W>(ngroups, ctas, smem, st, p);
-    case 192: return launch_n<192, EPI, W>(ngroups, ctas, smem, st, p);
-    case 224: return launch_n<224, EPI, W>(ngroups, ctas, smem, st, p);
-    default: return launch_n<256, EPI, W>(ngroups, ctas, smem, st, p);
+    case 32: return launch_n<32, EPI, W>(ngroups, smem, st, p);
+    case 64: return launch_n<64, EPI, W>(ngroups, smem, st, p);
+    case 96: return launch_n<96, EPI, W>(ngroups, smem, st, p);
+    case 128: return launch_n<128, EPI, W>(ngroups, smem, st, p);
+    case 160: return launch_n<160, EPI, W>(ngroups, smem, st, p);
+    case 192: return launch_n<192, EPI, W>(ngroups, smem, st, p);
+    case 224: return launch_n<224, EPI, W>(ngroups, smem, st, p);
+    default: return launch_n<256, EPI, W>(ngroups, smem, st, p);
   }
 }
 
 // CTAs per cluster for a launch whose weight boxes have box_rows rows (each half box, for the gate's two).
 // The default is 1 for every launch.  Measured on an H100 80GB HBM3 (power limit not reported), bench.py's step
 // (8 x 23 040, ms per step for the kind, CM = 1 / 2 / 4): skip GEMM 1.94 / 2.19 / 2.40, dZ_all 1.84 / 1.78 / 2.10, gate backward 4.62 / 4.77 /
-// 5.24, dx 3.97 / 4.28 / 4.68; whole step 24.9 / 25.5 / 27.2 ms.  Halving the weight bytes pulled from L2 does not pay
-// for the cluster-wide coupling of the ring while a tile's epilogue still runs after its mainloop in the same warpgroup.
+// 5.24, dx 3.97 / 4.28 / 4.68; whole step 24.9 / 25.5 / 27.2 ms (one consumer warpgroup per CTA).  With two consumer
+// warpgroups sharing each weight box, once on the same kind of card (CM = 1 / 2): skip GEMM 1.01 / 1.04, dZ_all 1.21 /
+// 1.24, gate backward 3.53 / 3.64, dx 2.74 / 2.78; step 20.53 / 20.76 ms.  Halving the weight bytes pulled from L2 again
+// does not pay for the cluster-wide coupling of the ring.
 // WNB_NT_CLUSTER=1, 2 or 4 in the environment forces CM (tests, A/B timing); it is read on every call.  Either way CM is
 // halved until each CTA's slice of a box is a whole number of 8-row swizzle atoms (1024 B tf32, 512 B bf16), the
 // alignment at which a slice lands in the same swizzled layout as the whole box.
@@ -611,11 +574,11 @@ int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, con
     p.seg[s] = Seg{s, segs[s].shift, segs[s].K, 4 + s, segs[s].k0, segs[s].n0, -1};
   }
   for (int s = nseg; s < 4; s++) { p.maps[s] = p.maps[0]; p.maps[4 + s] = p.maps[4]; }
-  if (!map3(&p.maps[8], out, ld_out, T, B, 32)) { set_error("gemm_nt_tc: output map failed"); return WNB_ERR_CUDA; }
+  if (!map3(&p.maps[8], out, ld_out, T, B, kStgRows)) { set_error("gemm_nt_tc: output map failed"); return WNB_ERR_CUDA; }
   p.maps[9] = p.maps[8];
   if (gate_dz) {   // R = 64 shorthand used by the fused-shape backward: whole gate in one launch
     const bool fused_dz = opts && opts->gate_fused_dz;
-    if (N != (fused_dz ? 192 : 128) || !gate_dpre || !bias || !map3(&p.maps[9], gate_dpre, 128, T, B, 32)) {
+    if (N != (fused_dz ? 192 : 128) || !gate_dpre || !bias || !map3(&p.maps[9], gate_dpre, 128, T, B, kStgRows)) {
       set_error("gemm_nt_tc: bad gate-backward configuration");
       return WNB_ERR_INVALID;
     }
@@ -630,7 +593,7 @@ int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, con
       set_error("gemm_nt_tc: bad gate configuration");
       return WNB_ERR_INVALID;
     }
-    if (gate->mode == 2 && !map3(&p.maps[9], gate->dpre, 2 * gate->R, T, B, 32)) {
+    if (gate->mode == 2 && !map3(&p.maps[9], gate->dpre, 2 * gate->R, T, B, kStgRows)) {
       set_error("gemm_nt_tc: dpre map failed");
       return WNB_ERR_CUDA;
     }
@@ -639,7 +602,7 @@ int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, con
     p.gate_mode = gate->mode; p.gate_c0 = gate->c0; p.gate_R = gate->R; p.gate_gc = GC;
   }
   if (out2) {
-    if (gate_dz || out2_col0 <= 0 || out2_col0 % 32 != 0 || out2_col0 >= N || !map3(&p.maps[9], out2, ld_out2, T, B, 32)) {
+    if (gate_dz || out2_col0 <= 0 || out2_col0 % 32 != 0 || out2_col0 >= N || !map3(&p.maps[9], out2, ld_out2, T, B, kStgRows)) {
       set_error("gemm_nt_tc: bad split-output configuration");
       return WNB_ERR_INVALID;
     }
@@ -661,26 +624,38 @@ int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, con
     set_error("gemm_nt_tc: the gate backward without z needs 64 gate channels and a 16-byte aligned dz");
     return WNB_ERR_INVALID;
   }
-  // shared memory: ring stages (A box + weight box) | accumulator copy | 4 warps x 2 staging boxes | barriers.  When three
-  // stages fit in half of the SM, two CTAs share it and one's epilogue overlaps the other's mainloop.
-  const int stage_bytes = kASub + N * (bf16 ? w_row_bytes<__nv_bfloat16>() : w_row_bytes<float>());
-  const int fixed = acc_bytes(N) + 4 * 2 * kStg + 1024 + 256;
-  const int sm_bytes = 227 * 1024, half = 113 * 1024;
-  const int ctas = fixed + 3 * stage_bytes <= half ? 2 : 1;
-  int nst = ((ctas == 2 ? half : sm_bytes) - fixed) / stage_bytes;
+  // the epilogue operand that TMA stages per tile: the gate backward's dz (64 gate channels), or the plain epilogue's
+  // residual add when it is at most 64 columns wide (wider ones, e.g. the post network's, are read with __ldg).  TMA needs a
+  // 16-byte aligned base and row pitch.
+  auto tma_ok = [](const void* ptr, int ld) { return !(reinterpret_cast<uintptr_t>(ptr) & 15) && ld % 4 == 0; };
+  const int add_cols = out2 ? out2_col0 : N;
+  if (p.gate_mode >= 2 && p.gate_gc == 64 && tma_ok(p.gate_dz, p.gate_ld_dz)) {
+    if (!map3(&p.maps[10], p.gate_dz, p.gate_ld_dz, T, B, kTM)) { set_error("gemm_nt_tc: dz map failed"); return WNB_ERR_CUDA; }
+    p.neop = 2;
+  } else if (!p.gate_mode && add && add_cols <= 32 * kMaxEop && tma_ok(add, ldadd)) {
+    if (!map3(&p.maps[10], add, ldadd, T, B, kTM)) { set_error("gemm_nt_tc: add map failed"); return WNB_ERR_CUDA; }
+    p.neop = add_cols / 32;
+  } else {
+    p.maps[10] = p.maps[8];
+  }
+  // shared memory: ring stages (two A boxes + weight box) | 8 warps x 2 staging boxes | 2 warpgroups x epilogue operand
+  // boxes | barriers
+  const int stage_bytes = 2 * kASub + N * (bf16 ? w_row_bytes<__nv_bfloat16>() : w_row_bytes<float>());
+  const int fixed = kStgBytes + 2 * p.neop * kEopBox + 1024 + 256;
+  int nst = (227 * 1024 - fixed) / stage_bytes;
   if (nst > 6) nst = 6;
   if (nst < 2) { set_error("gemm_nt_tc: N too large"); return WNB_ERR_INVALID; }
   p.nstages = nst;
   const size_t smem = (size_t)fixed + (size_t)nst * stage_bytes;
-  const int ngroups = cdiv(B * cdiv(T, kTM), p.cm) * p.nblk;
+  const int ngroups = cdiv(cdiv(B * cdiv(T, kTM), 2), p.cm) * p.nblk;
   cudaError_t le;
   if (bf16) {   // (the gate backward without z belongs to the tf32 stack only)
-    if (epi == EPI_PLAIN) le = launch_epi<EPI_PLAIN, __nv_bfloat16>(N, ngroups, ctas, smem, st, p);
-    else if (epi == EPI_GATE) le = launch_epi<EPI_GATE, __nv_bfloat16>(N, ngroups, ctas, smem, st, p);
+    if (epi == EPI_PLAIN) le = launch_epi<EPI_PLAIN, __nv_bfloat16>(N, ngroups, smem, st, p);
+    else if (epi == EPI_GATE) le = launch_epi<EPI_GATE, __nv_bfloat16>(N, ngroups, smem, st, p);
     else { set_error("gemm_nt_tc: no bf16 variant of the gate backward without z"); return WNB_ERR_INVALID; }
-  } else if (epi == EPI_PLAIN) le = launch_epi<EPI_PLAIN, float>(N, ngroups, ctas, smem, st, p);
-  else if (epi == EPI_GATE) le = launch_epi<EPI_GATE, float>(N, ngroups, ctas, smem, st, p);
-  else le = launch_epi<EPI_GATE_BWD_NOZ, float>(N, ngroups, ctas, smem, st, p);
+  } else if (epi == EPI_PLAIN) le = launch_epi<EPI_PLAIN, float>(N, ngroups, smem, st, p);
+  else if (epi == EPI_GATE) le = launch_epi<EPI_GATE, float>(N, ngroups, smem, st, p);
+  else le = launch_epi<EPI_GATE_BWD_NOZ, float>(N, ngroups, smem, st, p);
   if (le != cudaSuccess) { set_error("gemm_nt_tc: launch failed: %s", cudaGetErrorString(le)); return WNB_ERR_CUDA; }
   WNB_CHECK_LAUNCH("gemm_nt_tc");
   return WNB_OK;

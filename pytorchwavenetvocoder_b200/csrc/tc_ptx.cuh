@@ -92,6 +92,11 @@ struct SpinGuard {
     return now - t0 > 20000000000ull;
   }
 };
+// A kernel that sets per-warpgroup register budgets (setmaxnreg) ends a timed-out wait with kStoreFault: a store to
+// address 0, which the host sees as an illegal-address error.  A trap instruction anywhere in such a kernel makes ptxas
+// allocate every warpgroup at the launch bound instead of its setmaxnreg budget.
+enum WaitTimeout { kTrap = 0, kStoreFault = 1 };
+template <int kOnTimeout = kTrap>
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   SpinGuard guard;
@@ -100,7 +105,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 #ifdef WNB_WAIT_PRINTF
       printf("wnb200: mbarrier wait timed out after 20 s (block %d thread %d)\n", blockIdx.x, threadIdx.x);
 #endif
-      __trap();
+      if (kOnTimeout == kStoreFault) *reinterpret_cast<volatile int*>(0) = 0;
+      else __trap();
     }
   }
 }
@@ -197,6 +203,12 @@ __device__ __forceinline__ void wg_touch(float (&d)[R]) {
 #pragma unroll
   for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
+// per-thread register budget of the executing warpgroup (every thread of it executes the same call): a producer
+// warpgroup hands registers back so that the consumer warpgroups can take more than the launch bound gives
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 // barrier over `threads` threads (a multiple of 32) of the CTA; id 0 is __syncthreads
 __device__ __forceinline__ void named_bar(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");

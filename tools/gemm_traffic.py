@@ -5,10 +5,10 @@ the weight and activation bytes the SMs pull from L2, the algorithmic HBM bytes 
     python tools/gemm_traffic.py [--cm 1|2|4] [--batch B] [--length T] [--time [--steps N]]
 
 Shapes are bench.py's model (configs[1]: 30 blocks, R = 64, S = 512, Q = 256, A = 28 padded to 32) at --batch windows
-of --length samples (default: bench.py's batch, 8 x 23 040).  A gemm_nt_tc tile is 64 time rows of one column block and
-loads that block's whole [N x K] weight operand; CTAs in a cluster of CM share each weight box (multicast), so the
-weight column is divided by CM.  Rows a tensor map zero-fills (the dx launch's shifted segment reads a 64-row matrix
-through a 96-row box) are not counted.
+of --length samples (default: bench.py's batch, 8 x 23 040).  A gemm_nt_tc work item is a pair of 64-row time tiles
+(flattened over the batch) of one column block, and loads that block's whole [N x K] weight operand once for both
+tiles; CTAs in a cluster of CM share each weight box (multicast), so the weight column is divided by CM.  Rows a tensor
+map zero-fills (the dx launch's shifted segment reads a 64-row matrix through a 96-row box) are not counted.
 
 --time (needs the GPU) runs --steps training steps with CM forced to --cm (WNB_NT_CLUSTER) and wnb_profile_enable(1),
 as bench.py's roofline block does, and adds each stack kind's ms per step and the achieved L2->SM rate (weight +
@@ -24,7 +24,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench  # noqa: E402
 
-TM = 64   # time rows per gemm_nt_tc tile
+TM = 64   # time rows per gemm_nt_tc tile; a work item is two tiles
 
 
 def kinds(B, T, cm):
@@ -32,12 +32,13 @@ def kinds(B, T, cm):
     Q, A, R, S, depth, repeat, ks, _ = bench.CFG
     Ap, L = (A + 31) // 32 * 32, depth * repeat
     K1, bt, ntt, s = ks * R + Ap, B * T, B * -(-T // TM), 4
+    npairs = -(-ntt // 2)
     rows = []
 
     def gemm(name, n, segs, hbm):
-        """segs: [(K, weight rows read from memory per tile)]; n: N of all column blocks together"""
+        """segs: [(K, weight rows read from memory per tile pair)]; n: N of all column blocks together"""
         nblk = max(1, n // 256) if n > 256 else 1
-        w = sum(ntt * rows_ * k * s for k, rows_ in segs) / cm
+        w = sum(npairs * rows_ * k * s for k, rows_ in segs) / cm
         a = sum(ntt * nblk * TM * k * s for k, _ in segs)
         f = 2 * bt * n * sum(k for k, _ in segs)
         return [name, w, a, hbm, f]
