@@ -327,6 +327,23 @@ WNB_API int wnb_decode_warp_cluster(int B);
  * BIG (1: three 64 KB ring slots, 0: up to six 32 KB slots).  WNB_ERR_UNSUPPORTED when no ring fits. */
 WNB_API int wnb_decode_warp_form(int B, int L, int32_t* form);
 
+/* ---- a14-a16, opt-in bf16 tensor-core variant for the recipe sizes (WaveNet.decode_math = "bf16"): same contract as
+ * wnb_decode_stream (xs, pre-upsampling h with up_w / up_b, n_pad, ragged n_samples, supplied uniforms or in-kernel
+ * Philox with counter (step, batch index, 0, 0), optional logits_out, xs[b][P + n_b ..] untouched), but every product
+ * multiplies bf16 operands (fp32 accumulation) and the batch runs as ceil(B / 64) clusters of 8 CTAs (csrc/decode_bf16.cu).
+ * `weights` is the packed bf16 stream of wnb_decode_bf16_weights() 16-bit elements (layout in csrc/decode_bf16.cu,
+ * built by nets/wavenet.py::_decode_bf16_pack; the biases ride inside it); `queues` holds
+ * wnb_decode_bf16_workspace() bytes and is cleared by the call.  Covered (wnb_decode_bf16_supported): Q 256, ks 2 or 3,
+ * Ap <= 256, R/S 256/256, 512/256 or 512/512, L <= 64; otherwise WNB_ERR_UNSUPPORTED (no fallback). */
+WNB_API int wnb_decode_bf16_supported(int Q, int Ap, int R, int S, int ks, int L);
+WNB_API size_t wnb_decode_bf16_weights(int Q, int Ap, int R, int S, int ks, int L);
+WNB_API size_t wnb_decode_bf16_workspace(int B, int R, int ks, const int32_t* host_dilations, int L);
+WNB_API int wnb_decode_bf16(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
+                            const float* bf, const void* weights, const int32_t* host_dilations, int L, void* queues,
+                            const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P,
+                            int max_n, int n_pad, int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
+                            uint64_t seed, void* stream_handle);
+
 #ifdef __cplusplus
 }
 #endif

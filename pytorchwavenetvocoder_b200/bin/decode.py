@@ -118,6 +118,8 @@ def get_parser():
     parser.add_argument("--intervals", default=1000, type=int, help="log interval")
     parser.add_argument("--seed", default=1, type=int, help="seed number")
     parser.add_argument("--verbose", default=1, type=int, help="log level")
+    parser.add_argument("--decode_math", default="fp32", choices=["fp32", "bf16"],
+                        help="decode precision: fp32 (default) or the bf16 tensor-core decoder of the 512/256-size models")
     return parser
 
 
@@ -143,6 +145,7 @@ def gpu_decode(feat_list, gpu, args, config):
                 args.checkpoint, map_location=lambda storage, loc: storage, weights_only=False)["model"])
             model.eval()
             model.cuda()
+            model.decode_math = getattr(args, "decode_math", "fp32")
             scaler = StandardScaler()
             scaler.mean_ = read_hdf5(args.stats, "/" + config.feature_type + "/mean")
             scaler.scale_ = read_hdf5(args.stats, "/" + config.feature_type + "/scale")

@@ -49,6 +49,26 @@ def bf16_supported(cfg):
     return ok and lib.wnb_resblock_fwd_supported(R, S, _round_up(A, 32), ks, MATH_BF16) == 2
 
 
+def decode_bf16_supported(cfg):
+    """True when the opt-in bf16 tensor-core decoder (decode_math="bf16", csrc/decode_bf16.cu) covers WaveNet(*cfg)."""
+    lib = _lib.load()
+    Q, A, R, S, depth, repeat, ks, U = cfg
+    return bool(lib.wnb_decode_bf16_supported(Q, _round_up(A, 32), R, S, ks, depth * repeat))
+
+
+def _bf16_swizzle(t):
+    """(..., N, K) -> (..., K/64, N, 64): K split into 64-wide tiles, each tile in the 128B swizzle of the wgmma B operand
+    (element (n, k) at column ((k // 8) ^ (n % 8)) * 8 + k % 8 of row n)."""
+    *lead, N, K = t.shape
+    t = t.reshape(*lead, N, K // 64, 64).transpose(-3, -2)
+    k = torch.arange(64, device=t.device)
+    n = torch.arange(N, device=t.device)[:, None]
+    dst = (((k >> 3) ^ (n & 7)) << 3) + (k & 7)
+    out = torch.empty_like(t)
+    out.scatter_(-1, dst.expand_as(t), t)
+    return out
+
+
 def _device():
     if not torch.cuda.is_available():
         raise _lib.WnbError("no CUDA device: the wnb200 kernels need a CUDA GPU (there is no CPU fallback)")
@@ -594,6 +614,9 @@ class WaveNet(nn.Module):
         # and optimizer state stay fp32 in every mode. Decode (fast_generate / batch_fast_generate) is always fp32,
         # whatever math_mode says, so that argmax decoding keeps its parity with the reference.
         self.math_mode = "fp32"
+        # decode precision, separate from math_mode: "fp32" (default; argmax parity with the reference) or "bf16", the
+        # opt-in tensor-core decoder of the recipe sizes (decode_bf16_supported(); any other shape raises, no fallback)
+        self.decode_math = "fp32"
 
         # for preprocessing
         self.onehot = OneHot(self.n_quantize)
@@ -832,8 +855,44 @@ class WaveNet(nn.Module):
                           p2[:, r * Q // CL:(r + 1) * Q // CL].reshape(-1)]
             return torch.cat(parts).contiguous()
 
+    def _decode_bf16_pack(self):
+        """Per-CTA bf16 streams of the bf16 decoder, back to back, as one int16 tensor on the module's device (layout:
+        csrc/decode_bf16.cu, wnb_decode_bf16_weights).  Weights are rounded to nearest even; biases stay fp32 (two 16-bit
+        elements each)."""
+        with torch.no_grad():
+            wf, bf, W1, b1, W2, b2, Wp1, bp1, Wp2, bp2 = [t.detach().float() for t in self._pack()]
+            L = W1.size(0)
+            R, S, Q, ks, Ap = self.n_resch, self.n_skipch, self.n_quantize, self.kernel_size, self.n_aux_pad
+            Ak = _round_up(Ap, 64)
+            CR, CS, QC = R // 8, S // 8, Q // 8
+
+            def bf(t):
+                return t.to(torch.bfloat16).view(torch.int16)
+
+            def f32(t):
+                return t.contiguous().view(torch.int16)
+
+            # W1 columns [taps j = 0..ks-2 | x(t) | aux Ap] -> [aux Ak | taps | x(t)]
+            W1k = torch.cat([F.pad(W1[:, :, ks * R:], (0, Ak - Ap)), W1[:, :, :ks * R]], 2)
+            parts = []
+            for r in range(8):
+                rows = torch.cat([torch.arange(r * CR, (r + 1) * CR), R + torch.arange(r * CR, (r + 1) * CR)])
+                rrows = torch.cat([torch.arange(r * CR, (r + 1) * CR), R + torch.arange(r * CS, (r + 1) * CS)])
+                rows, rrows = rows.to(W1.device), rrows.to(W1.device)
+                per_layer = torch.cat([bf(_bf16_swizzle(W1k[:, rows])).reshape(L, -1), f32(b1[:, rows]).reshape(L, -1),
+                                       bf(_bf16_swizzle(W2[:, rrows])).reshape(L, -1), f32(b2[:, rrows]).reshape(L, -1)], 1)
+                parts += [per_layer.reshape(-1),
+                          bf(_bf16_swizzle(Wp1[r * CS:(r + 1) * CS])).reshape(-1), f32(bp1[r * CS:(r + 1) * CS]),
+                          bf(_bf16_swizzle(Wp2[r * QC:(r + 1) * QC])).reshape(-1), f32(bp2[r * QC:(r + 1) * QC])]
+            return torch.cat(parts).contiguous()
+
     def _decode(self, x, h, n_samples_list, mode, uniforms=None, return_logits=False, seed=None, kernel="auto"):
         lib = _lib.load()
+        decode_math = getattr(self, "decode_math", "fp32")
+        if decode_math not in ("fp32", "bf16"):
+            raise ValueError("decode_math should be fp32 or bf16, got %r" % (decode_math,))
+        if kernel == "auto" and decode_math == "bf16":
+            kernel = "bf16"
         if mode not in ("sampling", "argmax"):
             logging.error("mode should be sampling or argmax")
             sys.exit(1)
@@ -856,7 +915,8 @@ class WaveNet(nn.Module):
         w = self._decode_pack()
         dil = (ctypes.c_int32 * len(self.dilations))(*self.dilations)
         L = len(self.dilations)
-        qbytes = lib.wnb_decode_workspace(B, R, ks, dil, L)
+        qbytes = lib.wnb_decode_bf16_workspace(B, R, ks, dil, L) if kernel == "bf16" else \
+            lib.wnb_decode_workspace(B, R, ks, dil, L)
         queues = torch.empty(max(qbytes // 4, 1), dtype=torch.float32, device=dev)
         nsm = torch.tensor(n_list, dtype=torch.int32, device=dev)
         uni = None if uniforms is None else uniforms.to(dev).float().contiguous()
@@ -869,6 +929,19 @@ class WaveNet(nn.Module):
         cseed = ctypes.c_uint64(seed & 0xFFFFFFFFFFFFFFFF)
         rc = -3
         self.last_decode_kernel = None
+        if kernel == "bf16":
+            if not lib.wnb_decode_bf16_supported(Q, Ap, R, S, ks, L):
+                raise _lib.WnbError("decode_math='bf16' does not cover this model (n_quantize %d, n_aux %d, n_resch %d, "
+                                    "n_skipch %d, kernel_size %d, %d layers): see decode_bf16_supported()"
+                                    % (Q, A, R, S, ks, L))
+            wstream = self._decode_bf16_pack()
+            assert wstream.numel() == lib.wnb_decode_bf16_weights(Q, Ap, R, S, ks, L)
+            check(lib.wnb_decode_bf16(ptr(xs), ptr(h), ptr(upw), ptr(upb), ptr(w["wf"]), ptr(w["bf"]), ptr(wstream), dil,
+                                      L, ptr(queues), ptr(nsm), ptr(uni), ptr(lg), B, P, max_n, n_pad, Th, Q, A, Ap, R, S,
+                                      ks, U, cmode, cseed, stream()), "decode_bf16")
+            self.last_decode_kernel = "bf16"
+            gen = xs[:, P:]
+            return (gen, lg) if return_logits else gen
         if kernel in ("auto", "warp") and lib.wnb_decode_warp_supported(Q, Ap, R, S, ks, L):
             Wc, CLc = lib.wnb_decode_warp_plan(B), lib.wnb_decode_warp_cluster(B)
             wstream = self._decode_warp_pack(Wc, CLc)
@@ -908,7 +981,7 @@ class WaveNet(nn.Module):
         """GENERATE WAVEFORM WITH FAST ALGORITHM (reference wavenet.py:309-395).
 
         One persistent kernel launch; ``intervals`` only controls the summary log line.  Decoding is fp32 whatever
-        ``math_mode`` is (argmax parity with the reference)."""
+        ``math_mode`` is (argmax parity with the reference), unless ``decode_math`` is "bf16"."""
         start = time.time()
         gen = self._decode(x[:1], h[:1], [n_samples], mode)
         out = gen[0, :n_samples].cpu().numpy().astype(np.int64)
@@ -932,7 +1005,7 @@ class WaveNet(nn.Module):
 
         Returns the utterances in COMPLETION order (ascending length, ties by batch index) exactly
         like the reference's retirement loop (:487-509).  The caller's list is not mutated.  Decoding is fp32 whatever
-        ``math_mode`` is (argmax parity with the reference)."""
+        ``math_mode`` is (argmax parity with the reference), unless ``decode_math`` is "bf16"."""
         start = time.time()
         n_list = [int(n) for n in n_samples_list]
         gen = self._decode(x, h, n_list, mode).cpu().numpy().astype(np.int64)
