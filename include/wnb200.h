@@ -344,6 +344,54 @@ WNB_API int wnb_decode_bf16(int32_t* xs, const float* h, const float* up_w, cons
                             int max_n, int n_pad, int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
                             uint64_t seed, void* stream_handle);
 
+/* ---- resumable decode: the four decoders above, one time window per call ------------------------------------------
+ * Each _at entry point takes its twin's arguments plus (pos0, xs_base, h_frame0) and runs padded positions
+ * pos0 .. max(pos0, P - 1) + max_n - 1 only, so a session can decode an utterance chunk by chunk as its aux frames arrive;
+ * the twin is the call with pos0 = xs_base = h_frame0 = 0.  A chain of calls, each starting where the previous one
+ * stopped, computes exactly what one call over the whole range computes, bit for bit, whatever the chunk boundaries.
+ *   P, n_pad   keep their absolute meaning (P - 1 teacher-forced warm-up positions, then sample i at position P - 1 + i);
+ *   pos0       0 (the first call of a session: it runs the whole warm-up) or >= P - 1.  A call generates at least one
+ *              sample, so a chain never starts a call inside the warm-up; 0 < pos0 < P - 1 is rejected;
+ *   i0         = max(pos0 - (P - 1), 0), the first sample index of the call;
+ *   n_samples  (B) samples to generate in this call per utterance (sample indices i0 .. i0 + n_b - 1), max_n >= every
+ *              n_b; the call stops after max_n samples;
+ *   xs         (B, max(pos0, P - 1) + max_n + 1 - xs_base) int32: column c is absolute position xs_base + c.  The call
+ *              reads positions pos0 - (ks - 1) .. (those >= 0; so xs_base <= max(pos0 - (ks - 1), 0)), which must hold the
+ *              seed prefix or what earlier calls generated, and writes position pos + 1 for each sample it generates;
+ *   h          (B, A, Th): column c is absolute frame h_frame0 + c (aux column max(p - n_pad, 0), divided by U when
+ *              U > 0); h_frame0 <= the frame of pos0.  Lookups past the last column are clamped to it;
+ *   uniforms   (B, max_n) and logits_out (B, max_n, Q) are indexed by the call's own sample index i - i0; the in-kernel
+ *              Philox counter keeps the absolute i, so a sampled stream does not depend on the chunk boundaries.
+ * Between the calls of one session the caller keeps the queue workspace untouched and the same B (hence the same
+ * launch form: NU / W / CL of wnb_decode_warp, the utterances per CTA of wnb_decode_stream / wnb_decode, the cluster split
+ * of wnb_decode_bf16); the fp32 decoders never need cleared queues, wnb_decode_bf16_at clears them when pos0 == 0 only.
+ * Positions are int: the last position written must stay below 2^31 - 1.  WNB_ERR_INVALID for an inconsistent window. */
+WNB_API int wnb_decode_at(int32_t* xs, const float* h, const float* up_w, const float* up_b,
+                          const float* wf, const float* bf, const float* w1d, const float* b1, const float* w2d,
+                          const float* b2, const float* wp1d, const float* bp1, const float* wp2d, const float* bp2,
+                          const int32_t* host_dilations, int L, void* queues, const int32_t* n_samples,
+                          const float* uniforms, float* logits_out, int B, int P, int max_n, int n_pad, int Th,
+                          int Q, int A, int Ap, int R, int S, int ks, int U, int mode, uint64_t seed,
+                          int pos0, int xs_base, int h_frame0, void* stream);
+WNB_API int wnb_decode_stream_at(int32_t* xs, const float* h, const float* up_w, const float* up_b,
+                                 const float* wf, const float* bf, const float* stream, const float* b1,
+                                 const float* b2, const float* bp1, const float* bp2,
+                                 const int32_t* host_dilations, int L, void* queues, const int32_t* n_samples,
+                                 const float* uniforms, float* logits_out, int B, int P, int max_n, int n_pad,
+                                 int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
+                                 uint64_t seed, int pos0, int xs_base, int h_frame0, void* stream_handle);
+WNB_API int wnb_decode_warp_at(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
+                               const float* bf, const float* stream, const float* b1, const float* b2,
+                               const float* bp1, const float* bp2, const int32_t* host_dilations, int L,
+                               void* queues, const int32_t* n_samples, const float* uniforms, float* logits_out,
+                               int B, int P, int max_n, int n_pad, int Th, int A, int U, int mode, uint64_t seed,
+                               int W, int CL, int pos0, int xs_base, int h_frame0, void* stream_handle);
+WNB_API int wnb_decode_bf16_at(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
+                               const float* bf, const void* weights, const int32_t* host_dilations, int L, void* queues,
+                               const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P,
+                               int max_n, int n_pad, int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
+                               uint64_t seed, int pos0, int xs_base, int h_frame0, void* stream_handle);
+
 #ifdef __cplusplus
 }
 #endif

@@ -34,6 +34,7 @@ from pytorchwavenetvocoder_b200.utils import shape_hdf5
 from pytorchwavenetvocoder_b200.utils import have_soundfile
 from pytorchwavenetvocoder_b200.utils import write_wav
 from pytorchwavenetvocoder_b200.utils import write_wav_pcm16
+from pytorchwavenetvocoder_b200.utils import WavWriter
 
 
 def pad_list(batch_list, pad_value=0.0):
@@ -120,7 +121,38 @@ def get_parser():
     parser.add_argument("--verbose", default=1, type=int, help="log level")
     parser.add_argument("--decode_math", default="fp32", choices=["fp32", "bf16"],
                         help="decode precision: fp32 (default) or the bf16 tensor-core decoder of the 512/256-size models")
+    parser.add_argument("--chunk_frames", default=0, type=int,
+                        help="decode through a resumable session, feeding this many aux frames per call and writing each "
+                             "wav as its samples arrive (0: one launch per batch); the files are the same either way")
     return parser
+
+
+def _decode_chunked(model, x, h, n_samples_list, chunk_frames, paths, fs, n_quantize, pcm16):
+    """Decode one batch through ``WaveNet.decode_session`` in chunks of ``chunk_frames`` aux frames and append every
+    utterance's new samples to its wav as they arrive.  Same samples (hence same files) as the one-shot path."""
+    sess = model.decode_session(x, n_samples_list, "sampling")
+    writers = [WavWriter(p, fs) for p in paths]
+    try:
+        for f0 in range(0, h.size(2), chunk_frames):
+            if sess.done:
+                break
+            out = (sess.step_pcm16 if pcm16 else sess.step)(h[:, :, f0:f0 + chunk_frames])
+            counts = sess.last_counts
+            if max(counts) == 0:
+                continue
+            out = out.cpu().numpy()
+            for b, w in enumerate(writers):
+                if counts[b] == 0:
+                    continue
+                if pcm16:
+                    w.write_pcm16(out[b, :counts[b]])
+                else:
+                    w.write(decode_mu_law(out[b, :counts[b]].astype(np.int64), n_quantize))
+        if not sess.done:   # the one-shot path raises the same way instead of writing short files
+            raise ValueError("aux features too short: %d frames for %d samples" % (h.size(2), max(n_samples_list)))
+    finally:
+        for w in writers:
+            w.close()
 
 
 def gpu_decode(feat_list, gpu, args, config):
@@ -158,9 +190,16 @@ def gpu_decode(feat_list, gpu, args, config):
                 upsampling_factor=config.upsampling_factor,
                 use_upsampling_layer=config.use_upsampling_layer,
                 use_speaker_code=config.use_speaker_code)
+            chunk = getattr(args, "chunk_frames", 0)
             if args.batch_size > 1:
                 for feat_ids, (batch_x, batch_h, n_samples_list) in generator:
                     logging.info("decoding start")
+                    if chunk > 0:
+                        _decode_chunked(model, batch_x, batch_h, n_samples_list, chunk,
+                                        [args.outdir + "/" + f + ".wav" for f in feat_ids], args.fs, config.n_quantize,
+                                        not have_soundfile())
+                        logging.info("wrote %d wavs in %s." % (len(feat_ids), args.outdir))
+                        continue
                     # batch_fast_generate returns completion order = ascending length, ties by batch index
                     order = sorted(range(len(feat_ids)), key=lambda b: (n_samples_list[b], b))
                     if not have_soundfile():
@@ -179,6 +218,11 @@ def gpu_decode(feat_list, gpu, args, config):
             else:
                 for feat_id, (x, h, n_samples) in generator:
                     logging.info("decoding %s (length = %d)" % (feat_id, n_samples))
+                    if chunk > 0:
+                        _decode_chunked(model, x, h, [n_samples], chunk, [args.outdir + "/" + feat_id + ".wav"], args.fs,
+                                        config.n_quantize, False)
+                        logging.info("wrote %s.wav in %s." % (feat_id, args.outdir))
+                        continue
                     samples = model.fast_generate(x, h, n_samples, args.intervals)
                     wav = decode_mu_law(samples, config.n_quantize)
                     write_wav(args.outdir + "/" + feat_id + ".wav", wav, args.fs)

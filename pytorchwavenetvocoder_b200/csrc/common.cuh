@@ -90,6 +90,43 @@ enum { SCRATCH_WGRAD = 0, SCRATCH_EMBED = 1, SCRATCH_AUX = 2, SCRATCH_LOSS = 3, 
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 static inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// The window of one resumable decode call (wnb_decode_at and its twins, include/wnb200.h).  The kernels keep absolute
+// indices: the launcher shifts xs by -xs_base columns, h by -h_frame0 columns, uniforms by -i0 columns and logits_out by
+// -i0 rows, so that a kernel reads position pp at xs[.. + pp], frame f at h[.. + f], and sample i's uniform and logits at
+// i; n_samples become absolute ends (i0 + n_b).  A one-shot call is the window pos0 = xs_base = h_frame0 = 0.
+struct DecodeWindow {
+  int pos0, i0;      // first position; first sample index = max(pos0 - (P - 1), 0)
+  int i_last;        // i0 + max_n - 1: the last sample index the call may generate (the uniforms clamp)
+  int h_last;        // h_frame0 + Th - 1: the last frame of h (lookups past it are clamped to it)
+  int stride_xs;     // xs row stride: columns xs_base .. max(pos0, P - 1) + max_n
+};
+template <class T>
+static inline T* shift_ptr(T* ptr, long long n) {   // ptr + n elements, NULL stays NULL (n may be negative)
+  return ptr ? reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(ptr) + (uintptr_t)(n * (long long)sizeof(T))) : ptr;
+}
+// False (message set) when the window is inconsistent or its positions would not fit an int.
+static inline bool decode_window(const char* name, int P, int n_pad, int U, int ks, int max_n, int Th, int pos0,
+                                 int xs_base, int h_frame0, DecodeWindow* w) {
+  const int first = pos0 - (ks - 1) > 0 ? pos0 - (ks - 1) : 0;            // oldest column the front gather reads
+  const int j0 = pos0 - n_pad > 0 ? pos0 - n_pad : 0;                      // aux column of pos0
+  const int f0 = U > 0 ? j0 / U : j0;                                      // its frame
+  const long long last = (long long)(pos0 > P - 1 ? pos0 : P - 1) + max_n;  // last xs column written
+  // a call generates at least one sample, so a chain of calls never starts one inside the warm-up: pos0 is 0 (the first
+  // call) or past it
+  if (pos0 < 0 || (pos0 > 0 && pos0 < P - 1) || xs_base < 0 || xs_base > first || h_frame0 < 0 || h_frame0 > f0 ||
+      last >= 0x7fffffffLL || (long long)h_frame0 + Th > 0x7fffffffLL) {
+    set_error("%s: bad window (pos0 %d, xs_base %d, h_frame0 %d, P %d, n_pad %d, max_n %d)", name, pos0, xs_base,
+              h_frame0, P, n_pad, max_n);
+    return false;
+  }
+  w->pos0 = pos0;
+  w->i0 = pos0 > P - 1 ? pos0 - (P - 1) : 0;
+  w->i_last = w->i0 + max_n - 1;
+  w->h_last = h_frame0 + Th - 1;
+  w->stride_xs = (int)(last + 1 - xs_base);
+  return true;
+}
+
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 
 __device__ __forceinline__ float warp_sum(float v) {

@@ -27,6 +27,7 @@ struct DecodeParams {
   const float *wf, *bf, *w1d, *b1, *w2d, *b2, *wp1d, *bp1, *wp2d, *bp2;
   float* queues; const int32_t* n_samples; const float* uniforms; float* logits_out;
   int B, P, max_n, n_pad, Th, Q, A, Ap, R, S, ks, U, mode, L;
+  int pos0, i0, i_last, h_last, stride_xs;   // the call's window (common.cuh DecodeWindow)
   int O1, O2, Sp, Qp;  // padded (multiple of 4) output widths of the K-major matrices
   unsigned long long seed;
   int dil[kMaxLayers];
@@ -150,17 +151,17 @@ __global__ void __launch_bounds__(kDecThreads) decode_kernel(const DecodeParams 
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int u0 = blockIdx.x * NU;
-  const int stride_xs = p.P + p.max_n;
+  const int stride_xs = p.stride_xs;
 
-  if (tid < NU) s_n[tid] = (u0 + tid < p.B) ? p.n_samples[u0 + tid] : 0;
+  if (tid < NU) s_n[tid] = (u0 + tid < p.B) ? p.i0 + p.n_samples[u0 + tid] : 0;   // absolute end
   __syncthreads();
   int nmax = 0;
 #pragma unroll
   for (int u = 0; u < NU; u++) nmax = max(nmax, s_n[u]);
-  if (nmax == 0) return;
+  if (nmax <= p.i0) return;
   const int last_pos = p.P - 1 + nmax - 1;
 
-  for (int pos = 0; pos <= last_pos; pos++) {
+  for (int pos = p.pos0; pos <= last_pos; pos++) {
     const bool want = pos >= p.P - 1;  // free-running: need logits
     // ---- stage 0: front gather, aux column, queue-tap prefetch ----
     for (int e = tid; e < NU * R; e += kDecThreads) {
@@ -184,10 +185,10 @@ __global__ void __launch_bounds__(kDecThreads) decode_kernel(const DecodeParams 
       if (a < p.A) {
         const int j = max(pos - p.n_pad, 0);
         if (p.U > 0) {
-          const int tf = min(j / p.U, p.Th - 1), jj = j % p.U;
+          const int tf = min(j / p.U, p.h_last), jj = j % p.U;
           v = fmaf(__ldg(p.h + ((size_t)ug * p.A + a) * p.Th + tf), __ldg(p.up_w + jj), __ldg(p.up_b));
         } else {
-          v = __ldg(p.h + ((size_t)ug * p.A + a) * p.Th + min(j, p.Th - 1));
+          v = __ldg(p.h + ((size_t)ug * p.A + a) * p.Th + min(j, p.h_last));
         }
       }
       hcol[e] = v;
@@ -305,7 +306,7 @@ __global__ void __launch_bounds__(kDecThreads) decode_kernel(const DecodeParams 
           // inverse-CDF draw from softmax(logits)  (wavenet.py:377-379 uses torch Categorical)
           float uni;
           if (p.uniforms) {
-            uni = p.uniforms[(size_t)min(u0 + u, p.B - 1) * p.max_n + min(i, p.max_n - 1)];
+            uni = p.uniforms[(size_t)min(u0 + u, p.B - 1) * p.max_n + min(i, p.i_last)];
           } else {
             uint32_t r[4];
             philox4x32_10((uint32_t)i, (uint32_t)(u0 + u), 0u, 0u, (uint32_t)p.seed, (uint32_t)(p.seed >> 32), r);
@@ -369,6 +370,18 @@ WNB_API int wnb_decode(int32_t* xs, const float* h, const float* up_w, const flo
                void* queues, const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P,
                int max_n, int n_pad, int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
                uint64_t seed, void* stream) {
+  return wnb_decode_at(xs, h, up_w, up_b, wf, bf, w1d, b1, w2d, b2, wp1d, bp1, wp2d, bp2, host_dilations, L, queues,
+                       n_samples, uniforms, logits_out, B, P, max_n, n_pad, Th, Q, A, Ap, R, S, ks, U, mode, seed, 0, 0, 0,
+                       stream);
+}
+
+WNB_API int wnb_decode_at(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
+                          const float* bf, const float* w1d, const float* b1, const float* w2d, const float* b2,
+                          const float* wp1d, const float* bp1, const float* wp2d, const float* bp2,
+                          const int32_t* host_dilations, int L, void* queues, const int32_t* n_samples,
+                          const float* uniforms, float* logits_out, int B, int P, int max_n, int n_pad, int Th, int Q,
+                          int A, int Ap, int R, int S, int ks, int U, int mode, uint64_t seed, int pos0, int xs_base,
+                          int h_frame0, void* stream) {
   WNB_REQUIRE(B > 0 && P >= 1 && max_n >= 1 && Th >= 1 && Q > 0 && A > 0 && Ap >= A && R > 0 && S > 0 && ks >= 1 &&
                   U >= 0 && L >= 1, "decode: bad shape");
   WNB_REQUIRE(L <= kMaxLayers, "decode: more than %d layers", kMaxLayers);
@@ -383,6 +396,11 @@ WNB_API int wnb_decode(int32_t* xs, const float* h, const float* up_w, const flo
   p.n_samples = n_samples; p.uniforms = uniforms; p.logits_out = logits_out;
   p.B = B; p.P = P; p.max_n = max_n; p.n_pad = n_pad; p.Th = Th; p.Q = Q; p.A = A; p.Ap = Ap; p.R = R; p.S = S;
   p.ks = ks; p.U = U; p.mode = mode; p.L = L; p.seed = seed;
+  DecodeWindow win;
+  if (!decode_window("decode", P, n_pad, U, ks, max_n, Th, pos0, xs_base, h_frame0, &win)) return WNB_ERR_INVALID;
+  p.pos0 = win.pos0; p.i0 = win.i0; p.i_last = win.i_last; p.h_last = win.h_last; p.stride_xs = win.stride_xs;
+  p.xs = shift_ptr(xs, -(long long)xs_base); p.h = shift_ptr(h, -(long long)h_frame0);
+  p.uniforms = shift_ptr(uniforms, -(long long)win.i0); p.logits_out = shift_ptr(logits_out, -(long long)win.i0 * Q);
   p.O1 = (2 * R + 3) & ~3; p.O2 = (R + S + 3) & ~3; p.Sp = (S + 3) & ~3; p.Qp = (Q + 3) & ~3;
   long long off = 0;
   for (int l = 0; l < L; l++) {

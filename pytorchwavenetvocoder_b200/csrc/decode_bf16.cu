@@ -57,7 +57,7 @@
 //     fence.proxy.async.global after its queue stores; the consumer warpgroup then meets at a CTA barrier, and one thread
 //     arrives with .release.cluster on the step barrier of every CTA of the cluster.  A producer waits on its step
 //     barrier with .acquire.cluster for step t-1 before the first tap copy of step t.
-// Taps before the start (t - s < 0) read slots nobody has written yet in this launch: zeros.
+// Taps before the start (t - s < 0) read slots nobody has written yet in this session: zeros.
 //
 // Warm-up: the teacher-forced prefix steps (P - 1 of them, P = max(T0, receptive field)) run the gate and res+skip
 // products only (no post network, no pick).  Every wait is bounded by %globaltimer (tc_ptx.cuh) and traps; nothing in
@@ -90,6 +90,7 @@ struct Params {
   unsigned char* queues;
   const int32_t* n_samples; const float* uniforms; float* logits_out;
   int B, P, max_n, n_pad, Th, A, Ak, U, mode, L, ks, nstage, stage_bytes, bc;
+  int pos0, i0, i_last, h_last, stride_xs;   // the call's window (common.cuh DecodeWindow)
   long long cta_bytes;            // bytes of one CTA's stream
   long long q_cluster;            // bytes of one cluster's queues
   unsigned long long seed;
@@ -251,7 +252,7 @@ __global__ void __launch_bounds__(kThreads, 1) decode_bf16_kernel(const Params p
   const int cl = blockIdx.x / kCL;
   const int u0 = cl * p.bc;
   const int nu = min(p.bc, p.B - u0);
-  const int stride_xs = p.P + p.max_n;
+  const int stride_xs = p.stride_xs;
   const int ks = p.ks, L = p.L;
   const int nA = p.Ak / 64, nT = (ks - 1) * KT;       // gate chunks: aux, taps, then KT of x(t)
 
@@ -273,11 +274,11 @@ __global__ void __launch_bounds__(kThreads, 1) decode_bf16_kernel(const Params p
     ptx::mbar_init(&qbar, kCL);
     ptx::fence_barrier_init();
   }
-  if (tid < kM) s_n[tid] = (tid < nu) ? p.n_samples[u0 + tid] : 0;
+  if (tid < kM) s_n[tid] = (tid < nu) ? p.i0 + p.n_samples[u0 + tid] : 0;   // absolute end
   __syncthreads();
   int nmax = 0;
   for (int u = 0; u < nu; u++) nmax = max(nmax, s_n[u]);
-  if (nmax == 0) return;      // (the same in every CTA of the cluster)
+  if (nmax <= p.i0) return;   // (the same in every CTA of the cluster)
   // every CTA's barriers are initialised before the first remote arrival
   ptx::cluster_sync();
   const int last_pos = p.P - 1 + nmax - 1;
@@ -297,13 +298,14 @@ __global__ void __launch_bounds__(kThreads, 1) decode_bf16_kernel(const Params p
         if (tap) bulk_g2s(dst + NG * 128, tap, kTile, &full[st]);
         if (++st == p.nstage) { st = 0; ph ^= 1u; }
       };
-      for (int pos = 0; pos <= last_pos; pos++) {
+      for (int pos = p.pos0; pos <= last_pos; pos++) {
         const bool want = pos >= p.P - 1;
         const unsigned char* w = my_w;
         for (int l = 0; l < L; l++) {
           for (int c = 0; c < nA; c++, w += NG * 128) push(w, NG * 128, nullptr);
-          if (l == 0 && pos > 0) {
-            // every CTA's queue writes of step pos-1 (and before) are visible to the async proxy
+          if (l == 0 && pos > p.pos0) {
+            // every CTA's queue writes of step pos-1 (and before) are visible to the async proxy (those of an earlier
+            // launch are ordered by the launch boundary)
             wait_acquire_cluster(&qbar, qph);
             qph ^= 1u;
             fence_proxy_async_global();
@@ -378,7 +380,7 @@ __global__ void __launch_bounds__(kThreads, 1) decode_bf16_kernel(const Params p
   auto row_of = [&](int i) { return fr + 8 * ((i >> 1) & 1); };
   auto col_of = [&](int i) { return 8 * (i >> 2) + fk + (i & 1); };
 
-  for (int pos = 0; pos <= last_pos; pos++) {
+  for (int pos = p.pos0; pos <= last_pos; pos++) {
     const bool want = pos >= p.P - 1;
     const int istep = pos - (p.P - 1);
     // ---- step prologue: aux rows (bf16) and this CTA's slice of the front embedding (fp32, in registers) ----
@@ -392,10 +394,10 @@ __global__ void __launch_bounds__(kThreads, 1) decode_bf16_kernel(const Params p
         v[t] = 0.f;
         if (a + t < p.A) {
           if (p.U > 0) {
-            const int tf = min(j / p.U, p.Th - 1), jj = j % p.U;
+            const int tf = min(j / p.U, p.h_last), jj = j % p.U;
             v[t] = fmaf(__ldg(p.h + ((size_t)ug * p.A + a + t) * p.Th + tf), __ldg(p.up_w + jj), __ldg(p.up_b));
           } else {
-            v[t] = __ldg(p.h + ((size_t)ug * p.A + a + t) * p.Th + min(j, p.Th - 1));
+            v[t] = __ldg(p.h + ((size_t)ug * p.A + a + t) * p.Th + min(j, p.h_last));
           }
         }
       }
@@ -412,7 +414,8 @@ __global__ void __launch_bounds__(kThreads, 1) decode_bf16_kernel(const Params p
           const int pp = pos - (ks - 1 - k);
           int q = -1;
           if (k < ks && pp >= 0) {
-            q = (pp < p.P) ? p.xs[(size_t)ug * stride_xs + pp] : hist[pp & 3][row];
+            // the seed prefix and what earlier launches generated come from xs, this launch's picks from hist
+            q = (pp < p.P || pp <= p.pos0) ? p.xs[(size_t)ug * stride_xs + pp] : hist[pp & 3][row];
             q %= kQ;
             if (q < 0) q += kQ;
           }
@@ -610,7 +613,7 @@ __global__ void __launch_bounds__(kThreads, 1) decode_bf16_kernel(const Params p
       if (p.mode == WNB_MODE_SAMPLING) {
         float uni;
         if (p.uniforms) {
-          uni = p.uniforms[(size_t)min(u0 + row, p.B - 1) * p.max_n + min(istep, p.max_n - 1)];
+          uni = p.uniforms[(size_t)min(u0 + row, p.B - 1) * p.max_n + min(istep, p.i_last)];
         } else {
           uint32_t rr[4];
           philox4x32_10((uint32_t)istep, (uint32_t)(u0 + row), 0u, 0u, (uint32_t)p.seed, (uint32_t)(p.seed >> 32), rr);
@@ -728,6 +731,15 @@ WNB_API int wnb_decode_bf16(int32_t* xs, const float* h, const float* up_w, cons
                             const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P, int max_n,
                             int n_pad, int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
                             uint64_t seed, void* stream_handle) {
+  return wnb_decode_bf16_at(xs, h, up_w, up_b, wf, bf, weights, host_dilations, L, queues, n_samples, uniforms,
+                            logits_out, B, P, max_n, n_pad, Th, Q, A, Ap, R, S, ks, U, mode, seed, 0, 0, 0, stream_handle);
+}
+
+WNB_API int wnb_decode_bf16_at(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
+                               const float* bf, const void* weights, const int32_t* host_dilations, int L, void* queues,
+                               const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P,
+                               int max_n, int n_pad, int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
+                               uint64_t seed, int pos0, int xs_base, int h_frame0, void* stream_handle) {
   WNB_REQUIRE(B > 0 && P >= 1 && max_n >= 1 && Th >= 1 && Q > 0 && A > 0 && Ap >= A && R > 0 && S > 0 && ks >= 1 &&
                   U >= 0 && L >= 1, "decode_bf16: bad shape");
   WNB_REQUIRE(xs && h && wf && bf && weights && n_samples && queues && host_dilations, "decode_bf16: null pointer");
@@ -744,6 +756,11 @@ WNB_API int wnb_decode_bf16(int32_t* xs, const float* h, const float* up_w, cons
   p.n_samples = n_samples; p.uniforms = uniforms; p.logits_out = logits_out;
   p.B = B; p.P = P; p.max_n = max_n; p.n_pad = n_pad; p.Th = Th; p.A = A; p.Ak = db_aux_k(Ap); p.U = U; p.mode = mode;
   p.L = L; p.ks = ks; p.seed = seed;
+  DecodeWindow win;
+  if (!decode_window("decode_bf16", P, n_pad, U, ks, max_n, Th, pos0, xs_base, h_frame0, &win)) return WNB_ERR_INVALID;
+  p.pos0 = win.pos0; p.i0 = win.i0; p.i_last = win.i_last; p.h_last = win.h_last; p.stride_xs = win.stride_xs;
+  p.xs = shift_ptr(xs, -(long long)xs_base); p.h = shift_ptr(h, -(long long)h_frame0);
+  p.uniforms = shift_ptr(uniforms, -(long long)win.i0); p.logits_out = shift_ptr(logits_out, -(long long)win.i0 * Q);
   p.nstage = db_stages(R, S, Ap);
   p.stage_bytes = db_stage_bytes(R, S);
   const int ncl = cdiv(B, db::kM);
@@ -758,8 +775,9 @@ WNB_API int wnb_decode_bf16(int32_t* xs, const float* h, const float* up_w, cons
   }
   p.q_cluster = slots * (long long)R * db::kM * 2;
   cudaStream_t st = (cudaStream_t)stream_handle;
-  // taps before the start of the sequence read zeros: the queues start cleared
-  WNB_CUDA(cudaMemsetAsync(queues, 0, (size_t)ncl * p.q_cluster, st));
+  // taps before the start of the sequence read zeros: the queues start cleared (by the first call of a session only;
+  // later calls continue from what the previous one left)
+  if (pos0 == 0) WNB_CUDA(cudaMemsetAsync(queues, 0, (size_t)ncl * p.q_cluster, st));
   const size_t smem = db_fixed_smem(R, Ap) + (size_t)p.nstage * p.stage_bytes;
   auto launch = [&](auto kernel) -> cudaError_t {
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -31,6 +31,7 @@ struct StreamParams {
   const float* stream;       // packed weights (see header comment)
   float* queues; const int32_t* n_samples; const float* uniforms; float* logits_out;
   int B, P, max_n, n_pad, Th, Q, A, Ap, R, S, ks, U, mode, L;
+  int pos0, i0, i_last, h_last, stride_xs;   // the call's window (common.cuh DecodeWindow)
   int O1, Or, Os, Sp, Qp;    // padded widths
   int nslot;
   unsigned long long seed;
@@ -175,7 +176,7 @@ __global__ void __launch_bounds__(kStreamThreads, 1) decode_stream_kernel(const 
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int u0 = blockIdx.x * NU;
-  const int stride_xs = p.P + p.max_n;
+  const int stride_xs = p.stride_xs;
 
   if (tid == 0) {
     for (int i = 0; i < p.nslot; i++) {
@@ -184,19 +185,19 @@ __global__ void __launch_bounds__(kStreamThreads, 1) decode_stream_kernel(const 
     }
     ptx::fence_barrier_init();
   }
-  if (tid < NU) s_n[tid] = (u0 + tid < p.B) ? p.n_samples[u0 + tid] : 0;
+  if (tid < NU) s_n[tid] = (u0 + tid < p.B) ? p.i0 + p.n_samples[u0 + tid] : 0;   // absolute end
   __syncthreads();
   int nmax = 0;
 #pragma unroll
   for (int u = 0; u < NU; u++) nmax = max(nmax, s_n[u]);
-  if (nmax == 0) return;
+  if (nmax <= p.i0) return;
   const int last_pos = p.P - 1 + nmax - 1;
   Ring ring{ring_base, full, empty, p.nslot, 0u};
 
   if (warp == kConsThreads / 32) {
     // ================================ producer warp ================================
     if (lane == 0) {
-      for (int pos = 0; pos <= last_pos; pos++) {
+      for (int pos = p.pos0; pos <= last_pos; pos++) {
         const bool want = pos >= p.P - 1;
         for (int l = 0; l < L; l++) {
           const float* base = p.stream + (size_t)l * p.layer_stride;
@@ -214,7 +215,7 @@ __global__ void __launch_bounds__(kStreamThreads, 1) decode_stream_kernel(const 
   }
 
   // ================================ consumer warps ================================
-  for (int pos = 0; pos <= last_pos; pos++) {
+  for (int pos = p.pos0; pos <= last_pos; pos++) {
     const bool want = pos >= p.P - 1;
     for (int e = tid; e < NU * R; e += kConsThreads) {
       const int u = e / R, r = e - u * R;
@@ -237,10 +238,10 @@ __global__ void __launch_bounds__(kStreamThreads, 1) decode_stream_kernel(const 
       if (a < p.A) {
         const int j = max(pos - p.n_pad, 0);
         if (p.U > 0) {
-          const int tf = min(j / p.U, p.Th - 1), jj = j % p.U;
+          const int tf = min(j / p.U, p.h_last), jj = j % p.U;
           v = fmaf(__ldg(p.h + ((size_t)ug * p.A + a) * p.Th + tf), __ldg(p.up_w + jj), __ldg(p.up_b));
         } else {
-          v = __ldg(p.h + ((size_t)ug * p.A + a) * p.Th + min(j, p.Th - 1));
+          v = __ldg(p.h + ((size_t)ug * p.A + a) * p.Th + min(j, p.h_last));
         }
       }
       hcol[e] = v;
@@ -356,7 +357,7 @@ __global__ void __launch_bounds__(kStreamThreads, 1) decode_stream_kernel(const 
         if (p.mode == WNB_MODE_SAMPLING) {
           float uni;
           if (p.uniforms) {
-            uni = p.uniforms[(size_t)min(u0 + u, p.B - 1) * p.max_n + min(i, p.max_n - 1)];
+            uni = p.uniforms[(size_t)min(u0 + u, p.B - 1) * p.max_n + min(i, p.i_last)];
           } else {
             uint32_t rr[4];
             philox4x32_10s((uint32_t)i, (uint32_t)(u0 + u), 0u, 0u, (uint32_t)p.seed, (uint32_t)(p.seed >> 32), rr);
@@ -453,6 +454,18 @@ WNB_API int wnb_decode_stream(int32_t* xs, const float* h, const float* up_w, co
                               const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P,
                               int max_n, int n_pad, int Th, int Q, int A, int Ap, int R, int S, int ks, int U,
                               int mode, uint64_t seed, void* stream_handle) {
+  return wnb_decode_stream_at(xs, h, up_w, up_b, wf, bf, stream, b1, b2, bp1, bp2, host_dilations, L, queues, n_samples,
+                              uniforms, logits_out, B, P, max_n, n_pad, Th, Q, A, Ap, R, S, ks, U, mode, seed, 0, 0, 0,
+                              stream_handle);
+}
+
+WNB_API int wnb_decode_stream_at(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
+                                 const float* bf, const float* stream, const float* b1, const float* b2,
+                                 const float* bp1, const float* bp2, const int32_t* host_dilations, int L,
+                                 void* queues, const int32_t* n_samples, const float* uniforms, float* logits_out,
+                                 int B, int P, int max_n, int n_pad, int Th, int Q, int A, int Ap, int R, int S, int ks,
+                                 int U, int mode, uint64_t seed, int pos0, int xs_base, int h_frame0,
+                                 void* stream_handle) {
   WNB_REQUIRE(B > 0 && P >= 1 && max_n >= 1 && Th >= 1 && Q > 0 && A > 0 && Ap >= A && R > 0 && S > 0 && ks >= 1 &&
                   U >= 0 && L >= 1, "decode_stream: bad shape");
   WNB_REQUIRE(xs && h && wf && bf && stream && b1 && b2 && bp1 && bp2 && n_samples && (queues || ks == 1),
@@ -466,6 +479,11 @@ WNB_API int wnb_decode_stream(int32_t* xs, const float* h, const float* up_w, co
   p.logits_out = logits_out;
   p.B = B; p.P = P; p.max_n = max_n; p.n_pad = n_pad; p.Th = Th; p.Q = Q; p.A = A; p.Ap = Ap; p.R = R; p.S = S;
   p.ks = ks; p.U = U; p.mode = mode; p.L = L; p.seed = seed;
+  DecodeWindow win;
+  if (!decode_window("decode_stream", P, n_pad, U, ks, max_n, Th, pos0, xs_base, h_frame0, &win)) return WNB_ERR_INVALID;
+  p.pos0 = win.pos0; p.i0 = win.i0; p.i_last = win.i_last; p.h_last = win.h_last; p.stride_xs = win.stride_xs;
+  p.xs = shift_ptr(xs, -(long long)xs_base); p.h = shift_ptr(h, -(long long)h_frame0);
+  p.uniforms = shift_ptr(uniforms, -(long long)win.i0); p.logits_out = shift_ptr(logits_out, -(long long)win.i0 * Q);
   p.O1 = (2 * R + 3) & ~3; p.Or = (R + 3) & ~3; p.Os = (S + 3) & ~3; p.Sp = p.Os; p.Qp = (Q + 3) & ~3;
   const long long K1 = (long long)ks * R + Ap;
   p.off_w2res = K1 * p.O1;

@@ -61,6 +61,7 @@ struct Params {
   const float* stream;
   float* queues; const int32_t* n_samples; const float* uniforms; float* logits_out;
   int B, P, max_n, n_pad, Th, A, U, mode, L, nslot, split, big;
+  int pos0, i0, i_last, h_last, stride_xs;   // the call's window (common.cuh DecodeWindow)
   long long rank_stride;   // cluster form: floats between the two CTAs' streams
   unsigned long long seed;
   int dil[kMaxL];
@@ -284,7 +285,7 @@ __global__ void __launch_bounds__((W / CL) * 32 + 64, 1) decode_warp_kernel(cons
   const int rank = (CL == 2) ? (int)cluster_ctarank() : 0;
   const int vw = rank * WP + warp;          // virtual warp: owns gate channels CH*vw.., skip columns SV*vw.., logits QV*vw..
   const int u0 = (blockIdx.x / CL) * NU;
-  const int stride_xs = p.P + p.max_n;
+  const int stride_xs = p.stride_xs;
 
   if (tid == 0) {
     for (int i = 0; i < p.nslot; i++) {
@@ -295,12 +296,12 @@ __global__ void __launch_bounds__((W / CL) * 32 + 64, 1) decode_warp_kernel(cons
     *ready = 0u;
     ptx::fence_barrier_init();
   }
-  if (tid < NU) s_n[tid] = (u0 + tid < p.B) ? p.n_samples[u0 + tid] : 0;
+  if (tid < NU) s_n[tid] = (u0 + tid < p.B) ? p.i0 + p.n_samples[u0 + tid] : 0;   // absolute end
   __syncthreads();
   int nmax = 0;
 #pragma unroll
   for (int u = 0; u < NU; u++) nmax = max(nmax, s_n[u]);
-  if (nmax == 0) return;
+  if (nmax <= p.i0) return;
   XSync xs_{0u, 0u, 0u};
   uint32_t peer_delta = 0;
   if constexpr (CL == 2) {
@@ -328,7 +329,7 @@ __global__ void __launch_bounds__((W / CL) * 32 + 64, 1) decode_warp_kernel(cons
   if (warp == WP) {
     // ================================ producer warp ================================
     if (lane == 0) {
-      for (int pos = 0; pos <= last_pos; pos++) {
+      for (int pos = p.pos0; pos <= last_pos; pos++) {
         const bool want = pos >= p.P - 1;
         for (int l = 0; l < L; l++) {
           const float* base = my_stream + (size_t)l * kLayerF;
@@ -369,7 +370,7 @@ __global__ void __launch_bounds__((W / CL) * 32 + 64, 1) decode_warp_kernel(cons
     if (lane == 0) {
       const int per_layer_warm = kW1One ? 1 : ((BIG ? 2 : 3) + 1), per_layer_skip = 64 / KPC;
       const int post_chunks = 1 + kS / KPC + kS / (2 * KPC);
-      for (int pos = 0; pos <= last_pos; pos++) {
+      for (int pos = p.pos0; pos <= last_pos; pos++) {
         const bool want = pos >= p.P - 1;
         const int n = L * (per_layer_warm + (want ? per_layer_skip : 0)) + (want ? post_chunks : 0);
         for (int i = 0; i < n; i++) ring.gate();
@@ -389,10 +390,10 @@ __global__ void __launch_bounds__((W / CL) * 32 + 64, 1) decode_warp_kernel(cons
       if (a < p.A) {
         const int j = max(pos_t - p.n_pad, 0);
         if (p.U > 0) {
-          const int tf = min(j / p.U, p.Th - 1), jj = j % p.U;
+          const int tf = min(j / p.U, p.h_last), jj = j % p.U;
           v = fmaf(__ldg(p.h + ((size_t)ug * p.A + a) * p.Th + tf), __ldg(p.up_w + jj), __ldg(p.up_b));
         } else {
-          v = __ldg(p.h + ((size_t)ug * p.A + a) * p.Th + min(j, p.Th - 1));
+          v = __ldg(p.h + ((size_t)ug * p.A + a) * p.Th + min(j, p.h_last));
         }
       }
       hcol[e] = v;
@@ -420,7 +421,7 @@ __global__ void __launch_bounds__((W / CL) * 32 + 64, 1) decode_warp_kernel(cons
   float* my_pre = pre_s + warp * GV * NU;
   long long tacc[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   long long tlast = clock64();
-  for (int pos = 0; pos <= last_pos; pos++) {
+  for (int pos = p.pos0; pos <= last_pos; pos++) {
     const bool want = pos >= p.P - 1;
     if (pos == p.P - 1 && p.timing && tid == 0) {   // time only the free-running steps
       for (int i = 0; i < 12; i++) tacc[i] = 0;
@@ -750,7 +751,7 @@ __global__ void __launch_bounds__((W / CL) * 32 + 64, 1) decode_warp_kernel(cons
         if (p.mode == WNB_MODE_SAMPLING) {
           float uni;
           if (p.uniforms) {
-            uni = p.uniforms[(size_t)min(u0 + u, p.B - 1) * p.max_n + min(i, p.max_n - 1)];
+            uni = p.uniforms[(size_t)min(u0 + u, p.B - 1) * p.max_n + min(i, p.i_last)];
           } else if (uni_for == i) {
             uni = uni_next;            // drawn during the previous step's pick, off the critical path
           } else {
@@ -957,6 +958,16 @@ WNB_API int wnb_decode_warp(int32_t* xs, const float* h, const float* up_w, cons
                             const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P,
                             int max_n, int n_pad, int Th, int A, int U, int mode, uint64_t seed, int W, int CL,
                             void* stream_handle) {
+  return wnb_decode_warp_at(xs, h, up_w, up_b, wf, bf, stream, b1, b2, bp1, bp2, host_dilations, L, queues, n_samples,
+                            uniforms, logits_out, B, P, max_n, n_pad, Th, A, U, mode, seed, W, CL, 0, 0, 0, stream_handle);
+}
+
+WNB_API int wnb_decode_warp_at(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
+                               const float* bf, const float* stream, const float* b1, const float* b2, const float* bp1,
+                               const float* bp2, const int32_t* host_dilations, int L, void* queues,
+                               const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P,
+                               int max_n, int n_pad, int Th, int A, int U, int mode, uint64_t seed, int W, int CL,
+                               int pos0, int xs_base, int h_frame0, void* stream_handle) {
   WNB_REQUIRE(B > 0 && P >= 1 && max_n >= 1 && Th >= 1 && A > 0 && A <= dw::kAp && U >= 0 && L >= 1 && L <= dw::kMaxL,
               "decode_warp: bad shape");
   WNB_REQUIRE(xs && h && wf && bf && stream && b1 && b2 && bp1 && bp2 && n_samples && queues,
@@ -969,6 +980,12 @@ WNB_API int wnb_decode_warp(int32_t* xs, const float* h, const float* up_w, cons
   p.logits_out = logits_out;
   p.B = B; p.P = P; p.max_n = max_n; p.n_pad = n_pad; p.Th = Th; p.A = A; p.U = U; p.mode = mode; p.L = L;
   p.seed = seed;
+  const int Q = dw::kQ;
+  DecodeWindow win;
+  if (!decode_window("decode_warp", P, n_pad, U, 2, max_n, Th, pos0, xs_base, h_frame0, &win)) return WNB_ERR_INVALID;
+  p.pos0 = win.pos0; p.i0 = win.i0; p.i_last = win.i_last; p.h_last = win.h_last; p.stride_xs = win.stride_xs;
+  p.xs = shift_ptr(xs, -(long long)xs_base); p.h = shift_ptr(h, -(long long)h_frame0);
+  p.uniforms = shift_ptr(uniforms, -(long long)win.i0); p.logits_out = shift_ptr(logits_out, -(long long)win.i0 * Q);
   p.timing = g_decode_timing;
   long long off = 0;
   for (int l = 0; l < L; l++) {

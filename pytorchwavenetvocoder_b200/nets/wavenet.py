@@ -13,6 +13,7 @@ hand-written sm_90a kernel reached through the C ABI in ``include/wnb200.h``:
 PyTorch only owns the memory, the parameters and the streams.  There is no CPU fallback: calling the
 model with CPU tensors raises.
 """
+import collections
 import ctypes
 import logging
 import sys
@@ -27,7 +28,7 @@ from .. import _lib
 from .._lib import MATH_BF16, MATH_FP32, MATH_TF32, MODE_ARGMAX, MODE_SAMPLING, check, ptr, stream
 
 __all__ = ["encode_mu_law", "decode_mu_law", "initialize", "OneHot", "CausalConv1d", "UpSampling",
-           "WaveNet", "cross_entropy", "mulaw_pcm16_table", "codes_to_pcm16"]
+           "WaveNet", "cross_entropy", "mulaw_pcm16_table", "codes_to_pcm16", "DecodeSession", "decode_window"]
 
 # bench.py sets this to a list to get (start, end) CUDA-event pairs around every fused-block launch
 PROFILE_EVENTS = None
@@ -579,6 +580,208 @@ def _round_up(a, m):
     return (a + m - 1) // m * m
 
 
+# ------------------------------------------------------------------------------------------
+# resumable decoding (include/wnb200.h, wnb_decode_at): host arithmetic and the session object
+# ------------------------------------------------------------------------------------------
+DecodeWindow = collections.namedtuple("DecodeWindow", "pos0 end i0 n counts xs_base h_frame0")
+
+# positions are int in the kernels: the last xs column written (P - 1 + the longest utterance) must stay below this
+MAX_DECODE_POSITION = 2 ** 31 - 2
+
+
+def decode_window(pos, frames, P, n_pad, U, ks, totals):
+    """The next call of a resumable decode session: which positions it runs and the window arguments of wnb_decode_at.
+
+    ``pos`` is the first padded position not yet run, ``frames`` the aux columns received so far (frames before
+    up-sampling when U > 0, sample-rate columns when U == 0), ``P = max(T0, receptive_field)``, ``n_pad = P - T0``,
+    ``totals`` the samples wanted per utterance.  Position p needs aux column ``max(p - n_pad, 0)``, i.e. frame
+    ``max(p - n_pad, 0) // U``, so after ``frames`` frames the positions ``p < n_pad + frames * max(U, 1)`` can run.
+    A call runs ``pos0 = pos`` up to ``end - 1`` and must generate at least one sample, so the P - 1 warm-up positions run
+    in the first call that also reaches sample 0 (with a one-sample seed, the first call).  Returns None when no sample
+    can be generated yet, else a DecodeWindow: ``i0`` the first sample index, ``n`` the samples of the longest utterance
+    (max_n of the call), ``counts`` the samples per utterance (capped by ``totals``), ``xs_base`` the first xs column
+    the call reads, ``h_frame0`` the first aux frame it reads."""
+    Uc = max(U, 1)
+    avail = n_pad + frames * Uc if frames > 0 else 0
+    end = min(avail, P - 1 + max(totals))
+    n = end - max(pos, P - 1)
+    if n <= 0:
+        return None
+    i0 = max(pos - (P - 1), 0)
+    counts = [min(max(t - i0, 0), n) for t in totals]
+    return DecodeWindow(pos, end, i0, n, counts, max(pos - (ks - 1), 0), max(pos - n_pad, 0) // Uc)
+
+
+class DecodeSession(object):
+    """A resumable decode of a batch of utterances, fed with aux frames as they arrive (``WaveNet.decode_session``).
+
+    Each ``step(h_chunk)`` runs one launch of the decoder the one-shot path would use for this batch and returns the
+    samples whose aux has now arrived; the chained calls compute exactly what ``batch_fast_generate`` computes for the
+    same seed, whatever the chunk sizes.  Everything the calls share lives here, created once: the launch form, a snapshot
+    of the packed weights (and of ``decode_math``), the dilation queues, the last ks - 1 samples and the seed.  All
+    utterances advance together; utterance b stops at ``n_samples_list[b]``."""
+
+    def __init__(self, net, x, n_samples_list, mode="sampling", seed=None, uniforms=None, return_logits=False,
+                 kernel="auto"):
+        if mode not in ("sampling", "argmax"):
+            logging.error("mode should be sampling or argmax")
+            sys.exit(1)
+        if not x.is_cuda:
+            raise _lib.WnbError("decode sessions need CUDA tensors: this build has no CPU fallback")
+        lib = _lib.load()
+        decode_math = getattr(net, "decode_math", "fp32")
+        if decode_math not in ("fp32", "bf16"):
+            raise ValueError("decode_math should be fp32 or bf16, got %r" % (decode_math,))
+        if kernel == "auto":
+            kernel = "bf16" if decode_math == "bf16" else "auto"
+        self.device = dev = x.device
+        B, T0 = x.shape
+        self.totals = [int(n) for n in n_samples_list]
+        if len(self.totals) != B or min(self.totals) < 0:
+            raise ValueError("n_samples_list should hold %d non-negative lengths, got %r" % (B, n_samples_list))
+        self.Q, self.A, self.Ap, self.R, self.S, self.ks, self.U = (
+            net.n_quantize, net.n_aux, net.n_aux_pad, net.n_resch, net.n_skipch, net.kernel_size, net.upsampling_factor)
+        Q, Ap, R, S, ks, U = self.Q, self.Ap, self.R, self.S, self.ks, self.U
+        self.B, self.P = B, max(T0, net.receptive_field)
+        self.n_pad = self.P - T0
+        if self.P - 1 + max(self.totals) > MAX_DECODE_POSITION:
+            raise ValueError("a decode session covers at most %d positions (%d requested)"
+                             % (MAX_DECODE_POSITION, self.P - 1 + max(self.totals)))
+        L = len(net.dilations)
+        self.L = L
+        self.dil = (ctypes.c_int32 * L)(*net.dilations)
+        self.mode = MODE_ARGMAX if mode == "argmax" else MODE_SAMPLING
+        # a snapshot: _decode_pack() hands some entries (the front and post biases) out as the parameters themselves, and
+        # an in-place update of the model (load_state_dict, an optimizer step) must not reach a running session
+        params = {p.untyped_storage().data_ptr() for p in net.parameters()}
+        self.w = {k: v.clone() if v.untyped_storage().data_ptr() in params else v
+                  for k, v in net._decode_pack().items()}
+        if kernel == "bf16":
+            if not lib.wnb_decode_bf16_supported(Q, Ap, R, S, ks, L):
+                raise _lib.WnbError("decode_math='bf16' does not cover this model (n_quantize %d, n_aux %d, n_resch %d, "
+                                    "n_skipch %d, kernel_size %d, %d layers): see decode_bf16_supported()"
+                                    % (Q, self.A, R, S, ks, L))
+            self.wstream = net._decode_bf16_pack()
+            qbytes = lib.wnb_decode_bf16_workspace(B, R, ks, self.dil, L)
+        else:
+            form = (ctypes.c_int32 * 4)()
+            warp_ok = (lib.wnb_decode_warp_supported(Q, Ap, R, S, ks, L)
+                       and lib.wnb_decode_warp_form(B, L, form) == 0)
+            if kernel == "warp" and not warp_ok:
+                raise _lib.WnbError("decode kernel 'warp' does not cover this configuration")
+            if kernel == "auto":
+                kernel = "warp" if warp_ok else "stream"
+            if kernel == "warp":
+                self.W, self.CL = lib.wnb_decode_warp_plan(B), lib.wnb_decode_warp_cluster(B)
+                self.wstream = net._decode_warp_pack(self.W, self.CL)
+            elif kernel == "stream":
+                self.wstream = net._decode_stream_pack(self.w)
+            elif kernel != "direct":
+                raise ValueError("unknown decode kernel %r" % (kernel,))
+            qbytes = lib.wnb_decode_workspace(B, R, ks, self.dil, L)
+        self.kernel = kernel
+        self.queues = torch.empty(max(qbytes // 4, 1), dtype=torch.float32, device=dev)
+        self.upw = net.upsampling.conv.weight.detach().float().contiguous().view(-1).clone() if U > 0 else None
+        self.upb = net.upsampling.conv.bias.detach().float().contiguous().view(-1).clone() if U > 0 else None
+        if seed is None:
+            seed = int(torch.empty((), dtype=torch.int64).random_().item())  # follows torch.manual_seed, like _decode
+        self.seed = ctypes.c_uint64(seed & 0xFFFFFFFFFFFFFFFF)
+        self.uniforms = None if uniforms is None else uniforms.to(dev).float().contiguous()
+        self.return_logits = return_logits
+        self._totals_dev = torch.tensor(self.totals, dtype=torch.int32, device=dev)
+        # xs carry: the seed prefix first, then the last ks - 1 positions a call has written (absolute column _xs_base)
+        self._xs = torch.full((B, self.P), Q // 2, dtype=torch.int32, device=dev)
+        self._xs[:, self.n_pad:] = x.to(torch.int32)
+        self._xs_base = 0
+        # aux frames received and not yet behind every position run (absolute frame _h0 first)
+        self._h = torch.empty(B, self.A, 0, dtype=torch.float32, device=dev)
+        self._h0 = 0
+        self.frames = 0
+        self.pos = 0
+        self.last_counts = [0] * B
+        self._pcm_tab = torch.from_numpy(mulaw_pcm16_table(Q)).to(dev)
+
+    @property
+    def done(self):
+        """True once every utterance has all its samples."""
+        return self.pos >= self.P - 1 + max(self.totals)
+
+    def step(self, h_chunk):
+        """Feed the next aux frames ``(B, n_aux, F)`` (sample-rate columns when the model has no up-sampling layer) and
+        decode every position whose aux has now arrived.  Returns the new codes as a ``(B, n)`` int32 device tensor,
+        without synchronising; row b holds ``last_counts[b]`` valid samples (an utterance past its length gets none).
+        With ``return_logits`` the ``(B, n, Q)`` teacher-check logits come as a second value."""
+        lib = _lib.load()
+        if self.done:
+            raise RuntimeError("decode session: every utterance has finished")
+        if not h_chunk.is_cuda:
+            raise _lib.WnbError("decode sessions need CUDA tensors: this build has no CPU fallback")
+        if h_chunk.dim() != 3 or h_chunk.size(0) != self.B or h_chunk.size(1) != self.A:
+            raise ValueError("aux chunk should be (%d, %d, frames), got %s" % (self.B, self.A, tuple(h_chunk.shape)))
+        self._h = torch.cat([self._h, h_chunk.to(self.device).float()], 2)
+        self.frames += h_chunk.size(2)
+        win = decode_window(self.pos, self.frames, self.P, self.n_pad, self.U, self.ks, self.totals)
+        B, Q = self.B, self.Q
+        if win is None:
+            self.last_counts = [0] * B
+            gen = torch.empty(B, 0, dtype=torch.int32, device=self.device)
+            return (gen, torch.empty(B, 0, Q, device=self.device)) if self.return_logits else gen
+        h = self._h[:, :, win.h_frame0 - self._h0:].contiguous()
+        xs = torch.full((B, win.end + 1 - win.xs_base), Q // 2, dtype=torch.int32, device=self.device)
+        hi = min(self._xs_base + self._xs.size(1), win.end + 1)
+        xs[:, :hi - win.xs_base] = self._xs[:, win.xs_base - self._xs_base:hi - self._xs_base]
+        nsm = (self._totals_dev - win.i0).clamp_(0, win.n)
+        uni = None if self.uniforms is None else self.uniforms[:, win.i0:win.i0 + win.n].contiguous()
+        lg = torch.empty(B, win.n, Q, dtype=torch.float32, device=self.device) if self.return_logits else None
+        w, st = self.w, stream()
+        common = (B, self.P, win.n, self.n_pad, h.size(2))
+        window = (win.pos0, win.xs_base, win.h_frame0, st)
+        if self.kernel == "bf16":
+            rc = lib.wnb_decode_bf16_at(ptr(xs), ptr(h), ptr(self.upw), ptr(self.upb), ptr(w["wf"]), ptr(w["bf"]),
+                                        ptr(self.wstream), self.dil, self.L, ptr(self.queues), ptr(nsm), ptr(uni), ptr(lg),
+                                        *common, Q, self.A, self.Ap, self.R, self.S, self.ks, self.U, self.mode, self.seed,
+                                        *window)
+        elif self.kernel == "warp":
+            rc = lib.wnb_decode_warp_at(ptr(xs), ptr(h), ptr(self.upw), ptr(self.upb), ptr(w["wf"]), ptr(w["bf"]),
+                                        ptr(self.wstream), ptr(w["b1"]), ptr(w["b2"]), ptr(w["bp1"]), ptr(w["bp2"]),
+                                        self.dil, self.L, ptr(self.queues), ptr(nsm), ptr(uni), ptr(lg), *common, self.A,
+                                        self.U, self.mode, self.seed, self.W, self.CL, *window)
+        else:
+            rc = -3
+            if self.kernel == "stream":
+                rc = lib.wnb_decode_stream_at(ptr(xs), ptr(h), ptr(self.upw), ptr(self.upb), ptr(w["wf"]), ptr(w["bf"]),
+                                              ptr(self.wstream), ptr(w["b1"]), ptr(w["b2"]), ptr(w["bp1"]),
+                                              ptr(w["bp2"]), self.dil, self.L, ptr(self.queues), ptr(nsm), ptr(uni),
+                                              ptr(lg), *common, Q, self.A, self.Ap, self.R, self.S, self.ks, self.U,
+                                              self.mode, self.seed, *window)
+                if rc == -3 and win.pos0 == 0:   # shape outside the streaming kernel: the direct one, as _decode does
+                    self.kernel = "direct"
+            if self.kernel == "direct":
+                rc = lib.wnb_decode_at(ptr(xs), ptr(h), ptr(self.upw), ptr(self.upb), ptr(w["wf"]), ptr(w["bf"]),
+                                       ptr(w["w1d"]), ptr(w["b1"]), ptr(w["w2d"]), ptr(w["b2"]), ptr(w["wp1d"]),
+                                       ptr(w["bp1"]), ptr(w["wp2d"]), ptr(w["bp2"]), self.dil, self.L, ptr(self.queues),
+                                       ptr(nsm), ptr(uni), ptr(lg), *common, Q, self.A, self.Ap, self.R, self.S, self.ks,
+                                       self.U, self.mode, self.seed, *window)
+        check(rc, "decode_%s_at" % self.kernel)
+        self._xs, self._xs_base = xs, win.xs_base
+        self.pos = win.end
+        f = max(self.pos - self.n_pad, 0) // max(self.U, 1)   # frames before the next position are no longer needed
+        self._h, self._h0 = self._h[:, :, f - self._h0:], f
+        self.last_counts = win.counts
+        gen = xs[:, self.P + win.i0 - win.xs_base:self.P + win.i0 + win.n - win.xs_base]
+        return (gen, lg) if self.return_logits else gen
+
+    def step_pcm16(self, h_chunk):
+        """``step`` with the new samples as PCM_16 (``decode_mu_law`` + the wav writer's quantisation, one gather
+        kernel): a ``(B, n)`` int16 device tensor, without synchronising."""
+        gen = self.step(h_chunk)
+        codes = (gen[0] if self.return_logits else gen).contiguous()
+        out = torch.empty(codes.shape, dtype=torch.int16, device=self.device)
+        check(_lib.load().wnb_lut_i16(ptr(codes), ptr(self._pcm_tab), ptr(out), codes.numel(), self.Q, stream()),
+              "lut_i16")
+        return out
+
+
 class WaveNet(nn.Module):
     """CONDITIONAL WAVENET (reference wavenet.py:157-549).
 
@@ -1016,3 +1219,16 @@ class WaveNet(nn.Module):
             logging.info("%d utterances, %d samples generated in %.3f sec (%.6f sec / sample step)" % (
                 len(n_list), sum(n_list), el, el / max(max(n_list), 1)))
         return outs
+
+    def decode_session(self, x, n_samples_list=None, mode="sampling", seed=None):
+        """Start a resumable decode of the batch with seed samples ``x`` (B, T0) on the GPU: feed aux frames with
+        ``DecodeSession.step`` as they arrive and get the new samples back after each call.  Chunked decoding equals
+        ``batch_fast_generate`` (same ``seed``, or the same ``torch.manual_seed``) bit for bit, whatever the chunk sizes.
+        ``n_samples_list`` gives each utterance's length; None leaves the lengths open, so that every call decodes all the
+        aux it has been given (up to the session's position limit).  The session snapshots the weights and
+        ``decode_math`` now; later changes to the model do not reach it."""
+        if n_samples_list is None:
+            P = max(x.size(1), self.receptive_field)
+            n_samples_list = [MAX_DECODE_POSITION - (P - 1)] * x.size(0)
+        with torch.no_grad():
+            return DecodeSession(self, x, n_samples_list, mode, seed)

@@ -1,2 +1,2 @@
 from .utils import *  # noqa
-from .utils import have_soundfile, read_wav, write_wav, write_wav_pcm16  # noqa
+from .utils import have_soundfile, read_wav, write_wav, write_wav_pcm16, WavWriter  # noqa

@@ -220,3 +220,43 @@ def write_wav(path, x, fs):
             w.setsampwidth(2)
             w.setframerate(int(fs))
             w.writeframes(pcm.tobytes())
+
+
+class WavWriter(object):
+    """Mono PCM_16 wav written chunk by chunk, byte-identical to ``write_wav`` (float samples, ``write``) or
+    ``write_wav_pcm16`` (int16 samples, ``write_pcm16``) of the whole signal: soundfile's ``SoundFile`` in write mode when
+    present, else the stdlib ``wave`` writer; both patch the RIFF sizes on ``close``."""
+
+    def __init__(self, path, fs):
+        try:
+            import soundfile as sf
+            self._sf = sf.SoundFile(path, "w", int(fs), 1, "PCM_16")
+            self._w = None
+        except ImportError:
+            import wave
+            self._sf = None
+            self._w = wave.open(path, "wb")
+            self._w.setnchannels(1)
+            self._w.setsampwidth(2)
+            self._w.setframerate(int(fs))
+
+    def write(self, x):
+        if self._sf is not None:
+            self._sf.write(np.asarray(x))
+        else:
+            self.write_pcm16(np.clip(np.round(np.asarray(x, dtype=np.float64) * 32768.0), -32768, 32767))
+
+    def write_pcm16(self, pcm):
+        if self._sf is not None:
+            self._sf.write(np.ascontiguousarray(pcm, dtype=np.int16))
+        else:
+            self._w.writeframes(np.ascontiguousarray(pcm, dtype="<i2").tobytes())
+
+    def close(self):
+        (self._sf if self._sf is not None else self._w).close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
