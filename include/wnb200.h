@@ -392,6 +392,31 @@ WNB_API int wnb_decode_bf16_at(int32_t* xs, const float* h, const float* up_w, c
                                int max_n, int n_pad, int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
                                uint64_t seed, int pos0, int xs_base, int h_frame0, void* stream_handle);
 
+/* ---- the teacher-forced warm-up computed in parallel over time (csrc/decode_prefill.cu) ------------------------------
+ * wnb_decode_warp_prefill writes into `queues` (the workspace of wnb_decode_warp, same B) exactly what
+ * wnb_decode_warp_at(pos0 = 0) leaves there after the warm-up positions 0 .. P - 2, bit for bit, without running them one
+ * by one; the caller then runs wnb_decode_warp_at with pos0 = P - 1, xs_base = 0, h_frame0 = 0 and the same xs, h, CL.
+ * Only layer l's last S_l = (ks - 1) * (d_l + ... + d_{L-1}) warm-up positions are computed, so the cost does not depend
+ * on the seed length.  Queue slots of positions < 0 are left as they are, like the sequential warm-up leaves them.
+ *   xs      (B, P) int32, the padded seed prefix (columns 0 .. P - 1 of wnb_decode_warp's xs);
+ *   h, up_w, up_b, n_pad, Th, A, U   as for wnb_decode_warp (h_frame0 = 0);
+ *   w1d (L,160,128), b1 (L,128), w2d (L,64,576), b2 (L,576)   the plain K-major decode weights of wnb_decode, 16-byte
+ *           aligned (the arithmetic is fixed per element, not per layout, so the warp-tiled stream is not needed);
+ *   CL      wnb_decode_warp_cluster(B): the 2-CTA form sums half of the residual products in another order;
+ *   scratch wnb_decode_prefill_workspace(B, P, 64, 2, dilations, L) bytes (two fp32 copies of x_l over the largest
+ *           window; 0 bytes, and scratch may be NULL, when P == 1).
+ * Covers the shapes of wnb_decode_warp_supported; WNB_ERR_INVALID for a bad shape or pointer, before any device work. */
+/* the pruned windows: windows[l] = S_l = (ks - 1) * (d_l + ... + d_{L-1}), the warm-up positions before P - 1 on which
+ * layer l's input is needed (the prefill computes layer l's input on max(0, P - 1 - S_l) .. P - 2); WNB_ERR_INVALID for a
+ * dilation < 1.  wnb_decode_prefill_workspace returns 0 for such dilations. */
+WNB_API int wnb_decode_prefill_windows(const int32_t* host_dilations, int L, int ks, int64_t* windows);
+WNB_API size_t wnb_decode_prefill_workspace(int B, int P, int R, int ks, const int32_t* host_dilations, int L);
+WNB_API int wnb_decode_warp_prefill(const int32_t* xs, const float* h, const float* up_w, const float* up_b,
+                                    const float* wf, const float* bf, const float* w1d, const float* b1,
+                                    const float* w2d, const float* b2, const int32_t* host_dilations, int L,
+                                    void* queues, void* scratch, int B, int P, int n_pad, int Th, int A, int U, int CL,
+                                    void* stream_handle);
+
 #ifdef __cplusplus
 }
 #endif

@@ -612,6 +612,31 @@ def decode_window(pos, frames, P, n_pad, U, ks, totals):
     return DecodeWindow(pos, end, i0, n, counts, max(pos - (ks - 1), 0), max(pos - n_pad, 0) // Uc)
 
 
+def decode_prefill_windows(dilations, ks):
+    """The pruned windows of the parallel warm-up (csrc/decode_prefill.cu): ``S[l] = (ks - 1) * sum(dilations[l:])``, the
+    number of warm-up positions just before P - 1 on which layer l's input x_l is needed.  Layer l's queue holds its last
+    (ks - 1) * d_l, and x_{l+1} on its own window needs x_l on taps up to (ks - 1) * d_l further back; x_L is never
+    queued.  The library computes the same windows (``wnb_decode_prefill_windows``: the prefill launcher's ranges and the
+scratch size of ``wnb_decode_prefill_workspace``); the CPU tier checks that both agree."""
+    out, S = [], 0
+    for d in reversed(dilations):
+        S += (ks - 1) * d
+        out.append(S)
+    return out[::-1]
+
+
+def _warp_prefill(lib, xs, P, h, upw, upb, w, dil, L, queues, n_pad, A, U, CL):
+    """Run the warm-up positions 0 .. P - 2 of ``wnb_decode_warp`` in parallel over time (wnb_decode_warp_prefill):
+    the queues then hold what the sequential warm-up leaves there, and ``wnb_decode_warp_at`` continues from P - 1."""
+    B = xs.size(0)
+    nbytes = lib.wnb_decode_prefill_workspace(B, P, 64, 2, dil, L)
+    scratch = torch.empty(nbytes // 4, dtype=torch.float32, device=xs.device) if nbytes else None
+    check(lib.wnb_decode_warp_prefill(ptr(xs[:, :P].contiguous()), ptr(h), ptr(upw), ptr(upb), ptr(w["wf"]),
+                                      ptr(w["bf"]), ptr(w["w1d"]), ptr(w["b1"]), ptr(w["w2d"]), ptr(w["b2"]), dil, L,
+                                      ptr(queues), ptr(scratch), B, P, n_pad, h.size(2), A, U, CL, stream()),
+          "decode_warp_prefill")
+
+
 class DecodeSession(object):
     """A resumable decode of a batch of utterances, fed with aux frames as they arrive (``WaveNet.decode_session``).
 
@@ -742,6 +767,10 @@ class DecodeSession(object):
                                         *common, Q, self.A, self.Ap, self.R, self.S, self.ks, self.U, self.mode, self.seed,
                                         *window)
         elif self.kernel == "warp":
+            if win.pos0 == 0:   # the warm-up in parallel over time, then this call from P - 1 (xs and h start at 0)
+                _warp_prefill(lib, xs, self.P, h, self.upw, self.upb, w, self.dil, self.L, self.queues, self.n_pad,
+                              self.A, self.U, self.CL)
+                window = (self.P - 1, 0, 0, st)
             rc = lib.wnb_decode_warp_at(ptr(xs), ptr(h), ptr(self.upw), ptr(self.upb), ptr(w["wf"]), ptr(w["bf"]),
                                         ptr(self.wstream), ptr(w["b1"]), ptr(w["b2"]), ptr(w["bp1"]), ptr(w["bp2"]),
                                         self.dil, self.L, ptr(self.queues), ptr(nsm), ptr(uni), ptr(lg), *common, self.A,
@@ -1149,10 +1178,14 @@ class WaveNet(nn.Module):
             Wc, CLc = lib.wnb_decode_warp_plan(B), lib.wnb_decode_warp_cluster(B)
             wstream = self._decode_warp_pack(Wc, CLc)
             assert wstream.numel() == lib.wnb_decode_warp_floats(L, CLc)
-            rc = lib.wnb_decode_warp(ptr(xs), ptr(h), ptr(upw), ptr(upb), ptr(w["wf"]), ptr(w["bf"]), ptr(wstream),
-                                     ptr(w["b1"]), ptr(w["b2"]), ptr(w["bp1"]), ptr(w["bp2"]), dil, L, ptr(queues),
-                                     ptr(nsm), ptr(uni), ptr(lg), B, P, max_n, n_pad, Th, A, U, cmode, cseed, Wc,
-                                     CLc, stream())
+            pos0 = 0
+            if lib.wnb_decode_warp_form(B, L, (ctypes.c_int32 * 4)()) == 0:   # the launch below will run: prefill first
+                _warp_prefill(lib, xs, P, h, upw, upb, w, dil, L, queues, n_pad, A, U, CLc)
+                pos0 = P - 1
+            rc = lib.wnb_decode_warp_at(ptr(xs), ptr(h), ptr(upw), ptr(upb), ptr(w["wf"]), ptr(w["bf"]), ptr(wstream),
+                                        ptr(w["b1"]), ptr(w["b2"]), ptr(w["bp1"]), ptr(w["bp2"]), dil, L, ptr(queues),
+                                        ptr(nsm), ptr(uni), ptr(lg), B, P, max_n, n_pad, Th, A, U, cmode, cseed, Wc,
+                                        CLc, pos0, 0, 0, stream())
             if rc != -3 or kernel == "warp":
                 check(rc, "decode_warp")
             if rc == 0:
