@@ -416,6 +416,23 @@ WNB_API int wnb_decode_warp_prefill(const int32_t* xs, const float* h, const flo
                                     const float* w2d, const float* b2, const int32_t* host_dilations, int L,
                                     void* queues, void* scratch, int B, int P, int n_pad, int Th, int A, int U, int CL,
                                     void* stream_handle);
+/* wnb_decode_bf16_prefill: the same for the bf16 decoder (csrc/decode_bf16_prefill.cu).  After the call `queues` (the
+ * workspace of wnb_decode_bf16, same B, wnb_decode_bf16_workspace() bytes) holds exactly what wnb_decode_bf16_at(pos0 = 0)
+ * leaves there after the warm-up positions 0 .. P - 2, bit for bit, padding rows of each cluster included; the caller
+ * then runs wnb_decode_bf16_at with pos0 = P - 1, xs_base = 0, h_frame0 = 0 and the same xs, h, weights.  The call clears
+ * the queues first, as the pos0 = 0 call does.
+ *   xs      (B, P) int32, the padded seed prefix (columns 0 .. P - 1 of wnb_decode_bf16's xs);
+ *   h, up_w, up_b, wf, bf, weights, n_pad, Th, A, Ap, R, S, ks, U   as for wnb_decode_bf16 (h_frame0 = 0);
+ *   scratch wnb_decode_bf16_prefill_workspace(B, P, R, ks, dilations, L) bytes (x_l as fp32 and bf16 and the gate output
+ *           z as bf16 over the largest window; 0 bytes, and scratch may be NULL, when P == 1).
+ * WNB_ERR_INVALID for a bad shape or pointer and WNB_ERR_UNSUPPORTED for a shape outside wnb_decode_bf16_supported, both
+ * before any device work.  wnb_decode_bf16_prefill_workspace returns 0 for a bad shape or a dilation < 1. */
+WNB_API size_t wnb_decode_bf16_prefill_workspace(int B, int P, int R, int ks, const int32_t* host_dilations, int L);
+WNB_API int wnb_decode_bf16_prefill(const int32_t* xs, const float* h, const float* up_w, const float* up_b,
+                                    const float* wf, const float* bf, const void* weights,
+                                    const int32_t* host_dilations, int L, void* queues, void* scratch, int B, int P,
+                                    int n_pad, int Th, int A, int Ap, int R, int S, int ks, int U,
+                                    void* stream_handle);
 
 #ifdef __cplusplus
 }

@@ -60,25 +60,20 @@
 // Taps before the start (t - s < 0) read slots nobody has written yet in this session: zeros.
 //
 // Warm-up: the teacher-forced prefix steps (P - 1 of them, P = max(T0, receptive field)) run the gate and res+skip
-// products only (no post network, no pick).  Every wait is bounded by %globaltimer (tc_ptx.cuh) and traps; nothing in
-// the wgmma pipeline makes a call.
+// products only (no post network, no pick); decode_bf16_prefill.cu computes the same queue bits in parallel over time,
+// and a launch with pos0 = P - 1 continues from them.  Every wait is bounded by %globaltimer (tc_ptx.cuh) and traps;
+// nothing in the wgmma pipeline makes a call.
 //
 // Shared memory per CTA (R = 512, ks = 3, A = 80 -> aux K 128): x 64 KB + z 64 KB + aux 16 KB + ring 3 x 24 KB
 // (W1 chunk 128 x 64 bf16 = 16 KB + tap tile 8 KB) = 216 KB + 1 KB alignment slack + ~1.3 KB static, under the 227 KB
 // limit; a fourth stage (240 KB) does not fit.  The launcher takes as many stages as fit, at most 8 (R = 256: 8).
-#include "common.cuh"
-#include "tc_ptx.cuh"
+#include "decode_bf16_common.cuh"
 
 namespace wnb {
 namespace db {
 
-constexpr int kCL = 8;                    // CTAs per cluster (the portable maximum)
-constexpr int kM = 64;                    // utterance rows per cluster (wgmma M)
-constexpr int kQ = 256;
-constexpr int kQc = kQ / kCL;             // classes per CTA (post-2 N)
+// kCL, kM (here: utterance rows per cluster), kQ, kQc, kTile, kCons: decode_bf16_common.cuh
 constexpr int kMaxL = 64;
-constexpr int kTile = kM * 64 * 2;        // one [64 rows][64 ch] bf16 tile: 8 KB
-constexpr int kCons = 128;                // one consumer warpgroup
 constexpr int kThreads = kCons + 32;      // + producer warp
 constexpr int kMaxStages = 8;
 constexpr int kSmemLimit = 227 * 1024;
@@ -98,20 +93,6 @@ struct Params {
   long long qslot[kMaxL];         // first slot of layer l's queue
 };
 
-// byte offset of (row, k < 64) in a [64 rows][64] bf16 tile with the 128B swizzle; of (row, channel) in a buffer of tiles
-__device__ __forceinline__ uint32_t tile_off(int row, int k) {
-  return (uint32_t)(row * 128 + ((((k >> 3) ^ row) & 7) << 4) + ((k & 7) << 1));
-}
-__device__ __forceinline__ uint32_t act_off(int row, int ch) { return (uint32_t)((ch >> 6) * kTile) + tile_off(row, ch & 63); }
-
-__device__ __forceinline__ uint32_t ld_shared_b32(uint32_t a) {
-  uint32_t v;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_shared_b32(uint32_t a, uint32_t v) {
-  asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
-}
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -134,12 +115,7 @@ __device__ __forceinline__ void st_async_b32(uint32_t raddr, uint32_t v, uint32_
   asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];"
                ::"r"(raddr), "r"(v), "r"(rbar) : "memory");
 }
-__device__ __forceinline__ void bulk_g2s(uint32_t smem, const void* gmem, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem), "l"(gmem), "r"(bytes), "r"(ptx::smem_u32(bar)) : "memory");
-}
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
-__device__ __forceinline__ void cons_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kCons) : "memory"); }
 // the step barrier: release.cluster arrive on CTA `rank`'s barrier at `bar`'s offset / acquire.cluster wait on our own
 __device__ __forceinline__ void arrive_release_cluster(uint64_t* bar, uint32_t rank) {
   const uint32_t remote = mapa_u32(ptx::smem_u32(bar), rank);
@@ -170,68 +146,6 @@ __device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t
     k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
   }
   out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
-}
-
-// consumer side of the weight ring: stage `st` of phase parity `ph`; a stage is released (one arrive per warp) once the
-// wgmma group that read it has completed
-struct Ring {
-  uint32_t base; uint64_t* full; uint64_t* empty; int n; int bytes; int st; uint32_t ph; int prev;
-  __device__ __forceinline__ uint32_t wait() {
-    ptx::mbar_wait(&full[st], ph);
-    return base + (uint32_t)(st * bytes);
-  }
-  __device__ __forceinline__ void release(int s, int lane) {
-    __syncwarp();
-    if (lane == 0) ptx::mbar_arrive(&empty[s]);
-  }
-  // after the wgmma group of the current stage was committed: wait for it (M = 64 products are short; the producer keeps
-  // the other stages streaming meanwhile), then hand the previous stage back
-  __device__ __forceinline__ void committed(int lane) {
-    ptx::wg_wait<0>();
-    if (prev >= 0) release(prev, lane);
-    prev = st;
-    if (++st == n) { st = 0; ph ^= 1u; }
-  }
-};
-// a copy of v the compiler cannot see through: keeps per-thread address arithmetic inside the step / layer loops
-// instead of hoisting dozens of loop-invariant offsets into registers for the whole kernel
-__device__ __forceinline__ int opaque(int v) {
-  asm volatile("mov.b32 %0, %0;" : "+r"(v));
-  return v;
-}
-
-// one [64 x 64] A tile times one [N x 64] B tile, accumulated into d: 4 k16 steps, A fragments from shared memory
-template <int N>
-__device__ __forceinline__ void mma_tile(float (&d)[N / 2], uint32_t (&a)[4][4], uint32_t a_tile, uint32_t b_tile, int fr,
-                                         int fk) {
-#pragma unroll
-  for (int s = 0; s < 4; s++)
-#pragma unroll
-    for (int h = 0; h < 4; h++) a[s][h] = ld_shared_b32(a_tile + tile_off(fr + 8 * (h & 1), 16 * s + fk + 8 * (h >> 1)));
-  ptx::wg_fence();
-#pragma unroll
-  for (int s = 0; s < 4; s++) ptx::wgmma_rs_bf16<N>(d, a[s], ptx::gmma_desc_k_sw128(b_tile + 32 * s), 1);
-  ptx::wg_commit();
-}
-
-// d = sum over nch ring stages of A(c) x B(stage c); `pre(c)` runs before chunk c waits for its stage.  Returns the
-// shared-memory address of the last stage, which is NOT released yet (its bias tail is still to be read).
-template <int N, class ATile, class Pre>
-__device__ __forceinline__ uint32_t product(float (&d)[N / 2], Ring& rg, int nch, ATile atile, Pre pre, int fr, int fk,
-                                            int lane) {
-#pragma unroll
-  for (int i = 0; i < N / 2; i++) d[i] = 0.f;
-  uint32_t a[4][4];
-  uint32_t last = 0;
-#pragma unroll 1
-  for (int c = 0; c < nch; c++) {
-    pre(c);
-    last = rg.wait();
-    mma_tile<N>(d, a, atile(c, last), last, fr, fk);
-    rg.committed(lane);
-  }
-  ptx::wg_touch(d);
-  return last;
 }
 
 template <int R, int S>
@@ -668,7 +582,6 @@ __global__ void __launch_bounds__(kThreads, 1) decode_bf16_kernel(const Params p
 // ---------------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------------
-static int db_aux_k(int Ap) { return (Ap + 63) / 64 * 64; }
 static bool db_shape_ok(int R, int S) { return (R == 256 && S == 256) || (R == 512 && (S == 256 || S == 512)); }
 static int db_stage_bytes(int R, int S) {
   const int NG = R / 4, NR = R / 8 + S / 8;
@@ -684,13 +597,6 @@ static int db_stages(int R, int S, int Ap) {
   if (n > db::kMaxStages) n = db::kMaxStages;
   return n >= 3 ? n : 0;
 }
-static size_t db_cta_bytes(int Ap, int R, int S, int ks) {
-  const size_t NG = R / 4, NR = R / 8 + S / 8;
-  const size_t gate_k = (size_t)db_aux_k(Ap) + (size_t)ks * R;
-  const size_t layer = NG * gate_k * 2 + NG * 4 + NR * (size_t)R * 2 + NR * 4;
-  return layer;   // per layer; the post tail is added by the callers
-}
-static size_t db_post_bytes(int S) { return (size_t)(S / 8) * S * 2 + (S / 8) * 4 + (size_t)db::kQc * S * 2 + db::kQc * 4; }
 
 }  // namespace wnb
 
@@ -763,8 +669,8 @@ WNB_API int wnb_decode_bf16_at(int32_t* xs, const float* h, const float* up_w, c
   p.uniforms = shift_ptr(uniforms, -(long long)win.i0); p.logits_out = shift_ptr(logits_out, -(long long)win.i0 * Q);
   p.nstage = db_stages(R, S, Ap);
   p.stage_bytes = db_stage_bytes(R, S);
-  const int ncl = cdiv(B, db::kM);
-  p.bc = cdiv(B, ncl);
+  int ncl;
+  db_split(B, &ncl, &p.bc);
   p.cta_bytes = (long long)((size_t)L * db_cta_bytes(Ap, R, S, ks) + db_post_bytes(S));
   long long slots = 0;
   for (int l = 0; l < L; l++) {

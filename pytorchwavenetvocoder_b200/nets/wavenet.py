@@ -637,6 +637,18 @@ def _warp_prefill(lib, xs, P, h, upw, upb, w, dil, L, queues, n_pad, A, U, CL):
           "decode_warp_prefill")
 
 
+def _bf16_prefill(lib, xs, P, h, upw, upb, w, wstream, dil, L, queues, n_pad, A, Ap, R, S, ks, U):
+    """Run the warm-up positions 0 .. P - 2 of the bf16 decoder in parallel over time (wnb_decode_bf16_prefill): the
+    queues then hold what the sequential warm-up leaves there, and ``wnb_decode_bf16_at`` continues from P - 1."""
+    B = xs.size(0)
+    nbytes = lib.wnb_decode_bf16_prefill_workspace(B, P, R, ks, dil, L)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=xs.device) if nbytes else None
+    check(lib.wnb_decode_bf16_prefill(ptr(xs[:, :P].contiguous()), ptr(h), ptr(upw), ptr(upb), ptr(w["wf"]),
+                                      ptr(w["bf"]), ptr(wstream), dil, L, ptr(queues), ptr(scratch), B, P, n_pad,
+                                      h.size(2), A, Ap, R, S, ks, U, stream()),
+          "decode_bf16_prefill")
+
+
 class DecodeSession(object):
     """A resumable decode of a batch of utterances, fed with aux frames as they arrive (``WaveNet.decode_session``).
 
@@ -762,6 +774,10 @@ class DecodeSession(object):
         common = (B, self.P, win.n, self.n_pad, h.size(2))
         window = (win.pos0, win.xs_base, win.h_frame0, st)
         if self.kernel == "bf16":
+            if win.pos0 == 0:   # the warm-up in parallel over time, then this call from P - 1 (xs and h start at 0)
+                _bf16_prefill(lib, xs, self.P, h, self.upw, self.upb, w, self.wstream, self.dil, self.L, self.queues,
+                              self.n_pad, self.A, self.Ap, self.R, self.S, self.ks, self.U)
+                window = (self.P - 1, 0, 0, st)
             rc = lib.wnb_decode_bf16_at(ptr(xs), ptr(h), ptr(self.upw), ptr(self.upb), ptr(w["wf"]), ptr(w["bf"]),
                                         ptr(self.wstream), self.dil, self.L, ptr(self.queues), ptr(nsm), ptr(uni), ptr(lg),
                                         *common, Q, self.A, self.Ap, self.R, self.S, self.ks, self.U, self.mode, self.seed,
@@ -1168,9 +1184,11 @@ class WaveNet(nn.Module):
                                     % (Q, A, R, S, ks, L))
             wstream = self._decode_bf16_pack()
             assert wstream.numel() == lib.wnb_decode_bf16_weights(Q, Ap, R, S, ks, L)
-            check(lib.wnb_decode_bf16(ptr(xs), ptr(h), ptr(upw), ptr(upb), ptr(w["wf"]), ptr(w["bf"]), ptr(wstream), dil,
-                                      L, ptr(queues), ptr(nsm), ptr(uni), ptr(lg), B, P, max_n, n_pad, Th, Q, A, Ap, R, S,
-                                      ks, U, cmode, cseed, stream()), "decode_bf16")
+            # the warm-up in parallel over time, then the decoder from P - 1
+            _bf16_prefill(lib, xs, P, h, upw, upb, w, wstream, dil, L, queues, n_pad, A, Ap, R, S, ks, U)
+            check(lib.wnb_decode_bf16_at(ptr(xs), ptr(h), ptr(upw), ptr(upb), ptr(w["wf"]), ptr(w["bf"]), ptr(wstream),
+                                         dil, L, ptr(queues), ptr(nsm), ptr(uni), ptr(lg), B, P, max_n, n_pad, Th, Q, A,
+                                         Ap, R, S, ks, U, cmode, cseed, P - 1, 0, 0, stream()), "decode_bf16")
             self.last_decode_kernel = "bf16"
             gen = xs[:, P:]
             return (gen, lg) if return_logits else gen
