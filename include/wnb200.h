@@ -266,42 +266,64 @@ WNB_API int wnb_post_bwd(const float* skip, const float* r1, const float* dlogit
 WNB_API int wnb_cross_entropy(const float* logits, const int64_t* target /*(B,T)*/, double* loss_sum,
                       float* dlogits, int B, int T, int Q, int start, void* stream);
 
-/* ---- a14/a15/a16: persistent fast-generate kernel (wavenet.py:309-395, 397-511, 538-549) ----
- * One launch generates every sample of every utterance.  Queues live in `queues` (caller-allocated,
- * wnb_decode_workspace() bytes, need not be zeroed).
- *   xs      (B, P + max_n) int32: [0,P) = the padded/seed prefix (wavenet.py:330-334), the rest is
- *           written by the kernel (xs[b][P+i] = i-th generated sample);
- *   h       (B, A, Th) aux features BEFORE upsampling (U>0) or at sample rate (U==0);
- *   n_pad   number of left-replicated aux columns (wavenet.py:334): aux at padded position p is
- *           h_up[max(p - n_pad, 0)];
- *   n_samples (B) int32 per-utterance lengths; mode WNB_MODE_*; uniforms (B,max_n) optional
- *           externally supplied U[0,1) draws (tests), else Philox4x32-10(seed, utterance, step);
- *   logits_out (B, max_n, Q) optional teacher-check output (NULL in production).
- * Decode weights are K-major: wf (ks,Q,R), w1d (L,K1,2R), b1 (L,2R), w2d (L,R,R+S), b2 (L,R+S),
- * wp1d (S,S) [c][o], wp2d (S,Q) [c][o]. */
+/* ---- a14/a15/a16: persistent fast-generate kernels (wavenet.py:309-395, 397-511, 538-549) ----------------------------
+ * Four decoders, one entry point each: wnb_decode_at (weights read directly from L2), wnb_decode_stream_at,
+ * wnb_decode_warp_at and wnb_decode_bf16_at.  One launch generates the samples of every utterance over one window of
+ * padded positions, pos0 .. max(pos0, P - 1) + max_n - 1.  pos0 = xs_base = h_frame0 = 0 runs the whole range in one
+ * call: the P - 1 teacher-forced warm-up positions, then every sample.  A chain of calls, each starting where the previous
+ * one stopped, computes exactly what one call over the whole range computes, bit for bit, whatever the chunk boundaries,
+ * so a session can decode an utterance chunk by chunk as its aux frames arrive.  The arguments the four share:
+ *   P, n_pad   keep their absolute meaning: P - 1 warm-up positions, then sample i at position P - 1 + i; n_pad is the
+ *              number of left-replicated aux columns (wavenet.py:334): aux at padded position p is h_up[max(p - n_pad, 0)];
+ *   pos0       0 (the first call: it runs the whole warm-up) or >= P - 1.  A call generates at least one sample, so a
+ *              chain never starts a call inside the warm-up; 0 < pos0 < P - 1 is rejected;
+ *   i0         = max(pos0 - (P - 1), 0), the first sample index of the call;
+ *   n_samples  (B) int32, the samples to generate in this call per utterance (sample indices i0 .. i0 + n_b - 1),
+ *              max_n >= every n_b; the call stops after max_n samples;
+ *   xs         (B, max(pos0, P - 1) + max_n + 1 - xs_base) int32: column c is absolute position xs_base + c.  The call
+ *              reads positions pos0 - (ks - 1) .. (those >= 0; so xs_base <= max(pos0 - (ks - 1), 0)), which must hold the
+ *              padded seed prefix (wavenet.py:330-334) or what earlier calls generated, and writes position P + i with
+ *              sample i;
+ *   h          (B, A, Th) aux features BEFORE upsampling (U > 0, with up_w / up_b) or at sample rate (U == 0): column c is
+ *              absolute frame h_frame0 + c (aux column max(p - n_pad, 0), divided by U when U > 0); h_frame0 <= the frame
+ *              of pos0.  Lookups past the last column are clamped to it;
+ *   mode       WNB_MODE_*; uniforms (B, max_n) optional externally supplied U[0,1) draws (tests), else
+ *              Philox4x32-10(seed, utterance, step);
+ *   logits_out (B, max_n, Q) optional teacher-check output (NULL in production).  It and uniforms are indexed by the
+ *              call's own sample index i - i0; the in-kernel Philox counter keeps the absolute i, so a sampled stream does
+ *              not depend on the chunk boundaries;
+ *   queues     the dilation queues, caller-allocated (wnb_decode_workspace() bytes, need not be zeroed; the bf16 decoder
+ *              has its own size).  Between the calls of one chain the caller keeps them untouched and the same B (hence the
+ *              same launch form: NU / W / CL of wnb_decode_warp_at, the utterances per CTA of wnb_decode_stream_at /
+ *              wnb_decode_at, the cluster split of wnb_decode_bf16_at); the fp32 decoders never need cleared queues,
+ *              wnb_decode_bf16_at clears them when pos0 == 0 only.
+ * Positions are int: the last position written must stay below 2^31 - 1.  WNB_ERR_INVALID for an inconsistent window. */
 WNB_API size_t wnb_decode_workspace(int B, int R, int ks, const int32_t* host_dilations, int L);
-WNB_API int wnb_decode(int32_t* xs, const float* h, const float* up_w, const float* up_b,
-               const float* wf, const float* bf, const float* w1d, const float* b1, const float* w2d,
-               const float* b2, const float* wp1d, const float* bp1, const float* wp2d, const float* bp2,
-               const int32_t* host_dilations, int L, void* queues, const int32_t* n_samples,
-               const float* uniforms, float* logits_out, int B, int P, int max_n, int n_pad, int Th,
-               int Q, int A, int Ap, int R, int S, int ks, int U, int mode, uint64_t seed,
-               void* stream);
 
-/* ---- a14-a16, streaming variant: same contract as wnb_decode, but the K-major matrices arrive as ONE
+/* Decode weights of wnb_decode_at are K-major: wf (ks,Q,R), w1d (L,K1,2R), b1 (L,2R), w2d (L,R,R+S), b2 (L,R+S),
+ * wp1d (S,S) [c][o], wp2d (S,Q) [c][o]. */
+WNB_API int wnb_decode_at(int32_t* xs, const float* h, const float* up_w, const float* up_b,
+                          const float* wf, const float* bf, const float* w1d, const float* b1, const float* w2d,
+                          const float* b2, const float* wp1d, const float* bp1, const float* wp2d, const float* bp2,
+                          const int32_t* host_dilations, int L, void* queues, const int32_t* n_samples,
+                          const float* uniforms, float* logits_out, int B, int P, int max_n, int n_pad, int Th,
+                          int Q, int A, int Ap, int R, int S, int ks, int U, int mode, uint64_t seed,
+                          int pos0, int xs_base, int h_frame0, void* stream);
+
+/* ---- a14-a16, streaming variant: same contract as wnb_decode_at, but the K-major matrices arrive as ONE
  * packed stream consumed in order every step (a producer warp pushes it through a shared-memory ring
  * with cp.async.bulk while the consumer warps run the recurrence):
  *   per layer l: W1d [K1][O1] | W2res [R][Or] | W2skip [R][Os]   then  wp1d [S][Sp] | wp2d [S][Qp]
  * with O1 = 2R, Or = R, Os = Sp = S, Qp = Q each rounded up to a multiple of 4 (zero padded).
- * Returns WNB_ERR_UNSUPPORTED when the shape does not fit (caller uses wnb_decode). */
+ * Returns WNB_ERR_UNSUPPORTED when the shape does not fit, before any device work (the caller may run wnb_decode_at). */
 WNB_API size_t wnb_decode_stream_floats(int Q, int Ap, int R, int S, int ks, int L);
-WNB_API int wnb_decode_stream(int32_t* xs, const float* h, const float* up_w, const float* up_b,
-                              const float* wf, const float* bf, const float* stream, const float* b1,
-                              const float* b2, const float* bp1, const float* bp2,
-                              const int32_t* host_dilations, int L, void* queues, const int32_t* n_samples,
-                              const float* uniforms, float* logits_out, int B, int P, int max_n, int n_pad,
-                              int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
-                              uint64_t seed, void* stream_handle);
+WNB_API int wnb_decode_stream_at(int32_t* xs, const float* h, const float* up_w, const float* up_b,
+                                 const float* wf, const float* bf, const float* stream, const float* b1,
+                                 const float* b2, const float* bp1, const float* bp2,
+                                 const int32_t* host_dilations, int L, void* queues, const int32_t* n_samples,
+                                 const float* uniforms, float* logits_out, int B, int P, int max_n, int n_pad,
+                                 int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
+                                 uint64_t seed, int pos0, int xs_base, int h_frame0, void* stream_handle);
 
 /* ---- a14-a16, warp-tiled variant for the BASELINE shape (R 64, S 512, Q 256, Ap 32, ks 2): same contract,
  * weights as ONE stream in warp-tile order (layout documented in csrc/decode_warp.cu; built by
@@ -312,80 +334,32 @@ WNB_API size_t wnb_decode_warp_floats(int L, int CL);
 /* debug aid: per-phase cycle counters of the free-running steps (16 int64 per CTA; NULL = off) */
 WNB_API void wnb_decode_warp_set_timing(long long* device_buf);
 WNB_API int wnb_decode_warp_supported(int Q, int Ap, int R, int S, int ks, int L);
-WNB_API int wnb_decode_warp(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
-                            const float* bf, const float* stream, const float* b1, const float* b2,
-                            const float* bp1, const float* bp2, const int32_t* host_dilations, int L,
-                            void* queues, const int32_t* n_samples, const float* uniforms, float* logits_out,
-                            int B, int P, int max_n, int n_pad, int Th, int A, int U, int mode, uint64_t seed,
-                            int W, int CL, void* stream_handle);
-/* consumer warps (8 or 16) / CTAs per utterance (1 or 2) the launcher uses for B utterances; the stream layout depends
- * on both */
-WNB_API int wnb_decode_warp_plan(int B);
-WNB_API int wnb_decode_warp_cluster(int B);
-/* the kernel instantiation decode_warp_kernel<NU, W, BIG, CL> that wnb_decode_warp runs for B utterances of L layers,
- * under the current WNB_DECODE_BIG: form[0..3] = NU (utterances per CTA), W (consumer warps), CL (CTAs per cluster),
- * BIG (1: three 64 KB ring slots, 0: up to six 32 KB slots).  WNB_ERR_UNSUPPORTED when no ring fits. */
-WNB_API int wnb_decode_warp_form(int B, int L, int32_t* form);
-
-/* ---- a14-a16, opt-in bf16 tensor-core variant for the recipe sizes (WaveNet.decode_math = "bf16"): same contract as
- * wnb_decode_stream (xs, pre-upsampling h with up_w / up_b, n_pad, ragged n_samples, supplied uniforms or in-kernel
- * Philox with counter (step, batch index, 0, 0), optional logits_out, xs[b][P + n_b ..] untouched), but every product
- * multiplies bf16 operands (fp32 accumulation) and the batch runs as ceil(B / 64) clusters of 8 CTAs (csrc/decode_bf16.cu).
- * `weights` is the packed bf16 stream of wnb_decode_bf16_weights() 16-bit elements (layout in csrc/decode_bf16.cu,
- * built by nets/wavenet.py::_decode_bf16_pack; the biases ride inside it); `queues` holds
- * wnb_decode_bf16_workspace() bytes and is cleared by the call.  Covered (wnb_decode_bf16_supported): Q 256, ks 2 or 3,
- * Ap <= 256, R/S 256/256, 512/256 or 512/512, L <= 64; otherwise WNB_ERR_UNSUPPORTED (no fallback). */
-WNB_API int wnb_decode_bf16_supported(int Q, int Ap, int R, int S, int ks, int L);
-WNB_API size_t wnb_decode_bf16_weights(int Q, int Ap, int R, int S, int ks, int L);
-WNB_API size_t wnb_decode_bf16_workspace(int B, int R, int ks, const int32_t* host_dilations, int L);
-WNB_API int wnb_decode_bf16(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
-                            const float* bf, const void* weights, const int32_t* host_dilations, int L, void* queues,
-                            const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P,
-                            int max_n, int n_pad, int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
-                            uint64_t seed, void* stream_handle);
-
-/* ---- resumable decode: the four decoders above, one time window per call ------------------------------------------
- * Each _at entry point takes its twin's arguments plus (pos0, xs_base, h_frame0) and runs padded positions
- * pos0 .. max(pos0, P - 1) + max_n - 1 only, so a session can decode an utterance chunk by chunk as its aux frames arrive;
- * the twin is the call with pos0 = xs_base = h_frame0 = 0.  A chain of calls, each starting where the previous one
- * stopped, computes exactly what one call over the whole range computes, bit for bit, whatever the chunk boundaries.
- *   P, n_pad   keep their absolute meaning (P - 1 teacher-forced warm-up positions, then sample i at position P - 1 + i);
- *   pos0       0 (the first call of a session: it runs the whole warm-up) or >= P - 1.  A call generates at least one
- *              sample, so a chain never starts a call inside the warm-up; 0 < pos0 < P - 1 is rejected;
- *   i0         = max(pos0 - (P - 1), 0), the first sample index of the call;
- *   n_samples  (B) samples to generate in this call per utterance (sample indices i0 .. i0 + n_b - 1), max_n >= every
- *              n_b; the call stops after max_n samples;
- *   xs         (B, max(pos0, P - 1) + max_n + 1 - xs_base) int32: column c is absolute position xs_base + c.  The call
- *              reads positions pos0 - (ks - 1) .. (those >= 0; so xs_base <= max(pos0 - (ks - 1), 0)), which must hold the
- *              seed prefix or what earlier calls generated, and writes position pos + 1 for each sample it generates;
- *   h          (B, A, Th): column c is absolute frame h_frame0 + c (aux column max(p - n_pad, 0), divided by U when
- *              U > 0); h_frame0 <= the frame of pos0.  Lookups past the last column are clamped to it;
- *   uniforms   (B, max_n) and logits_out (B, max_n, Q) are indexed by the call's own sample index i - i0; the in-kernel
- *              Philox counter keeps the absolute i, so a sampled stream does not depend on the chunk boundaries.
- * Between the calls of one session the caller keeps the queue workspace untouched and the same B (hence the same
- * launch form: NU / W / CL of wnb_decode_warp, the utterances per CTA of wnb_decode_stream / wnb_decode, the cluster split
- * of wnb_decode_bf16); the fp32 decoders never need cleared queues, wnb_decode_bf16_at clears them when pos0 == 0 only.
- * Positions are int: the last position written must stay below 2^31 - 1.  WNB_ERR_INVALID for an inconsistent window. */
-WNB_API int wnb_decode_at(int32_t* xs, const float* h, const float* up_w, const float* up_b,
-                          const float* wf, const float* bf, const float* w1d, const float* b1, const float* w2d,
-                          const float* b2, const float* wp1d, const float* bp1, const float* wp2d, const float* bp2,
-                          const int32_t* host_dilations, int L, void* queues, const int32_t* n_samples,
-                          const float* uniforms, float* logits_out, int B, int P, int max_n, int n_pad, int Th,
-                          int Q, int A, int Ap, int R, int S, int ks, int U, int mode, uint64_t seed,
-                          int pos0, int xs_base, int h_frame0, void* stream);
-WNB_API int wnb_decode_stream_at(int32_t* xs, const float* h, const float* up_w, const float* up_b,
-                                 const float* wf, const float* bf, const float* stream, const float* b1,
-                                 const float* b2, const float* bp1, const float* bp2,
-                                 const int32_t* host_dilations, int L, void* queues, const int32_t* n_samples,
-                                 const float* uniforms, float* logits_out, int B, int P, int max_n, int n_pad,
-                                 int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
-                                 uint64_t seed, int pos0, int xs_base, int h_frame0, void* stream_handle);
 WNB_API int wnb_decode_warp_at(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
                                const float* bf, const float* stream, const float* b1, const float* b2,
                                const float* bp1, const float* bp2, const int32_t* host_dilations, int L,
                                void* queues, const int32_t* n_samples, const float* uniforms, float* logits_out,
                                int B, int P, int max_n, int n_pad, int Th, int A, int U, int mode, uint64_t seed,
                                int W, int CL, int pos0, int xs_base, int h_frame0, void* stream_handle);
+/* consumer warps (8 or 16) / CTAs per utterance (1 or 2) the launcher uses for B utterances; the stream layout depends
+ * on both */
+WNB_API int wnb_decode_warp_plan(int B);
+WNB_API int wnb_decode_warp_cluster(int B);
+/* the kernel instantiation decode_warp_kernel<NU, W, BIG, CL> that wnb_decode_warp_at runs for B utterances of L layers,
+ * under the current WNB_DECODE_BIG: form[0..3] = NU (utterances per CTA), W (consumer warps), CL (CTAs per cluster),
+ * BIG (1: three 64 KB ring slots, 0: up to six 32 KB slots).  WNB_ERR_UNSUPPORTED when no ring fits. */
+WNB_API int wnb_decode_warp_form(int B, int L, int32_t* form);
+
+/* ---- a14-a16, opt-in bf16 tensor-core variant for the recipe sizes (WaveNet.decode_math = "bf16"): same contract as
+ * wnb_decode_stream_at (xs, pre-upsampling h with up_w / up_b, n_pad, ragged n_samples, supplied uniforms or in-kernel
+ * Philox with counter (step, batch index, 0, 0), optional logits_out, xs[b][P + n_b ..] untouched), but every product
+ * multiplies bf16 operands (fp32 accumulation) and the batch runs as ceil(B / 64) clusters of 8 CTAs (csrc/decode_bf16.cu).
+ * `weights` is the packed bf16 stream of wnb_decode_bf16_weights() 16-bit elements (layout in csrc/decode_bf16.cu,
+ * built by nets/wavenet.py::_decode_bf16_pack; the biases ride inside it); `queues` holds
+ * wnb_decode_bf16_workspace() bytes and is cleared by a call with pos0 == 0.  Covered (wnb_decode_bf16_supported): Q 256,
+ * ks 2 or 3, Ap <= 256, R/S 256/256, 512/256 or 512/512, L <= 64; otherwise WNB_ERR_UNSUPPORTED (no fallback). */
+WNB_API int wnb_decode_bf16_supported(int Q, int Ap, int R, int S, int ks, int L);
+WNB_API size_t wnb_decode_bf16_weights(int Q, int Ap, int R, int S, int ks, int L);
+WNB_API size_t wnb_decode_bf16_workspace(int B, int R, int ks, const int32_t* host_dilations, int L);
 WNB_API int wnb_decode_bf16_at(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
                                const float* bf, const void* weights, const int32_t* host_dilations, int L, void* queues,
                                const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P,
@@ -393,14 +367,14 @@ WNB_API int wnb_decode_bf16_at(int32_t* xs, const float* h, const float* up_w, c
                                uint64_t seed, int pos0, int xs_base, int h_frame0, void* stream_handle);
 
 /* ---- the teacher-forced warm-up computed in parallel over time (csrc/decode_prefill.cu) ------------------------------
- * wnb_decode_warp_prefill writes into `queues` (the workspace of wnb_decode_warp, same B) exactly what
+ * wnb_decode_warp_prefill writes into `queues` (the workspace of wnb_decode_warp_at, same B) exactly what
  * wnb_decode_warp_at(pos0 = 0) leaves there after the warm-up positions 0 .. P - 2, bit for bit, without running them one
  * by one; the caller then runs wnb_decode_warp_at with pos0 = P - 1, xs_base = 0, h_frame0 = 0 and the same xs, h, CL.
  * Only layer l's last S_l = (ks - 1) * (d_l + ... + d_{L-1}) warm-up positions are computed, so the cost does not depend
  * on the seed length.  Queue slots of positions < 0 are left as they are, like the sequential warm-up leaves them.
- *   xs      (B, P) int32, the padded seed prefix (columns 0 .. P - 1 of wnb_decode_warp's xs);
- *   h, up_w, up_b, n_pad, Th, A, U   as for wnb_decode_warp (h_frame0 = 0);
- *   w1d (L,160,128), b1 (L,128), w2d (L,64,576), b2 (L,576)   the plain K-major decode weights of wnb_decode, 16-byte
+ *   xs      (B, P) int32, the padded seed prefix (columns 0 .. P - 1 of the xs of wnb_decode_warp_at);
+ *   h, up_w, up_b, n_pad, Th, A, U   as for wnb_decode_warp_at (h_frame0 = 0);
+ *   w1d (L,160,128), b1 (L,128), w2d (L,64,576), b2 (L,576)   the plain K-major decode weights of wnb_decode_at, 16-byte
  *           aligned (the arithmetic is fixed per element, not per layout, so the warp-tiled stream is not needed);
  *   CL      wnb_decode_warp_cluster(B): the 2-CTA form sums half of the residual products in another order;
  *   scratch wnb_decode_prefill_workspace(B, P, 64, 2, dilations, L) bytes (two fp32 copies of x_l over the largest
@@ -417,12 +391,12 @@ WNB_API int wnb_decode_warp_prefill(const int32_t* xs, const float* h, const flo
                                     void* queues, void* scratch, int B, int P, int n_pad, int Th, int A, int U, int CL,
                                     void* stream_handle);
 /* wnb_decode_bf16_prefill: the same for the bf16 decoder (csrc/decode_bf16_prefill.cu).  After the call `queues` (the
- * workspace of wnb_decode_bf16, same B, wnb_decode_bf16_workspace() bytes) holds exactly what wnb_decode_bf16_at(pos0 = 0)
+ * workspace of wnb_decode_bf16_at, same B, wnb_decode_bf16_workspace() bytes) holds exactly what wnb_decode_bf16_at(pos0 = 0)
  * leaves there after the warm-up positions 0 .. P - 2, bit for bit, padding rows of each cluster included; the caller
  * then runs wnb_decode_bf16_at with pos0 = P - 1, xs_base = 0, h_frame0 = 0 and the same xs, h, weights.  The call clears
  * the queues first, as the pos0 = 0 call does.
- *   xs      (B, P) int32, the padded seed prefix (columns 0 .. P - 1 of wnb_decode_bf16's xs);
- *   h, up_w, up_b, wf, bf, weights, n_pad, Th, A, Ap, R, S, ks, U   as for wnb_decode_bf16 (h_frame0 = 0);
+ *   xs      (B, P) int32, the padded seed prefix (columns 0 .. P - 1 of the xs of wnb_decode_bf16_at);
+ *   h, up_w, up_b, wf, bf, weights, n_pad, Th, A, Ap, R, S, ks, U   as for wnb_decode_bf16_at (h_frame0 = 0);
  *   scratch wnb_decode_bf16_prefill_workspace(B, P, R, ks, dilations, L) bytes (x_l as fp32 and bf16 and the gate output
  *           z as bf16 over the largest window; 0 bytes, and scratch may be NULL, when P == 1).
  * WNB_ERR_INVALID for a bad shape or pointer and WNB_ERR_UNSUPPORTED for a shape outside wnb_decode_bf16_supported, both

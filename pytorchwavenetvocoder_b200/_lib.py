@@ -54,20 +54,16 @@ SIGNATURES = {
     "wnb_post_bwd": (_I, [_P] * 11 + [_I] * 5 + [_P]),
     "wnb_cross_entropy": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "wnb_decode_workspace": (_c.c_size_t, [_I, _I, _I, _P, _I]),
-    "wnb_decode": (_I, [_P] * 14 + [_P, _I] + [_P] * 4 + [_I] * 13 + [_c.c_uint64, _P]),
     "wnb_decode_stream_floats": (_c.c_size_t, [_I] * 6),
-    "wnb_decode_stream": (_I, [_P] * 11 + [_P, _I] + [_P] * 4 + [_I] * 13 + [_c.c_uint64, _P]),
     "wnb_decode_warp_floats": (_c.c_size_t, [_I, _I]),
     "wnb_decode_warp_set_timing": (None, [_P]),
     "wnb_decode_warp_supported": (_I, [_I] * 6),
-    "wnb_decode_warp": (_I, [_P] * 11 + [_P, _I] + [_P] * 4 + [_I] * 8 + [_c.c_uint64, _I, _I, _P]),
     "wnb_decode_warp_plan": (_I, [_I]),
     "wnb_decode_warp_cluster": (_I, [_I]),
     "wnb_decode_warp_form": (_I, [_I, _I, _P]),
     "wnb_decode_bf16_supported": (_I, [_I] * 6),
     "wnb_decode_bf16_weights": (_c.c_size_t, [_I] * 6),
     "wnb_decode_bf16_workspace": (_c.c_size_t, [_I, _I, _I, _P, _I]),
-    "wnb_decode_bf16": (_I, [_P] * 7 + [_P, _I] + [_P] * 4 + [_I] * 13 + [_c.c_uint64, _P]),
     "wnb_decode_at": (_I, [_P] * 14 + [_P, _I] + [_P] * 4 + [_I] * 13 + [_c.c_uint64] + [_I] * 3 + [_P]),
     "wnb_decode_stream_at": (_I, [_P] * 11 + [_P, _I] + [_P] * 4 + [_I] * 13 + [_c.c_uint64] + [_I] * 3 + [_P]),
     "wnb_decode_warp_at": (_I, [_P] * 11 + [_P, _I] + [_P] * 4 + [_I] * 8 + [_c.c_uint64, _I, _I] + [_I] * 3 + [_P]),

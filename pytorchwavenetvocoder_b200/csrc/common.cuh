@@ -90,7 +90,7 @@ enum { SCRATCH_WGRAD = 0, SCRATCH_EMBED = 1, SCRATCH_AUX = 2, SCRATCH_LOSS = 3, 
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 static inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
-// The window of one resumable decode call (wnb_decode_at and its twins, include/wnb200.h).  The kernels keep absolute
+// The window of one resumable decode call (the four decode _at launchers, include/wnb200.h).  The kernels keep absolute
 // indices: the launcher shifts xs by -xs_base columns, h by -h_frame0 columns, uniforms by -i0 columns and logits_out by
 // -i0 rows, so that a kernel reads position pp at xs[.. + pp], frame f at h[.. + f], and sample i's uniform and logits at
 // i; n_samples become absolute ends (i0 + n_b).  A one-shot call is the window pos0 = xs_base = h_frame0 = 0.

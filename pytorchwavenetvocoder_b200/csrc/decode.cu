@@ -364,17 +364,6 @@ WNB_API size_t wnb_decode_workspace(int B, int R, int ks, const int32_t* host_di
   return per * sizeof(float) * (size_t)B;
 }
 
-WNB_API int wnb_decode(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf, const float* bf,
-               const float* w1d, const float* b1, const float* w2d, const float* b2, const float* wp1d,
-               const float* bp1, const float* wp2d, const float* bp2, const int32_t* host_dilations, int L,
-               void* queues, const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P,
-               int max_n, int n_pad, int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
-               uint64_t seed, void* stream) {
-  return wnb_decode_at(xs, h, up_w, up_b, wf, bf, w1d, b1, w2d, b2, wp1d, bp1, wp2d, bp2, host_dilations, L, queues,
-                       n_samples, uniforms, logits_out, B, P, max_n, n_pad, Th, Q, A, Ap, R, S, ks, U, mode, seed, 0, 0, 0,
-                       stream);
-}
-
 WNB_API int wnb_decode_at(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
                           const float* bf, const float* w1d, const float* b1, const float* w2d, const float* b2,
                           const float* wp1d, const float* bp1, const float* wp2d, const float* bp2,

@@ -632,15 +632,6 @@ WNB_API size_t wnb_decode_bf16_workspace(int B, int R, int ks, const int32_t* ho
   return (size_t)cdiv(B, db::kM) * slots * (size_t)R * db::kM * 2;
 }
 
-WNB_API int wnb_decode_bf16(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
-                            const float* bf, const void* weights, const int32_t* host_dilations, int L, void* queues,
-                            const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P, int max_n,
-                            int n_pad, int Th, int Q, int A, int Ap, int R, int S, int ks, int U, int mode,
-                            uint64_t seed, void* stream_handle) {
-  return wnb_decode_bf16_at(xs, h, up_w, up_b, wf, bf, weights, host_dilations, L, queues, n_samples, uniforms,
-                            logits_out, B, P, max_n, n_pad, Th, Q, A, Ap, R, S, ks, U, mode, seed, 0, 0, 0, stream_handle);
-}
-
 WNB_API int wnb_decode_bf16_at(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
                                const float* bf, const void* weights, const int32_t* host_dilations, int L, void* queues,
                                const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P,

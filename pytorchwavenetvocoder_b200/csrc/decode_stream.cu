@@ -400,7 +400,7 @@ static size_t stream_work_floats(int NU, int R, int S, int Qp, int Ap, int ks, i
   return (size_t)NU * (K1 + 2 * R + 2 * S + Qp + Ap + (size_t)(ks - 1) * L * R + omax);
 }
 
-// returns WNB_ERR_UNSUPPORTED when the shape does not fit this kernel (caller falls back to decode v1)
+// returns WNB_ERR_UNSUPPORTED when the shape does not fit this kernel (the caller may run wnb_decode_at instead)
 int decode_stream_launch(StreamParams& p, cudaStream_t st) {
   const int widths[5] = {p.O1, p.Or, p.Os, p.Sp, p.Qp};
   for (int i = 0; i < 5; i++)
@@ -446,17 +446,6 @@ WNB_API size_t wnb_decode_stream_floats(int Q, int Ap, int R, int S, int ks, int
   const size_t O1 = (2 * R + 3) & ~3, Or = (R + 3) & ~3, Os = (S + 3) & ~3, Sp = Os, Qp = (Q + 3) & ~3;
   const size_t K1 = (size_t)ks * R + Ap;
   return (size_t)L * (K1 * O1 + (size_t)R * Or + (size_t)R * Os) + (size_t)S * Sp + (size_t)S * Qp;
-}
-
-WNB_API int wnb_decode_stream(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
-                              const float* bf, const float* stream, const float* b1, const float* b2,
-                              const float* bp1, const float* bp2, const int32_t* host_dilations, int L, void* queues,
-                              const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P,
-                              int max_n, int n_pad, int Th, int Q, int A, int Ap, int R, int S, int ks, int U,
-                              int mode, uint64_t seed, void* stream_handle) {
-  return wnb_decode_stream_at(xs, h, up_w, up_b, wf, bf, stream, b1, b2, bp1, bp2, host_dilations, L, queues, n_samples,
-                              uniforms, logits_out, B, P, max_n, n_pad, Th, Q, A, Ap, R, S, ks, U, mode, seed, 0, 0, 0,
-                              stream_handle);
 }
 
 WNB_API int wnb_decode_stream_at(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,

@@ -911,7 +911,7 @@ WNB_API size_t wnb_decode_warp_floats(int L, int CL) {
   return per_rank * CL;
 }
 
-// debug: device buffer (16 int64 per CTA) that the next wnb_decode_warp launches fill with per-phase cycle
+// debug: device buffer (16 int64 per CTA) that the next wnb_decode_warp_at launches fill with per-phase cycle
 // counts of the free-running steps (NULL switches it off).  Slots: 0 prologue, 1 sync, 2 gate GEMV, 3 reduce+gate,
 // 4 sync, 5 res GEMV, 6 skip GEMV, 7 sync, 8 post1 (+relu+sync), 9 post2 (+sync), 10 pick (+sync)
 static long long* g_decode_timing = nullptr;
@@ -950,16 +950,6 @@ WNB_API int wnb_decode_warp_form(int B, int L, int32_t* form) {
   }
   form[0] = NU; form[1] = W; form[2] = CL; form[3] = big ? 1 : 0;
   return WNB_OK;
-}
-
-WNB_API int wnb_decode_warp(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,
-                            const float* bf, const float* stream, const float* b1, const float* b2, const float* bp1,
-                            const float* bp2, const int32_t* host_dilations, int L, void* queues,
-                            const int32_t* n_samples, const float* uniforms, float* logits_out, int B, int P,
-                            int max_n, int n_pad, int Th, int A, int U, int mode, uint64_t seed, int W, int CL,
-                            void* stream_handle) {
-  return wnb_decode_warp_at(xs, h, up_w, up_b, wf, bf, stream, b1, b2, bp1, bp2, host_dilations, L, queues, n_samples,
-                            uniforms, logits_out, B, P, max_n, n_pad, Th, A, U, mode, seed, W, CL, 0, 0, 0, stream_handle);
 }
 
 WNB_API int wnb_decode_warp_at(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,

@@ -7,7 +7,8 @@ hand-written sm_90a kernel reached through the C ABI in ``include/wnb200.h``:
 
 * ``WaveNet.forward``  (reference wavenet.py:212-241)  -> front gather, aux up-sampling, ONE fused
   kernel per residual block, post network; backward through ``torch.autograd.Function``.
-* ``fast_generate`` / ``batch_fast_generate`` (wavenet.py:309-511) -> one persistent kernel launch.
+* ``fast_generate`` / ``batch_fast_generate`` (wavenet.py:309-511) -> one persistent kernel launch, run as a
+  ``DecodeSession`` given every aux frame in one call (the same object decodes chunk by chunk as frames arrive).
 * ``encode_mu_law`` / ``decode_mu_law`` (wavenet.py:17-47) -> device kernels, numpy in / numpy out.
 
 PyTorch only owns the memory, the parameters and the streams.  There is no CPU fallback: calling the
@@ -626,7 +627,7 @@ scratch size of ``wnb_decode_prefill_workspace``); the CPU tier checks that both
 
 
 def _warp_prefill(lib, xs, P, h, upw, upb, w, dil, L, queues, n_pad, A, U, CL):
-    """Run the warm-up positions 0 .. P - 2 of ``wnb_decode_warp`` in parallel over time (wnb_decode_warp_prefill):
+    """Run the warm-up positions 0 .. P - 2 of ``wnb_decode_warp_at`` in parallel over time (wnb_decode_warp_prefill):
     the queues then hold what the sequential warm-up leaves there, and ``wnb_decode_warp_at`` continues from P - 1."""
     B = xs.size(0)
     nbytes = lib.wnb_decode_prefill_workspace(B, P, 64, 2, dil, L)
@@ -652,11 +653,16 @@ def _bf16_prefill(lib, xs, P, h, upw, upb, w, wstream, dil, L, queues, n_pad, A,
 class DecodeSession(object):
     """A resumable decode of a batch of utterances, fed with aux frames as they arrive (``WaveNet.decode_session``).
 
-    Each ``step(h_chunk)`` runs one launch of the decoder the one-shot path would use for this batch and returns the
+    This is the one place that picks a decoder and launches it: one-shot decoding (``WaveNet._decode``) is a session
+    given every aux frame in its first call.  Each ``step(h_chunk)`` runs one launch of the decoder and returns the
     samples whose aux has now arrived; the chained calls compute exactly what ``batch_fast_generate`` computes for the
     same seed, whatever the chunk sizes.  Everything the calls share lives here, created once: the launch form, a snapshot
     of the packed weights (and of ``decode_math``), the dilation queues, the last ks - 1 samples and the seed.  All
-    utterances advance together; utterance b stops at ``n_samples_list[b]``."""
+    utterances advance together; utterance b stops at ``n_samples_list[b]``.
+
+    ``kernel``: "auto" runs the bf16 decoder under ``decode_math="bf16"`` (an uncovered shape raises), and otherwise the
+    warp-tiled decoder where it covers the shape, else the streaming one, else the direct one.  A named kernel ("warp",
+    "stream", "direct", "bf16") runs that kernel or raises."""
 
     def __init__(self, net, x, n_samples_list, mode="sampling", seed=None, uniforms=None, return_logits=False,
                  kernel="auto"):
@@ -669,8 +675,12 @@ class DecodeSession(object):
         decode_math = getattr(net, "decode_math", "fp32")
         if decode_math not in ("fp32", "bf16"):
             raise ValueError("decode_math should be fp32 or bf16, got %r" % (decode_math,))
-        if kernel == "auto":
-            kernel = "bf16" if decode_math == "bf16" else "auto"
+        if kernel not in ("auto", "warp", "stream", "direct", "bf16"):
+            raise ValueError("unknown decode kernel %r" % (kernel,))
+        if kernel == "auto" and decode_math == "bf16":
+            kernel = "bf16"
+        # fp32 "auto" only: the streaming kernel finds out at its first launch whether it covers the shape
+        self._stream_fallback = kernel == "auto"
         self.device = dev = x.device
         B, T0 = x.shape
         self.totals = [int(n) for n in n_samples_list]
@@ -699,22 +709,24 @@ class DecodeSession(object):
                                     "n_skipch %d, kernel_size %d, %d layers): see decode_bf16_supported()"
                                     % (Q, self.A, R, S, ks, L))
             self.wstream = net._decode_bf16_pack()
+            assert self.wstream.numel() == lib.wnb_decode_bf16_weights(Q, Ap, R, S, ks, L)
             qbytes = lib.wnb_decode_bf16_workspace(B, R, ks, self.dil, L)
         else:
-            form = (ctypes.c_int32 * 4)()
-            warp_ok = (lib.wnb_decode_warp_supported(Q, Ap, R, S, ks, L)
-                       and lib.wnb_decode_warp_form(B, L, form) == 0)
-            if kernel == "warp" and not warp_ok:
-                raise _lib.WnbError("decode kernel 'warp' does not cover this configuration")
-            if kernel == "auto":
-                kernel = "warp" if warp_ok else "stream"
+            if kernel in ("auto", "warp"):
+                if (lib.wnb_decode_warp_supported(Q, Ap, R, S, ks, L)
+                        and lib.wnb_decode_warp_form(B, L, (ctypes.c_int32 * 4)()) == 0):
+                    kernel = "warp"
+                elif kernel == "warp":
+                    raise _lib.WnbError("decode kernel 'warp' does not cover this configuration")
+                else:
+                    kernel = "stream"
             if kernel == "warp":
                 self.W, self.CL = lib.wnb_decode_warp_plan(B), lib.wnb_decode_warp_cluster(B)
                 self.wstream = net._decode_warp_pack(self.W, self.CL)
+                assert self.wstream.numel() == lib.wnb_decode_warp_floats(L, self.CL)
             elif kernel == "stream":
                 self.wstream = net._decode_stream_pack(self.w)
-            elif kernel != "direct":
-                raise ValueError("unknown decode kernel %r" % (kernel,))
+                assert self.wstream.numel() == lib.wnb_decode_stream_floats(Q, Ap, R, S, ks, L)
             qbytes = lib.wnb_decode_workspace(B, R, ks, self.dil, L)
         self.kernel = kernel
         self.queues = torch.empty(max(qbytes // 4, 1), dtype=torch.float32, device=dev)
@@ -736,7 +748,7 @@ class DecodeSession(object):
         self.frames = 0
         self.pos = 0
         self.last_counts = [0] * B
-        self._pcm_tab = torch.from_numpy(mulaw_pcm16_table(Q)).to(dev)
+        self._pcm_tab = None   # built by the first step_pcm16: it costs a launch and a synchronisation
 
     @property
     def done(self):
@@ -799,7 +811,7 @@ class DecodeSession(object):
                                               ptr(w["bp2"]), self.dil, self.L, ptr(self.queues), ptr(nsm), ptr(uni),
                                               ptr(lg), *common, Q, self.A, self.Ap, self.R, self.S, self.ks, self.U,
                                               self.mode, self.seed, *window)
-                if rc == -3 and win.pos0 == 0:   # shape outside the streaming kernel: the direct one, as _decode does
+                if rc == -3 and self._stream_fallback and win.pos0 == 0:   # shape outside the streaming kernel
                     self.kernel = "direct"
             if self.kernel == "direct":
                 rc = lib.wnb_decode_at(ptr(xs), ptr(h), ptr(self.upw), ptr(self.upb), ptr(w["wf"]), ptr(w["bf"]),
@@ -818,7 +830,9 @@ class DecodeSession(object):
 
     def step_pcm16(self, h_chunk):
         """``step`` with the new samples as PCM_16 (``decode_mu_law`` + the wav writer's quantisation, one gather
-        kernel): a ``(B, n)`` int16 device tensor, without synchronising."""
+        kernel): a ``(B, n)`` int16 device tensor, without synchronising after the first call."""
+        if self._pcm_tab is None:
+            self._pcm_tab = torch.from_numpy(mulaw_pcm16_table(self.Q)).to(self.device)
         gen = self.step(h_chunk)
         codes = (gen[0] if self.return_logits else gen).contiguous()
         out = torch.empty(codes.shape, dtype=torch.int16, device=self.device)
@@ -1064,7 +1078,7 @@ class WaveNet(nn.Module):
                         w2d_res=pad4(W2[:, :R].transpose(1, 2)), w2d_skip=pad4(W2[:, R:].transpose(1, 2)))
 
     def _decode_stream_pack(self, w):
-        """One contiguous fp32 stream in consumption order (include/wnb200.h, wnb_decode_stream)."""
+        """One contiguous fp32 stream in consumption order (include/wnb200.h, wnb_decode_stream_at)."""
         R = self.n_resch
         parts = []
         for l in range(len(self.dilations)):
@@ -1073,7 +1087,7 @@ class WaveNet(nn.Module):
         return torch.cat(parts).contiguous()
 
     def _decode_warp_pack(self, W, CL=1):
-        """Warp-tile ordered stream for wnb_decode_warp with W (virtual) consumer warps (layout: csrc/decode_warp.cu).
+        """Warp-tile ordered stream for wnb_decode_warp_at with W (virtual) consumer warps (layout: csrc/decode_warp.cu).
         CL = 2: one stream per CTA of the cluster, back to back -- CTA r gets the tiles of warps r*W/2 .. (r+1)*W/2 - 1
         (= gate / residual channels, skip / post columns of its half) and the full bias vectors."""
         with torch.no_grad():
@@ -1135,101 +1149,23 @@ class WaveNet(nn.Module):
             return torch.cat(parts).contiguous()
 
     def _decode(self, x, h, n_samples_list, mode, uniforms=None, return_logits=False, seed=None, kernel="auto"):
-        lib = _lib.load()
-        decode_math = getattr(self, "decode_math", "fp32")
-        if decode_math not in ("fp32", "bf16"):
-            raise ValueError("decode_math should be fp32 or bf16, got %r" % (decode_math,))
-        if kernel == "auto" and decode_math == "bf16":
-            kernel = "bf16"
-        if mode not in ("sampling", "argmax"):
-            logging.error("mode should be sampling or argmax")
-            sys.exit(1)
+        """Decode every sample at once: one call of a ``DecodeSession`` given all the aux frames, i.e. one launch over
+        positions 0 .. P - 1 + max_n - 1 (after the parallel warm-up on ``warp`` and ``bf16``).  Returns the (B, max_n)
+        int32 codes, and the (B, max_n, Q) teacher-check logits with ``return_logits``; ``last_decode_kernel`` names the
+        decoder that ran.  ``x`` may be on the CPU, ``h`` may not."""
         if not h.is_cuda:
             raise _lib.WnbError("generation needs CUDA tensors: this build has no CPU fallback")
-        dev = h.device
-        B, T0 = x.shape
         n_list = [int(n) for n in n_samples_list]
-        max_n = max(n_list)
-        Q, A, Ap, R, S, ks, U = (self.n_quantize, self.n_aux, self.n_aux_pad, self.n_resch, self.n_skipch,
-                                 self.kernel_size, self.upsampling_factor)
-        P = max(T0, self.receptive_field)
-        n_pad = P - T0
-        xs = torch.full((B, P + max_n), Q // 2, dtype=torch.int32, device=dev)
-        xs[:, n_pad:P] = x.to(dev).to(torch.int32)
-        h = h.contiguous().float()
-        Th = h.size(2)
-        if Th * max(U, 1) < max_n + T0 - 1:
+        max_n, T0, Th = max(n_list), x.size(1), h.size(2)
+        if Th * max(self.upsampling_factor, 1) < max_n + T0 - 1:
             raise ValueError("aux features too short: %d frames for %d samples" % (Th, max_n + T0))
-        w = self._decode_pack()
-        dil = (ctypes.c_int32 * len(self.dilations))(*self.dilations)
-        L = len(self.dilations)
-        qbytes = lib.wnb_decode_bf16_workspace(B, R, ks, dil, L) if kernel == "bf16" else \
-            lib.wnb_decode_workspace(B, R, ks, dil, L)
-        queues = torch.empty(max(qbytes // 4, 1), dtype=torch.float32, device=dev)
-        nsm = torch.tensor(n_list, dtype=torch.int32, device=dev)
-        uni = None if uniforms is None else uniforms.to(dev).float().contiguous()
-        lg = torch.empty(B, max_n, Q, dtype=torch.float32, device=dev) if return_logits else None
-        if seed is None:
-            seed = int(torch.empty((), dtype=torch.int64).random_().item())  # follows torch.manual_seed
-        upw = self.upsampling.conv.weight.detach().float().contiguous().view(-1) if U > 0 else None
-        upb = self.upsampling.conv.bias.detach().float().contiguous().view(-1) if U > 0 else None
-        cmode = MODE_ARGMAX if mode == "argmax" else MODE_SAMPLING
-        cseed = ctypes.c_uint64(seed & 0xFFFFFFFFFFFFFFFF)
-        rc = -3
-        self.last_decode_kernel = None
-        if kernel == "bf16":
-            if not lib.wnb_decode_bf16_supported(Q, Ap, R, S, ks, L):
-                raise _lib.WnbError("decode_math='bf16' does not cover this model (n_quantize %d, n_aux %d, n_resch %d, "
-                                    "n_skipch %d, kernel_size %d, %d layers): see decode_bf16_supported()"
-                                    % (Q, A, R, S, ks, L))
-            wstream = self._decode_bf16_pack()
-            assert wstream.numel() == lib.wnb_decode_bf16_weights(Q, Ap, R, S, ks, L)
-            # the warm-up in parallel over time, then the decoder from P - 1
-            _bf16_prefill(lib, xs, P, h, upw, upb, w, wstream, dil, L, queues, n_pad, A, Ap, R, S, ks, U)
-            check(lib.wnb_decode_bf16_at(ptr(xs), ptr(h), ptr(upw), ptr(upb), ptr(w["wf"]), ptr(w["bf"]), ptr(wstream),
-                                         dil, L, ptr(queues), ptr(nsm), ptr(uni), ptr(lg), B, P, max_n, n_pad, Th, Q, A,
-                                         Ap, R, S, ks, U, cmode, cseed, P - 1, 0, 0, stream()), "decode_bf16")
-            self.last_decode_kernel = "bf16"
-            gen = xs[:, P:]
-            return (gen, lg) if return_logits else gen
-        if kernel in ("auto", "warp") and lib.wnb_decode_warp_supported(Q, Ap, R, S, ks, L):
-            Wc, CLc = lib.wnb_decode_warp_plan(B), lib.wnb_decode_warp_cluster(B)
-            wstream = self._decode_warp_pack(Wc, CLc)
-            assert wstream.numel() == lib.wnb_decode_warp_floats(L, CLc)
-            pos0 = 0
-            if lib.wnb_decode_warp_form(B, L, (ctypes.c_int32 * 4)()) == 0:   # the launch below will run: prefill first
-                _warp_prefill(lib, xs, P, h, upw, upb, w, dil, L, queues, n_pad, A, U, CLc)
-                pos0 = P - 1
-            rc = lib.wnb_decode_warp_at(ptr(xs), ptr(h), ptr(upw), ptr(upb), ptr(w["wf"]), ptr(w["bf"]), ptr(wstream),
-                                        ptr(w["b1"]), ptr(w["b2"]), ptr(w["bp1"]), ptr(w["bp2"]), dil, L, ptr(queues),
-                                        ptr(nsm), ptr(uni), ptr(lg), B, P, max_n, n_pad, Th, A, U, cmode, cseed, Wc,
-                                        CLc, pos0, 0, 0, stream())
-            if rc != -3 or kernel == "warp":
-                check(rc, "decode_warp")
-            if rc == 0:
-                self.last_decode_kernel = "warp"
-        elif kernel == "warp":
-            raise _lib.WnbError("decode kernel 'warp' does not cover this configuration")
-        if rc == -3 and kernel in ("auto", "stream"):
-            wstream = self._decode_stream_pack(w)
-            assert wstream.numel() == lib.wnb_decode_stream_floats(Q, Ap, R, S, ks, L)
-            rc = lib.wnb_decode_stream(ptr(xs), ptr(h), ptr(upw), ptr(upb), ptr(w["wf"]), ptr(w["bf"]), ptr(wstream),
-                                       ptr(w["b1"]), ptr(w["b2"]), ptr(w["bp1"]), ptr(w["bp2"]), dil, L, ptr(queues),
-                                       ptr(nsm), ptr(uni), ptr(lg), B, P, max_n, n_pad, Th, Q, A, Ap, R, S, ks, U,
-                                       cmode, cseed, stream())
-            if rc != -3 or kernel == "stream":
-                check(rc, "decode_stream")
-        if rc == -3:   # WNB_ERR_UNSUPPORTED: shape outside the streaming kernel -> direct-from-L2 kernel
-            check(lib.wnb_decode(ptr(xs), ptr(h), ptr(upw), ptr(upb), ptr(w["wf"]), ptr(w["bf"]), ptr(w["w1d"]),
-                                 ptr(w["b1"]), ptr(w["w2d"]), ptr(w["b2"]), ptr(w["wp1d"]), ptr(w["bp1"]),
-                                 ptr(w["wp2d"]), ptr(w["bp2"]), dil, L, ptr(queues), ptr(nsm), ptr(uni), ptr(lg),
-                                 B, P, max_n, n_pad, Th, Q, A, Ap, R, S, ks, U, cmode, cseed, stream()), "decode")
-        if self.last_decode_kernel is None:
-            self.last_decode_kernel = "stream" if rc == 0 else "direct"
-        gen = xs[:, P:]
-        if return_logits:
-            return gen, lg
-        return gen
+        if max_n < 1:
+            raise _lib.WnbError("decode: every requested length is 0")
+        with torch.no_grad():
+            s = DecodeSession(self, x.to(h.device), n_list, mode, seed, uniforms, return_logits, kernel)
+            out = s.step(h)
+        self.last_decode_kernel = s.kernel
+        return out
 
     def fast_generate(self, x, h, n_samples, intervals=None, mode="sampling"):
         """GENERATE WAVEFORM WITH FAST ALGORITHM (reference wavenet.py:309-395).

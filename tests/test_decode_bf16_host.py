@@ -30,8 +30,8 @@ def test_supported_and_sizes():
     dil = (ctypes.c_int32 * 4)(1, 2, 4, 8)
     assert lib.wnb_decode_bf16_workspace(64, 512, 3, dil, 4) == 1 * 2 * 15 * 512 * 64 * 2
     assert lib.wnb_decode_bf16_workspace(65, 512, 2, dil, 4) == 2 * 15 * 512 * 64 * 2
-    rc = lib.wnb_decode_bf16(None, None, None, None, None, None, None, dil, 4, None, None, None, None, 2, 1, 5, 0, 10,
-                             256, 28, 32, 512, 256, 2, 0, 0, 0, None)
+    rc = lib.wnb_decode_bf16_at(None, None, None, None, None, None, None, dil, 4, None, None, None, None, 2, 1, 5, 0, 10,
+                                256, 28, 32, 512, 256, 2, 0, 0, 0, 0, 0, 0, None)
     assert rc == -1 and b"null pointer" in lib.wnb_last_error()
 
 

@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""GPU tier: resumable decode sessions (``WaveNet.decode_session``, the ``wnb_decode*_at`` entry points).
+"""GPU tier: resumable decode sessions (``WaveNet.decode_session``, the ``_at`` decode entry points).
 
 Chunked decoding must equal one-shot decoding BIT FOR BIT -- the codes and the teacher-check logits -- in argmax mode,
 with supplied uniforms and with in-kernel Philox, on every launch form:
@@ -10,6 +10,7 @@ with supplied uniforms and with in-kernel Philox, on every launch form:
   than the receptive field) a first chunk inside the warm-up; ragged lengths finish in different chunks;
 * 10 000 Philox steps at the bench shape in 80-sample chunks;
 * two sessions interleaved on one model, and on two streams, equal each run alone;
+* the library launches of one one-shot decode (a one-call session) on each kernel, the count bench.py reports;
 * every error case, and ``bin/decode.py --chunk_frames 7`` writing the same wav bytes as the one-shot run."""
 import argparse
 import ctypes
@@ -199,6 +200,34 @@ def test_long_philox_run_in_80_sample_chunks():
     for b in range(B):
         assert np.array_equal(codes[b], gen[b, :n_list[b]]), b
         assert np.array_equal(logits[b].view(np.uint32), lg[b, :n_list[b]].view(np.uint32)), b
+
+
+# library launches of one _decode call: the decode launch, after the parallel warm-up on warp (the front conv and one
+# launch per layer but the last: L = 30 here) and on bf16 (the front conv, then a gate and a res launch per layer but the
+# last: L = 8 here).  bench.py reports this count as gpu_launches.
+LAUNCHES = {
+    "warp_cl2": (WARP_FORMS["1x16_big_cl2"], "auto", "warp", 31),
+    "warp_cl1": (WARP_FORMS["1x16_big_cl1"], "auto", "warp", 31),
+    "stream": ((SHALLOW, lambda n: 5, None, None), "stream", "stream", 1),
+    "direct": ((SHALLOW, lambda n: 5, None, None), "direct", "direct", 1),
+    "bf16": (((256, 28, 256, 256, 4, 2, 2, 4), lambda n: 3, None, None), "auto", "bf16", 16),
+}
+
+
+@pytest.mark.parametrize("case", list(LAUNCHES))
+def test_oneshot_launch_count(case):
+    from pytorchwavenetvocoder_b200 import _lib
+    (t, bfn, _, form), kernel, ran, want = LAUNCHES[case]
+    cfg, net = _model(t, "bf16" if ran == "bf16" else "fp32")
+    B = bfn(_nsm())
+    if form is not None:
+        assert _warp_form(B, len(cfg.dilations)) == form
+    x, h, n_list = _inputs(cfg, B, 1, 8, 900)
+    l0 = _lib.launch_count()
+    net._decode(x, h, n_list, "sampling", seed=3, kernel=kernel)
+    launches = _lib.launch_count() - l0
+    assert net.last_decode_kernel == ran
+    assert launches == want, (case, launches)
 
 
 def test_sessions_are_isolated():
