@@ -408,6 +408,37 @@ WNB_API int wnb_decode_bf16_prefill(const int32_t* xs, const float* h, const flo
                                     int n_pad, int Th, int A, int Ap, int R, int S, int ks, int U,
                                     void* stream_handle);
 
+/* ---- continuous batching on the bf16 decoder (csrc/decode_bf16_pool.cu, nets/wavenet.py::DecodePool) ----------------
+ * A pool of `capacity` rows runs wnb_decode_bf16_at unchanged on B = capacity with P = 1, n_pad = 0, U = 0, a global
+ * step counter g as the window (pos0 = g0 >= ks - 1, xs_base = g0 - (ks - 1), h_frame0 = g0, Th = max_n = n) and its
+ * queues allocated zeroed (pos0 is never 0, so the launcher never clears them).  Every row then reads queue slot
+ * g mod (ks-1) d_l, xs column g, aux column g and uniform column g, and the two calls below fill those with what one-shot
+ * decoding gives the stream in that row, so each stream's codes equal one-shot decoding bit for bit.
+ *
+ * wnb_decode_bf16_pool_transplant moves n admitted streams into the pool: row src_rows[i] of `src_queues` (a workspace
+ * of wnb_decode_bf16_at for src_B utterances, after wnb_decode_bf16_prefill) goes to row dst_slots[i] of `dst_queues`
+ * (the pool's workspace, B = capacity), layer l's slot s to slot (s + rotations[i]) mod (ks-1) d_l, with
+ * rotations[i] = g_a - (P - 1) for a stream whose first sample is the pool's step g_a.  Every slot of the row is written.
+ *   src_rows, dst_slots, rotations   host int32 arrays of n (1 <= n <= 64); the slots must be distinct.
+ * WNB_ERR_INVALID for a bad shape, row, slot, dilation or pointer, before any device work.
+ *
+ * wnb_decode_bf16_pool_inputs writes the call's aux window and uniforms for wnb_decode_bf16_at:
+ *   frames   (B, A, F) fp32, each row's aux frames as given (before up-sampling when U > 0);
+ *   table    (5, B) int32 device, per row: [0] the absolute frame of frames[b][.][0], [1] the aux column of the row's
+ *            first step, [2] its first sample index, [3] its stream id (the Philox counter's second word), [4] its samples
+ *            in this call (0: an idle row), which is also the n_samples of wnb_decode_bf16_at;
+ *   aux      (B, A, n) out: column k of row b = fmaf(frames[b][a][j / U - [0]], up_w[j % U], up_b[0]) with j = [1] + k
+ *            (frames[b][a][j - [0]] when U = 0), the fp32 value the decoder computes in-kernel; 0 for k >= [4];
+ *   uniforms (B, n) out, or NULL (argmax): column k = (r0 >> 8) * 2^-24 of Philox4x32-10((sample [2] + k, stream id [3],
+ *            0, 0), seed), the decoder's own draw; 0 for k >= [4].
+ * WNB_ERR_INVALID for a bad shape or pointer, before any device work. */
+WNB_API int wnb_decode_bf16_pool_transplant(const void* src_queues, int src_B, const int32_t* src_rows, void* dst_queues,
+                                            int capacity, const int32_t* dst_slots, const int32_t* rotations, int n,
+                                            int R, int ks, const int32_t* host_dilations, int L, void* stream_handle);
+WNB_API int wnb_decode_bf16_pool_inputs(const float* frames, const float* up_w, const float* up_b, const int32_t* table,
+                                        float* aux, float* uniforms, int B, int A, int F, int n, int U, uint64_t seed,
+                                        void* stream_handle);
+
 #ifdef __cplusplus
 }
 #endif

@@ -17,6 +17,7 @@ model with CPU tensors raises.
 import collections
 import ctypes
 import logging
+import math
 import sys
 import time
 
@@ -29,7 +30,8 @@ from .. import _lib
 from .._lib import MATH_BF16, MATH_FP32, MATH_TF32, MODE_ARGMAX, MODE_SAMPLING, check, ptr, stream
 
 __all__ = ["encode_mu_law", "decode_mu_law", "initialize", "OneHot", "CausalConv1d", "UpSampling",
-           "WaveNet", "cross_entropy", "mulaw_pcm16_table", "codes_to_pcm16", "DecodeSession", "decode_window"]
+           "WaveNet", "cross_entropy", "mulaw_pcm16_table", "codes_to_pcm16", "DecodeSession", "DecodePool",
+           "decode_window"]
 
 # bench.py sets this to a list to get (start, end) CUDA-event pairs around every fused-block launch
 PROFILE_EVENTS = None
@@ -638,6 +640,31 @@ def _warp_prefill(lib, xs, P, h, upw, upb, w, dil, L, queues, n_pad, A, U, CL):
           "decode_warp_prefill")
 
 
+def _decode_snapshot(net):
+    """The decode weights a session or pool keeps for its whole life: ``_decode_pack()`` and the up-sampling weight and
+    bias (None without an up-sampling layer).  Copies: ``_decode_pack()`` hands some entries (the front and post biases)
+    out as the parameters themselves, and an in-place update of the model (load_state_dict, an optimizer step) must not
+    reach a running decode."""
+    params = {p.untyped_storage().data_ptr() for p in net.parameters()}
+    w = {k: v.clone() if v.untyped_storage().data_ptr() in params else v for k, v in net._decode_pack().items()}
+    U = net.upsampling_factor
+    upw = net.upsampling.conv.weight.detach().float().contiguous().view(-1).clone() if U > 0 else None
+    upb = net.upsampling.conv.bias.detach().float().contiguous().view(-1).clone() if U > 0 else None
+    return w, upw, upb
+
+
+def _bf16_weight_stream(lib, net):
+    """The packed weight stream of the bf16 decoder (``_decode_bf16_pack``); raises for a shape it does not cover."""
+    Q, A, Ap, R, S, ks, L = (net.n_quantize, net.n_aux, net.n_aux_pad, net.n_resch, net.n_skipch, net.kernel_size,
+                             len(net.dilations))
+    if not lib.wnb_decode_bf16_supported(Q, Ap, R, S, ks, L):
+        raise _lib.WnbError("decode_math='bf16' does not cover this model (n_quantize %d, n_aux %d, n_resch %d, "
+                            "n_skipch %d, kernel_size %d, %d layers): see decode_bf16_supported()" % (Q, A, R, S, ks, L))
+    wstream = net._decode_bf16_pack()
+    assert wstream.numel() == lib.wnb_decode_bf16_weights(Q, Ap, R, S, ks, L)
+    return wstream
+
+
 def _bf16_prefill(lib, xs, P, h, upw, upb, w, wstream, dil, L, queues, n_pad, A, Ap, R, S, ks, U):
     """Run the warm-up positions 0 .. P - 2 of the bf16 decoder in parallel over time (wnb_decode_bf16_prefill): the
     queues then hold what the sequential warm-up leaves there, and ``wnb_decode_bf16_at`` continues from P - 1."""
@@ -698,18 +725,9 @@ class DecodeSession(object):
         self.L = L
         self.dil = (ctypes.c_int32 * L)(*net.dilations)
         self.mode = MODE_ARGMAX if mode == "argmax" else MODE_SAMPLING
-        # a snapshot: _decode_pack() hands some entries (the front and post biases) out as the parameters themselves, and
-        # an in-place update of the model (load_state_dict, an optimizer step) must not reach a running session
-        params = {p.untyped_storage().data_ptr() for p in net.parameters()}
-        self.w = {k: v.clone() if v.untyped_storage().data_ptr() in params else v
-                  for k, v in net._decode_pack().items()}
+        self.w, self.upw, self.upb = _decode_snapshot(net)
         if kernel == "bf16":
-            if not lib.wnb_decode_bf16_supported(Q, Ap, R, S, ks, L):
-                raise _lib.WnbError("decode_math='bf16' does not cover this model (n_quantize %d, n_aux %d, n_resch %d, "
-                                    "n_skipch %d, kernel_size %d, %d layers): see decode_bf16_supported()"
-                                    % (Q, self.A, R, S, ks, L))
-            self.wstream = net._decode_bf16_pack()
-            assert self.wstream.numel() == lib.wnb_decode_bf16_weights(Q, Ap, R, S, ks, L)
+            self.wstream = _bf16_weight_stream(lib, net)
             qbytes = lib.wnb_decode_bf16_workspace(B, R, ks, self.dil, L)
         else:
             if kernel in ("auto", "warp"):
@@ -730,8 +748,6 @@ class DecodeSession(object):
             qbytes = lib.wnb_decode_workspace(B, R, ks, self.dil, L)
         self.kernel = kernel
         self.queues = torch.empty(max(qbytes // 4, 1), dtype=torch.float32, device=dev)
-        self.upw = net.upsampling.conv.weight.detach().float().contiguous().view(-1).clone() if U > 0 else None
-        self.upb = net.upsampling.conv.bias.detach().float().contiguous().view(-1).clone() if U > 0 else None
         if seed is None:
             seed = int(torch.empty((), dtype=torch.int64).random_().item())  # follows torch.manual_seed, like _decode
         self.seed = ctypes.c_uint64(seed & 0xFFFFFFFFFFFFFFFF)
@@ -839,6 +855,313 @@ class DecodeSession(object):
         check(_lib.load().wnb_lut_i16(ptr(codes), ptr(self._pcm_tab), ptr(out), codes.numel(), self.Q, stream()),
               "lut_i16")
         return out
+
+
+# A decode pool's global step counter g is a decoder position: it stays at or below this (the last position of a call,
+# g0 + n).  Before a call would pass it, g drops by a multiple of every queue length, which leaves every slot in place.
+POOL_COUNTER_LIMIT = MAX_DECODE_POSITION
+# steps of one pool call at most: the call's aux window is staged at sample rate, (capacity, n_aux, n) fp32
+POOL_MAX_STEPS = 8192
+# streams one admission prefill takes at most: one cluster of the bf16 decoder
+POOL_ADMIT_ROWS = 64
+
+PoolCall = collections.namedtuple("PoolCall", "g0 n admit rows finished")
+
+
+class PoolStream(object):
+    """One stream of a decode pool: seed length T0 (P = max(T0, rf), n_pad = P - T0), length, aux frames received,
+    samples decoded and the pool slot it occupies (None while it waits)."""
+
+    def __init__(self, sid, T0, total, rf):
+        self.sid, self.T0, self.total = sid, T0, total
+        self.P = max(T0, rf)
+        self.n_pad = self.P - T0
+        self.frames, self.done, self.slot = 0, 0, None
+
+    def runnable(self, U, ks):
+        """Samples after the decoded ones whose aux has arrived (``decode_window``'s rule)."""
+        win = decode_window(self.P - 1 + self.done, self.frames, self.P, self.n_pad, U, ks, [self.total])
+        return win.n if win is not None else 0
+
+    def aux_column(self, i):
+        """The aux column (sample rate) of sample i: position P - 1 + i less the n_pad replicated columns."""
+        return self.T0 - 1 + i
+
+
+class PoolSchedule(object):
+    """The host arithmetic of a ``DecodePool``, with no device work: which streams enter which slots, how many steps a
+    call runs and which samples every row makes.  ``next_call`` applies the rules of ``DecodePool.step`` and returns a
+    ``PoolCall``, or None when no stream can run:
+      * ``g0``, ``n``: the call runs the pool's steps g0 .. g0 + n - 1;
+      * ``admit``: groups ``(T0, [stream, ...])`` of at most POOL_ADMIT_ROWS streams with one seed length, each one
+        prefill; a stream's queue slots rotate by ``g0 - (P - 1)`` (its first sample is step g0);
+      * ``rows``: ``(slot, stream, i0, count)`` for every occupied slot: samples i0 .. i0 + count - 1;
+      * ``finished``: the ids of the streams this call completes (their slots are free for the next call)."""
+
+    def __init__(self, capacity, receptive_field, dilations, ks, U):
+        self.capacity, self.rf, self.ks, self.U = capacity, receptive_field, ks, U
+        self.period = 1                      # lcm of the queue lengths (ks - 1) d_l
+        for d in dilations:
+            q = (ks - 1) * d
+            self.period = self.period * q // math.gcd(self.period, q)
+        self.g = ks - 1                      # the front gather reads g - (ks - 1) .. g: never a position below 0
+        self.slots = [None] * capacity
+        self.waiting = []                    # FIFO
+        self.streams = {}                    # id -> PoolStream, until it finishes
+        self.finished = set()
+
+    def add(self, sid, T0, total):
+        st = PoolStream(sid, T0, total, self.rf)
+        self.streams[sid] = st
+        self.waiting.append(st)
+        return st
+
+    def next_call(self, max_samples=None):
+        U, ks = self.U, self.ks
+        free = [s for s, st in enumerate(self.slots) if st is None]
+        ready = [st for st in self.waiting if st.runnable(U, ks) > 0][:len(free)]
+        active = [st for st in self.slots if st is not None] + ready
+        if not active:
+            return None
+        # one launch for every row: a stream whose aux is still incomplete bounds the call by what it can run
+        n = max(st.total - st.done for st in active)
+        for st in active:
+            r = st.runnable(U, ks)
+            if r < st.total - st.done:
+                n = min(n, r)
+        n = min(n, POOL_MAX_STEPS if max_samples is None else min(max_samples, POOL_MAX_STEPS))
+        if n <= 0:
+            return None
+        if self.g + n > POOL_COUNTER_LIMIT:
+            self.g = ks - 1 + (self.g - (ks - 1)) % self.period
+            if self.g >= POOL_COUNTER_LIMIT:
+                raise ValueError("POOL_COUNTER_LIMIT %d leaves no step after a rebase to %d"
+                                 % (POOL_COUNTER_LIMIT, self.g))
+            n = min(n, POOL_COUNTER_LIMIT - self.g)
+        groups = collections.OrderedDict()
+        for st, s in zip(ready, free):
+            self.waiting.remove(st)
+            st.slot, self.slots[s] = s, st
+            groups.setdefault(st.T0, []).append(st)
+        admit = [(T0, sts[k:k + POOL_ADMIT_ROWS]) for T0, sts in groups.items()
+                 for k in range(0, len(sts), POOL_ADMIT_ROWS)]
+        rows, finished = [], []
+        for s, st in enumerate(self.slots):
+            if st is None:
+                continue
+            c = min(st.total - st.done, n)
+            rows.append((s, st, st.done, c))
+            st.done += c
+            if st.done == st.total:
+                finished.append(st.sid)
+                self.slots[s] = None          # (st.slot keeps the row: this call's admission still needs it)
+                del self.streams[st.sid]
+                self.finished.add(st.sid)
+        g0 = self.g
+        self.g += n
+        return PoolCall(g0, n, admit, rows, finished)
+
+
+def _pinned_int32(values, dev):
+    """A host list as an int32 device tensor, copied without synchronising the host (pinned staging)."""
+    return torch.tensor(values, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
+
+
+class DecodePool(object):
+    """Continuous batching on the bf16 decoder (``WaveNet.decode_pool``): streams join a free row of a running batch and
+    leave it the moment they finish, so requests that arrive at different times share one cluster's weight read.
+
+    The pool is one ``wnb_decode_bf16_at`` batch of ``capacity`` rows, launched once per ``step`` over the pool's global
+    steps g0 .. g0 + n - 1 with P = 1, n_pad = 0, U = 0 (include/wnb200.h, DESIGN §3.7).  A stream's warm-up runs as the
+    usual parallel prefill when it is admitted, and its queues are moved into its row, rotated so that its first sample
+    is the pool's step of admission; each call's aux window and uniforms are written per row for the row's own stream
+    (``wnb_decode_bf16_pool_inputs``).  Stream k of a pool with seed S decodes exactly what row k of
+    ``net._decode(X, H, n_list, mode, seed=S, kernel="bf16")`` decodes, bit for bit.
+
+    ``step`` runs one launch for every row, so it advances in lock step: a stream whose aux frames have not arrived
+    holds back the whole launch (the call runs only what that stream can run, and nothing if it can run nothing).  The
+    bf16 decoder is much slower than real time (about 1.6 k samples/s per stream at arctic 512/256), so an acoustic model
+    feeding it stays ahead.  The pool snapshots the weights at its creation."""
+
+    def __init__(self, net, capacity=64, mode="sampling", seed=None):
+        if mode not in ("sampling", "argmax"):
+            raise ValueError("mode should be sampling or argmax, got %r" % (mode,))
+        capacity = int(capacity)
+        if capacity < 1:
+            raise ValueError("a decode pool needs a capacity of at least 1, got %d" % capacity)
+        if getattr(net, "decode_math", "fp32") != "bf16":
+            raise _lib.WnbError("decode pools run the bf16 decoder: set decode_math='bf16' (got %r)"
+                                % (getattr(net, "decode_math", "fp32"),))
+        lib = _lib.load()
+        self.device = dev = _device()
+        self.Q, self.A, self.Ap, self.R, self.S, self.ks, self.U = (
+            net.n_quantize, net.n_aux, net.n_aux_pad, net.n_resch, net.n_skipch, net.kernel_size, net.upsampling_factor)
+        self.rf, self.L, self.capacity = net.receptive_field, len(net.dilations), capacity
+        self.dil = (ctypes.c_int32 * self.L)(*net.dilations)
+        self.wstream = _bf16_weight_stream(lib, net)
+        self.w, self.upw, self.upb = _decode_snapshot(net)
+        self.mode = MODE_ARGMAX if mode == "argmax" else MODE_SAMPLING
+        if seed is None:
+            seed = int(torch.empty((), dtype=torch.int64).random_().item())  # follows torch.manual_seed, like _decode
+        self.seed = ctypes.c_uint64(seed & 0xFFFFFFFFFFFFFFFF)
+        # zeroed once: the decoder is never launched with pos0 = 0 here, so it never clears them
+        self.queues = torch.zeros(lib.wnb_decode_bf16_workspace(capacity, self.R, self.ks, self.dil, self.L),
+                                  dtype=torch.uint8, device=dev)
+        self._admit_queues = torch.empty(lib.wnb_decode_bf16_workspace(POOL_ADMIT_ROWS, self.R, self.ks, self.dil,
+                                                                       self.L), dtype=torch.uint8, device=dev)
+        self._tail = torch.full((capacity, self.ks), self.Q // 2, dtype=torch.int32, device=dev)   # xs at g - ks + 1 .. g
+        self._sched = PoolSchedule(capacity, self.rf, net.dilations, self.ks, self.U)
+        self._x = {}        # id -> seed codes, until admitted
+        self._h = {}        # id -> [aux frames (A, F) on the device, absolute frame of column 0]
+        self._admitted = 0
+        self._pcm_tab = None
+
+    @property
+    def active(self):
+        """Ids of the streams in the pool's rows, by row."""
+        return [st.sid for st in self._sched.slots if st is not None]
+
+    @property
+    def waiting(self):
+        """Ids of the admitted streams that wait for a row (or for the aux frames of their first sample), in order."""
+        return [st.sid for st in self._sched.waiting]
+
+    def finished(self, stream):
+        """True once every sample of ``stream`` has been returned by ``step``."""
+        if stream in self._sched.finished:
+            return True
+        if stream not in self._sched.streams:
+            raise KeyError("decode pool: unknown stream %r" % (stream,))
+        return False
+
+    def admit(self, x, n_samples, h=None, stream=None):
+        """Queue a stream with seed codes ``x`` (1-D, on the GPU) and ``n_samples`` samples to decode, optionally with
+        its first aux frames ``h`` (n_aux, F).  Returns its id: ``stream``, or by default the number of streams admitted
+        before it.  The id is the stream's Philox counter word, as the batch index is in one-shot decoding."""
+        if not x.is_cuda or (h is not None and not h.is_cuda):
+            raise _lib.WnbError("decode pools need CUDA tensors: this build has no CPU fallback")
+        if x.dim() != 1 or x.numel() < 1:
+            raise ValueError("seed codes should be a non-empty 1-D tensor, got shape %s" % (tuple(x.shape),))
+        sid = self._admitted if stream is None else stream
+        if not isinstance(sid, int) or not 0 <= sid < 2 ** 31:
+            raise ValueError("stream ids are ints in [0, 2^31), got %r" % (sid,))
+        if sid in self._sched.streams or sid in self._sched.finished:
+            raise ValueError("decode pool: stream %d exists already" % sid)
+        n_samples = int(n_samples)
+        P = max(x.numel(), self.rf)
+        if n_samples < 1 or P - 1 + n_samples > MAX_DECODE_POSITION:
+            raise ValueError("a stream decodes 1 .. %d samples, got %d" % (MAX_DECODE_POSITION - (P - 1), n_samples))
+        self._admitted += 1
+        self._sched.add(sid, x.numel(), n_samples)
+        self._x[sid] = x.to(torch.int32)
+        self._h[sid] = [torch.empty(self.A, 0, dtype=torch.float32, device=self.device), 0]
+        if h is not None:
+            self.feed(sid, h)
+        return sid
+
+    def feed(self, stream, h_chunk):
+        """Append aux frames ``h_chunk`` (n_aux, F) to ``stream`` (sample-rate columns when the model has no
+        up-sampling layer)."""
+        st = self._sched.streams.get(stream)
+        if st is None:
+            raise KeyError("decode pool: unknown or finished stream %r" % (stream,))
+        if not h_chunk.is_cuda:
+            raise _lib.WnbError("decode pools need CUDA tensors: this build has no CPU fallback")
+        if h_chunk.dim() != 2 or h_chunk.size(0) != self.A:
+            raise ValueError("aux chunk should be (%d, frames), got %s" % (self.A, tuple(h_chunk.shape)))
+        buf = self._h[stream]
+        buf[0] = torch.cat([buf[0], h_chunk.to(self.device).float()], 1)
+        st.frames += h_chunk.size(1)
+
+    def step(self, max_samples=None):
+        """Admit the waiting streams whose first aux frames have arrived and run one launch of at most ``max_samples``
+        steps.  Returns ``{stream: new codes}`` (int32 device tensors, without synchronising) for every stream in a row;
+        ``{}`` and no launch when no stream can run."""
+        call, gen = self._call(max_samples)
+        return {} if call is None else {st.sid: gen[slot, :c] for slot, st, _, c in call.rows}
+
+    def step_pcm16(self, max_samples=None):
+        """``step`` with the new samples as PCM_16 (one ``wnb_lut_i16`` gather for the whole call): int16 device
+        tensors, without synchronising after the first call."""
+        call, gen = self._call(max_samples)
+        if call is None:
+            return {}
+        if self._pcm_tab is None:
+            self._pcm_tab = torch.from_numpy(mulaw_pcm16_table(self.Q)).to(self.device)
+        codes = gen.contiguous()
+        out = torch.empty(codes.shape, dtype=torch.int16, device=self.device)
+        check(_lib.load().wnb_lut_i16(ptr(codes), ptr(self._pcm_tab), ptr(out), codes.numel(), self.Q, stream()),
+              "lut_i16")
+        return {st.sid: out[slot, :c] for slot, st, _, c in call.rows}
+
+    def _admit_group(self, lib, T0, group, g0):
+        """Prefill a group of streams with one seed length and move their queues into their rows."""
+        P = max(T0, self.rf)
+        n_pad, Bg, ks = P - T0, len(group), self.ks
+        xs = torch.full((Bg, P), self.Q // 2, dtype=torch.int32, device=self.device)
+        xs[:, n_pad:] = torch.stack([self._x.pop(st.sid) for st in group])
+        Fg = min(self._h[st.sid][0].size(1) for st in group)
+        h = torch.stack([self._h[st.sid][0][:, :Fg] for st in group]).contiguous()
+        _bf16_prefill(lib, xs, P, h, self.upw, self.upb, self.w, self.wstream, self.dil, self.L, self._admit_queues,
+                      n_pad, self.A, self.Ap, self.R, self.S, ks, self.U)
+        check(lib.wnb_decode_bf16_pool_transplant(ptr(self._admit_queues), Bg, (ctypes.c_int32 * Bg)(*range(Bg)),
+                                                  ptr(self.queues), self.capacity,
+                                                  (ctypes.c_int32 * Bg)(*[st.slot for st in group]),
+                                                  (ctypes.c_int32 * Bg)(*[g0 - (P - 1)] * Bg), Bg, self.R, ks, self.dil,
+                                                  self.L, stream()),
+              "decode_bf16_pool_transplant")
+        for k, st in enumerate(group):
+            self._tail[st.slot] = xs[k, P - ks:]
+
+    def _call(self, max_samples):
+        """One pool call: (PoolCall, (capacity, n) int32 codes of steps g0 .. g0 + n - 1), or (None, None)."""
+        if max_samples is not None and int(max_samples) < 1:
+            raise ValueError("max_samples should be at least 1, got %r" % (max_samples,))
+        call = self._sched.next_call(max_samples)
+        if call is None:
+            return None, None
+        lib = _lib.load()
+        C, A, ks, Uc, n = self.capacity, self.A, self.ks, max(self.U, 1), call.n
+        for T0, group in call.admit:
+            self._admit_group(lib, T0, group, call.g0)
+        # each row's frames from the one of its first step, and the table of wnb_decode_bf16_pool_inputs
+        table = [[0] * C for _ in range(5)]
+        spans = []
+        for slot, st, i0, c in call.rows:
+            j0 = st.aux_column(i0)
+            f0, f1 = j0 // Uc, (j0 + c - 1) // Uc + 1
+            spans.append((slot, st, f0, f1))
+            for r, v in enumerate((f0, j0, i0, st.sid, c)):
+                table[r][slot] = v
+        frames = torch.empty(C, A, max(f1 - f0 for _, _, f0, f1 in spans), dtype=torch.float32, device=self.device)
+        for slot, st, f0, f1 in spans:
+            buf, h0 = self._h[st.sid]
+            frames[slot, :, :f1 - f0] = buf[:, f0 - h0:f1 - h0]
+        tab = _pinned_int32(table, self.device)
+        aux = torch.empty(C, A, n, dtype=torch.float32, device=self.device)
+        uni = torch.empty(C, n, dtype=torch.float32, device=self.device) if self.mode == MODE_SAMPLING else None
+        st_ = stream()
+        check(lib.wnb_decode_bf16_pool_inputs(ptr(frames), ptr(self.upw), ptr(self.upb), ptr(tab), ptr(aux), ptr(uni), C,
+                                              A, frames.size(2), n, self.U, self.seed, st_),
+              "decode_bf16_pool_inputs")
+        xs = torch.empty(C, ks + n, dtype=torch.int32, device=self.device)
+        xs[:, :ks] = self._tail
+        w, g0 = self.w, call.g0
+        check(lib.wnb_decode_bf16_at(ptr(xs), ptr(aux), None, None, ptr(w["wf"]), ptr(w["bf"]), ptr(self.wstream),
+                                     self.dil, self.L, ptr(self.queues), ptr(tab[4]), ptr(uni), None, C, 1, n, 0, n,
+                                     self.Q, A, self.Ap, self.R, self.S, ks, 0, self.mode, self.seed, g0, g0 - (ks - 1),
+                                     g0, st_),
+              "decode_bf16_at")
+        self._tail = xs[:, n:].contiguous()
+        # frames before each stream's next sample are no longer needed
+        for slot, st, f0, f1 in spans:
+            if st.sid in call.finished:
+                del self._h[st.sid]
+            else:
+                buf = self._h[st.sid]
+                f = st.aux_column(st.done) // Uc
+                buf[0], buf[1] = buf[0][:, f - buf[1]:], f
+        return call, xs[:, ks:]
 
 
 class WaveNet(nn.Module):
@@ -1219,3 +1542,12 @@ class WaveNet(nn.Module):
             n_samples_list = [MAX_DECODE_POSITION - (P - 1)] * x.size(0)
         with torch.no_grad():
             return DecodeSession(self, x, n_samples_list, mode, seed)
+
+    def decode_pool(self, capacity=64, mode="sampling", seed=None):
+        """Start a continuous-batching decode pool of ``capacity`` rows on the bf16 decoder (``decode_math="bf16"``):
+        ``admit`` streams at any time, ``feed`` their aux frames and ``step`` to decode; a stream takes a free row as
+        soon as its first frames arrive and leaves it when it finishes.  Stream k of a pool with ``seed`` S decodes
+        what row k of a one-shot bf16 decode with seed S decodes, bit for bit (``DecodePool``).  The pool snapshots the
+        weights now; ``seed`` is drawn from torch's generator when not given."""
+        with torch.no_grad():
+            return DecodePool(self, capacity, mode, seed)
