@@ -58,7 +58,8 @@ unsigned int* sched_counters(cudaStream_t st);
 // pointer handed out earlier remains valid).  Used for the per-CTA partial sums that make the gradient reductions independent of scheduling,
 // and for the bf16 copies of the weights a WNB_MATH_BF16 call multiplies with.
 void* scratch_buffer(cudaStream_t st, int slot, size_t bytes);
-enum { SCRATCH_WGRAD = 0, SCRATCH_EMBED = 1, SCRATCH_AUX = 2, SCRATCH_LOSS = 3, SCRATCH_EMBED_PART = 4, SCRATCH_BF16 = 5 };
+enum { SCRATCH_WGRAD = 0, SCRATCH_EMBED = 1, SCRATCH_AUX = 2, SCRATCH_LOSS = 3, SCRATCH_EMBED_PART = 4, SCRATCH_BF16 = 5,
+       SCRATCH_SIMT = 6 };
 
 #define WNB_REQUIRE(cond, ...)            \
   do {                                    \

@@ -7,8 +7,10 @@
 //                              writes z and dpre = [dz*th*sg*(1-sg) | dz*sg*(1-th^2)].
 //   gemm_nt_kernel           : C[t][m] = sum_seg sum_k A_seg[m][k] * B_seg[t+shift][k] (+bias, +add, relu,
 //                              mask, accumulate): used for the data gradients and the post network.
-//   gemm_tn_kernel           : weight gradients  dW[m][n] += sum_t A[t][m] * B[t+shift][n]  (split over time,
-//                              fp32 atomics), colsum_kernel: bias gradients.
+//   gemm_tn_kernel           : weight gradients  dW[m][n] += sum_t A[t][m] * B[t+shift][n], split over (batch, time
+//                              range); colsum_kernel: bias gradients, split over row ranges.  Each CTA writes its
+//                              partial sum to its own slot of a per-stream scratch and slot_reduce_kernel adds the
+//                              slots in slot order (no atomics: the gradients do not depend on scheduling).
 //
 // All activations are channels-last (B,T,C).  Everything here is fp32 FFMA: this is the parity path and
 // the fallback for shapes the tensor-core paths do not cover.
@@ -275,6 +277,7 @@ struct TnParams {
   const float* b; int ldb; int N; int shift; int relu_b;
   float* c; int ldc; int coff;
   int T, B, tchunk;
+  float* part;   // (B * nsplit, M, N) slot per (batch, time range), set by launch_tn; null: one slot, += straight into c
 };
 
 __global__ void __launch_bounds__(kThreads) gemm_tn_kernel(TnParams p) {
@@ -296,6 +299,7 @@ __global__ void __launch_bounds__(kThreads) gemm_tn_kernel(TnParams p) {
     return p.relu_b ? fmaxf(v, 0.f) : v;
   };
   tile_mainloop<8, false, false>(acc, fa, fb, tlen, sm);
+  float* slot = p.part ? p.part + (size_t)blockIdx.z * p.M * p.N : nullptr;
 #pragma unroll
   for (int i = 0; i < 8; i++) {
     const int m = m0 + ty * 8 + i;
@@ -303,20 +307,36 @@ __global__ void __launch_bounds__(kThreads) gemm_tn_kernel(TnParams p) {
 #pragma unroll
     for (int j = 0; j < kTN; j++) {
       const int n = n0 + tx * 4 + j;
-      if (n < p.N) atomicAdd(p.c + (size_t)m * p.ldc + p.coff + n, acc[i][j]);
+      if (n >= p.N) continue;
+      if (slot) slot[(size_t)m * p.N + n] = acc[i][j];
+      else p.c[(size_t)m * p.ldc + p.coff + n] += acc[i][j];
     }
   }
 }
 
-// out[m] += sum over rows of a[row][m]  (rows = B*T)
+// sum over rows of a[row][m] (rows = B*T) in ranges of rows_per_block: block i writes part[i][m], or adds into out[m]
+// when part is null (a single block)
 __global__ void colsum_kernel(const float* __restrict__ a, int lda, int M, int64_t rows, int rows_per_block,
-                              float* __restrict__ out) {
+                              float* __restrict__ part, float* __restrict__ out) {
   const int64_t r0 = (int64_t)blockIdx.x * rows_per_block;
   const int64_t r1 = min(r0 + rows_per_block, rows);
   for (int m = threadIdx.x; m < M; m += blockDim.x) {
     float s = 0.f;
     for (int64_t r = r0; r < r1; r++) s += a[r * lda + m];
-    atomicAdd(out + m, s);
+    if (part) part[(size_t)blockIdx.x * M + m] = s;
+    else out[m] += s;
+  }
+}
+
+// c[m][coff + n] += part[0][m][n] + part[1][m][n] + ... + part[nslots-1][m][n], added in slot order
+__global__ void slot_reduce_kernel(const float* __restrict__ part, int nslots, int M, int N, float* __restrict__ c, int ldc,
+                                   int coff) {
+  const int64_t mn = (int64_t)M * N;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < mn; i += (int64_t)gridDim.x * blockDim.x) {
+    float s = 0.f;
+    for (int z = 0; z < nslots; z++) s += part[z * mn + i];
+    const int m = (int)(i / N), n = (int)(i - (int64_t)m * N);
+    c[(size_t)m * ldc + coff + n] += s;
   }
 }
 
@@ -327,20 +347,40 @@ static int launch_nt(const NtParams& p, cudaStream_t st) {
   return WNB_OK;
 }
 
-static int launch_tn(const TnParams& p, cudaStream_t st) {
-  const int nsplit = cdiv(p.T, p.tchunk);
-  dim3 grid(cdiv(p.M, 128), cdiv(p.N, kBN), p.B * nsplit);
+// the per-stream scratch the partial sums of one launch go to (the launches of a stream run one after the other)
+static float* simt_slots(cudaStream_t st, int64_t floats) {
+  float* part = static_cast<float*>(scratch_buffer(st, SCRATCH_SIMT, (size_t)floats * sizeof(float)));
+  if (!part) set_error("fp32 gradients: cannot allocate the partial-sum scratch (%lld floats)", (long long)floats);
+  return part;
+}
+
+static int launch_slot_reduce(const float* part, int nslots, int M, int N, float* c, int ldc, int coff, cudaStream_t st) {
+  const int64_t mn = (int64_t)M * N;
+  const int grid = (int)(cdiv64(mn, 256) < device_sms() * 8 ? cdiv64(mn, 256) : device_sms() * 8);
+  slot_reduce_kernel<<<grid, 256, 0, st>>>(part, nslots, M, N, c, ldc, coff);
+  WNB_CHECK_LAUNCH("slot_reduce");
+  return WNB_OK;
+}
+
+static int launch_tn(TnParams p, cudaStream_t st) {
+  const int nsplit = cdiv(p.T, p.tchunk), nslots = p.B * nsplit;
+  p.part = nullptr;
+  if (nslots > 1 && !(p.part = simt_slots(st, (int64_t)nslots * p.M * p.N))) return WNB_ERR_CUDA;
+  dim3 grid(cdiv(p.M, 128), cdiv(p.N, kBN), nslots);
   gemm_tn_kernel<<<grid, kThreads, 0, st>>>(p);
   WNB_CHECK_LAUNCH("gemm_tn");
-  return WNB_OK;
+  return p.part ? launch_slot_reduce(p.part, nslots, p.M, p.N, p.c, p.ldc, p.coff, st) : WNB_OK;
 }
 
 static int launch_colsum(const float* a, int lda, int M, int64_t rows, float* out, cudaStream_t st) {
   const int rpb = 512;
   const int threads = M >= 256 ? 256 : ((M + 31) / 32) * 32;
-  colsum_kernel<<<(int)cdiv64(rows, rpb), threads, 0, st>>>(a, lda, M, rows, rpb, out);
+  const int nblocks = (int)cdiv64(rows, rpb);
+  float* part = nullptr;
+  if (nblocks > 1 && !(part = simt_slots(st, (int64_t)nblocks * M))) return WNB_ERR_CUDA;
+  colsum_kernel<<<nblocks, threads, 0, st>>>(a, lda, M, rows, rpb, part, out);
   WNB_CHECK_LAUNCH("colsum");
-  return WNB_OK;
+  return part ? launch_slot_reduce(part, nblocks, 1, M, out, 0, 0, st) : WNB_OK;
 }
 
 static int pick_tchunk(int B, int T, int tiles) {

@@ -32,6 +32,16 @@ so with s = sigmoid(a), th = tanh(g):
                                        + e_dz (e_s + e_th) + 6u |dz| s
 first order in the propagated errors plus the second-order terms above (eps = 2^-10.987, u = 2^-24).
 
+fp32 (SIMT) path.  ``math_mode="fp32"`` multiplies fp32 operands as given (``cv=exact``: every product is exact in
+float64) and accumulates with one ``fmaf`` per term, so the linear bound above holds with room to spare (gamma_K is
+K * 2^-24 for any order).  Its gates are ``sigmoidf_(a) = 1 / (1 + expf(-a))`` with IEEE division and libm ``tanhf``;
+without fast-math both ``expf`` and ``tanhf`` are within 2 ulp (CUDA C Programming Guide, mathematical functions), i.e.
+relative error <= LIBM_REL = 2^-22.  With e = exp(-a), 1 - s = e / (1 + e):
+    s^ = s (1 + d3) / ((1 + d2)(1 + (1-s) d1)),  |d1| <= LIBM_REL, |d2|, |d3| <= u
+so  e_s <= s(1-s) e_a + 0.1 e_a^2 + s ((1-s) LIBM_REL + 3u)  (3u: two roundings plus the second-order terms, valid
+while expf(-a) does not overflow, |a| < 88), and  e_th <= (1-th^2) e_g + 0.77 e_g^2 + |th| LIBM_REL.  ``gate_fn``
+selects the model: GATE_TANH_APPROX (the tensor-core kernels, the default) or GATE_LIBM (the SIMT kernels).
+
 Stages whose input never leaves the chip (the fused per-block forward keeps z in shared memory) take the propagated
 bound of that input as ``e_in``: the kernel's operand then differs from the reference's by e_in plus one tf32
 conversion step of each (2^-10 relative each), which enters through |W|.
@@ -44,7 +54,18 @@ C_ACC = 2.0
 U = 2.0 ** -24                  # fp32 unit roundoff
 TANH_REL = 2.0 ** -10.987       # tanh.approx.f32
 TF32_REL = 2.0 ** -10           # largest relative change of one tf32 conversion (truncation)
+LIBM_REL = 2.0 ** -22           # expf / tanhf without fast-math: 2 ulp
 F64 = torch.float64
+
+
+def GATE_TANH_APPROX(s, th):
+    """function error of the tensor-core gates: (e_s, e_th) of sigmoid = 0.5 tanh.approx(a/2) + 0.5, tanh.approx"""
+    return (s - 0.5).abs() * TANH_REL + 2 * U, th.abs() * TANH_REL + U
+
+
+def GATE_LIBM(s, th):
+    """function error of the SIMT gates: (e_s, e_th) of 1 / (1 + expf(-a)) and tanhf"""
+    return s * ((1 - s) * LIBM_REL + 3 * U), th.abs() * LIBM_REL
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -113,19 +134,20 @@ def gate_pre(xin, haux, w1, b1, d, ks, cv=to_tf32):
     return pre, lin_bound(mag, K1) + U * (acc.abs() + b.abs())
 
 
-def _gate_parts(pre, e_pre):
+def _gate_parts(pre, e_pre, gate_fn):
     R = pre.shape[-1] // 2
     a, g, ea, eg = pre[..., :R], pre[..., R:], e_pre[..., :R], e_pre[..., R:]
     s, th = torch.sigmoid(a), torch.tanh(g)
-    es = s * (1 - s) * ea + 0.1 * ea * ea + (s - 0.5).abs() * TANH_REL + 2 * U
-    eth = (1 - th * th) * eg + 0.77 * eg * eg + th.abs() * TANH_REL + U
+    fs, fth = gate_fn(s, th)
+    es = s * (1 - s) * ea + 0.1 * ea * ea + fs
+    eth = (1 - th * th) * eg + 0.77 * eg * eg + fth
     return s, th, es, eth
 
 
-def gate_fwd(xin, haux, w1, b1, d, ks, cv=to_tf32):
+def gate_fwd(xin, haux, w1, b1, d, ks, cv=to_tf32, gate_fn=GATE_TANH_APPROX):
     """z = sigmoid(a) tanh(g) (B,T,R) and its bound"""
     pre, e = gate_pre(xin, haux, w1, b1, d, ks, cv)
-    s, th, es, eth = _gate_parts(pre, e)
+    s, th, es, eth = _gate_parts(pre, e, gate_fn)
     z = s * th
     return z, th.abs() * es + s * eth + es * eth + 2 * U * z.abs()
 
@@ -200,10 +222,10 @@ def dz_perblock(dout, dskip, w2, cv=to_tf32):
     return acc, lin_bound(mag, K)
 
 
-def gate_bwd(xin, haux, w1, b1, d, ks, dz, e_dz, cv=to_tf32):
+def gate_bwd(xin, haux, w1, b1, d, ks, dz, e_dz, cv=to_tf32, gate_fn=GATE_TANH_APPROX):
     """dpre (B,T,2R) = [d pre-sigmoid | d pre-tanh] from the recomputed gate and dz (known to within e_dz)"""
     pre, e = gate_pre(xin, haux, w1, b1, d, ks, cv)
-    s, th, es, eth = _gate_parts(pre, e)
+    s, th, es, eth = _gate_parts(pre, e, gate_fn)
     dz = dz.to(F64)
     adz = dz.abs()
     ds = s * (1 - s)

@@ -1,6 +1,7 @@
 # -*- coding: utf-8 -*-
 """GPU tier: the same inputs give the same results, bit for bit, run after run -- a tf32 training step of the
-deferred-skip stack (every gradient, including the reductions over time that CTAs share) and a sampling-mode decode."""
+deferred-skip stack and an fp32 (SIMT) training step of the per-block path (every gradient, including the reductions
+over time that CTAs share), and a sampling-mode decode."""
 import numpy as np
 import pytest
 import torch
@@ -11,8 +12,7 @@ from tests.util import our_model
 pytestmark = pytest.mark.gpu
 
 
-def test_training_step_gradients_identical_across_runs():
-    cfg = O.Config(256, 28, 64, 128, 6, 2, 2, 16)
+def _training_step_gradients_identical_across_runs(cfg, math_mode):
     p = O.make_params(cfg, 8)
     rng = np.random.RandomState(3)
     B, T = 2, 4096
@@ -21,7 +21,7 @@ def test_training_step_gradients_identical_across_runs():
     h = torch.from_numpy(rng.standard_normal((B, 28, T // 16)).astype(np.float32)).cuda()
     runs = []
     for _ in range(3):
-        net = our_model(cfg, p, math_mode="tf32").train()
+        net = our_model(cfg, p, math_mode=math_mode).train()
         loss = net.forward_loss(x, h, t, 64)
         loss.backward()
         runs.append((loss.item(), {k: v.grad.clone() for k, v in net.named_parameters() if v.grad is not None}))
@@ -29,6 +29,16 @@ def test_training_step_gradients_identical_across_runs():
         assert loss == runs[0][0]
         for k, g in runs[0][1].items():
             assert torch.equal(g, grads[k]), k
+
+
+def test_training_step_gradients_identical_across_runs():
+    _training_step_gradients_identical_across_runs(O.Config(256, 28, 64, 128, 6, 2, 2, 16), "tf32")
+
+
+def test_fp32_training_step_gradients_identical_across_runs():
+    """the SIMT weight and bias gradients are split over (batch, time range) CTAs whose partial sums are added in slot
+    order, so they do not depend on which CTA finishes first"""
+    _training_step_gradients_identical_across_runs(O.Config(256, 28, 128, 96, 4, 2, 3, 16), "fp32")
 
 
 def test_sampling_decode_identical_across_runs():

@@ -8,6 +8,10 @@ enough to catch the faults tiled kernels make.
   orders, tanh perturbed by up to 2^-11 relative) stays inside the bounds over a few hundred seeded draws.
 * Sensitivity: faults planted into otherwise exact results at the stage-test shapes are reported by assert_within,
   which names the tile.
+* The same two checks for the fp32 (SIMT) model (cv=exact, gate_fn=GATE_LIBM): a float32 emulation of the SIMT kernels
+  (one sequential fmaf per term, bias and epilogue roundings in kernel order, weight gradients summed per (batch, time
+  range) slot and the slots in order, expf / tanhf off by up to 2 ulp) stays inside the bounds, and the faults a tiled
+  FFMA kernel makes (a dropped 16-term K chunk, time tile, gate pass, tap or time range) are reported.
 """
 import numpy as np
 import pytest
@@ -270,3 +274,191 @@ def test_planted_faults_are_reported(case):
     bad_z = m["zall"].clone()
     bad_z[..., 0:R] = m["zall"][..., R:2 * R]
     _raises(ref.skip_gemm(bad_z, m["wskip"], m["bskip"], False)[0], sk, "skip, wrong slice")
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# the fp32 (SIMT) model: float32 emulation of the FFMA kernels
+# ------------------------------------------------------------------------------------------------------------------
+F32 = torch.float32
+
+
+class EmuF32:
+    """The SIMT kernels' arithmetic: every term added with one fmaf in K order (gemm_simt.cuh streams K in chunks of 16
+    into one register accumulator), weight gradients per (batch, time range) slot with the slots added in order, expf /
+    tanhf perturbed by up to 2 ulp (emulated fmaf: the float64 sum of an exact product is rounded twice, which only adds
+    to the error the bounds must cover)."""
+
+    def __init__(self, seed):
+        self.g = torch.Generator().manual_seed(seed)
+
+    @staticmethod
+    def fma_seq(a, b, acc=None):
+        """acc + sum_k a[..., k] b[k, :] with one fmaf per k, k in order; a (M, K), b (K, N) float32"""
+        a, b = a.double(), b.double()
+        acc = torch.zeros(a.shape[0], b.shape[1], dtype=F32) if acc is None else acc
+        for k in range(a.shape[1]):
+            acc = (a[:, k:k + 1] * b[k:k + 1, :] + acc.double()).float()
+        return acc
+
+    def mm(self, a, w):
+        """a (..., K) @ w (N, K)^T"""
+        return self.fma_seq(a.reshape(-1, a.shape[-1]), w.t()).reshape(*a.shape[:-1], w.shape[0])
+
+    def fn(self, exact64):
+        """a libm result within 2 ulp of the exact value: round(exact + delta ulp), |delta| <= 1.5, half the draws at
+        the extremes"""
+        _, ex = torch.frexp(exact64)
+        ulp = torch.ldexp(torch.ones_like(exact64), ex - 24)
+        dl = (torch.rand(exact64.shape, generator=self.g, dtype=F64) * 2 - 1) * 1.5
+        edge = torch.rand(exact64.shape, generator=self.g) < 0.5
+        dl = torch.where(edge, dl.sign() * 1.5, dl)
+        return (exact64 + dl * ulp).float()
+
+    def gates(self, pre):
+        R = pre.shape[-1] // 2
+        e = self.fn(torch.exp(-pre[..., :R].double()))
+        s = (1 / (1 + e.double()).float().double()).float()
+        th = self.fn(torch.tanh(pre[..., R:].double()))
+        return s, th
+
+    def pre(self, xin, haux, w1, b1, d, ks):
+        a = torch.cat(ref.taps(xin, ks, d) + [haux], -1)
+        return self.mm(a, w1) + b1
+
+    def wgrad(self, a, b, init, tchunk):
+        """init + sum over slots (b, time range of tchunk) of a^T b, slots in order; a (B,T,M), b (B,T,N)"""
+        B, T = a.shape[:2]
+        total = None
+        for bi in range(B):
+            for t0 in range(0, T, tchunk):
+                part = self.fma_seq(a[bi, t0:t0 + tchunk].t(), b[bi, t0:t0 + tchunk])
+                total = part if total is None else total + part
+        return init + total
+
+    @staticmethod
+    def colsum(a, init, rows_per_block=512):
+        a = a.reshape(-1, a.shape[-1])
+        total = None
+        for r0 in range(0, a.shape[0], rows_per_block):
+            s = torch.zeros(a.shape[1], dtype=F32)
+            for r in range(r0, min(r0 + rows_per_block, a.shape[0])):
+                s = s + a[r]
+            total = s if total is None else total + s
+        return init + total
+
+
+_FP32_KW = dict(cv=ref.exact, gate_fn=ref.GATE_LIBM)
+
+
+@pytest.mark.parametrize("seed", range(24))
+def test_fp32_bounds_hold_under_emulated_simt_arithmetic(seed):
+    """every fp32 stage per draw, 24 draws, from the emulated kernel's own inputs; the largest err/bound is printed"""
+    g = torch.Generator().manual_seed(500 + seed)
+    em = EmuF32(seed)
+    R, Ap, ks = [24, 40, 20][seed % 3], [32, 16, 8][seed % 3], 1 + seed % 4
+    B, T, d, S = 1 + seed % 2, [1, 9, 23][seed % 3], 1 + seed % 5, 36
+    K1 = ks * R + Ap
+    xin, haux = _rand(g, B, T, R), _rand(g, B, T, Ap)
+    w1, b1 = _rand(g, 2 * R, K1, scale=2 * K1 ** -0.5), _rand(g, 2 * R, scale=0.3)
+    w2, b2 = _rand(g, R + S, R, scale=R ** -0.5), _rand(g, R + S, scale=0.1)
+    worst = 0.0
+    # forward: z, the residual output and the skip accumulation from the emulated z
+    s, th = em.gates(em.pre(xin, haux, w1, b1, d, ks))
+    z = s * th
+    worst = max(worst, ref.assert_within(z, *ref.gate_fwd(xin, haux, w1, b1, d, ks, **_FP32_KW), "z"))
+    xout = (em.mm(z, w2[:R]) + b2[:R]) + xin
+    worst = max(worst, ref.assert_within(xout, *ref.res_out(xin, z, w2[:R], b2[:R], cv=ref.exact), "xout"))
+    skip0 = _rand(g, B, T, S)
+    sk = skip0 + (em.mm(z, w2[R:]) + b2[R:])
+    worst = max(worst, ref.assert_within(sk, *ref.skip_gemm(z, w2[R:], b2[R:], False, cv=ref.exact, skip_in=skip0),
+                                         "skip"))
+    # backward: dz = [dout | dskip] W2 in one K loop, the gate from a recomputed pre, dpre in kernel order
+    dout, dskip = _rand(g, B, T, R), _rand(g, B, T, S)
+    dz = em.mm(torch.cat([dout, dskip], -1), w2.t().contiguous())
+    dz_ref, e_dz = ref.dz_perblock(dout, dskip, w2, cv=ref.exact)
+    worst = max(worst, ref.assert_within(dz, dz_ref, e_dz, "dz"))
+    s, th = em.gates(em.pre(xin, haux, w1, b1, d, ks))
+    dpre = torch.cat([dz * th * s * (1 - s), dz * s * (1 - th * th)], -1)
+    worst = max(worst, ref.assert_within(dpre, *ref.gate_bwd(xin, haux, w1, b1, d, ks, dz_ref, e_dz, **_FP32_KW),
+                                         "dpre"))
+    # dx: one K loop over the ks shifted taps of dpre, then + dout
+    dx = em.mm(torch.cat([ref.tshift(dpre, (ks - 1 - j) * d) for j in range(ks)], -1),
+               torch.cat([w1[:, j * R:(j + 1) * R].t() for j in range(ks)], -1)) + dout
+    worst = max(worst, ref.assert_within(dx, *ref.dx_stage(dpre, w1, d, ks, dout, cv=ref.exact), "dx"))
+    # weight and bias gradients: time ranges of tchunk (the kernel's are >= 64; shorter here so several slots add up)
+    tchunk = [1, 4, 16][seed % 3]
+    nsm = B * -(-T // tchunk)
+    bm = torch.cat(ref.taps(xin, ks, d) + [haux], -1)
+    init_w, init_b = _rand(g, 2 * R, K1), _rand(g, 2 * R)
+    dw1 = em.wgrad(dpre, bm, init_w, tchunk)
+    db1 = em.colsum(dpre, init_b, rows_per_block=[1, 5, 512][seed % 3])
+    (dw, bw), (db, bb) = ref.wgrad(dpre, ref.taps(xin, ks, d) + [haux], init_w, init_b, cv=ref.exact, nsm=nsm)
+    worst = max(worst, ref.assert_within(dw1, dw, bw, "dW1"))
+    worst = max(worst, ref.assert_within(db1, db, bb, "db1"))
+    print("seed %d: largest err/bound %.3f" % (seed, worst))
+
+
+def _fp32_model():
+    """a block at SIMT tiling edges: R = 100 (two 64-channel gate passes, the second partial), K1 = 3*100 + 80 = 380
+    (23 full 16-term K chunks and a partial one), T = 130 (three 64-row time tiles, the last of 2 rows)"""
+    g = torch.Generator().manual_seed(77)
+    R, S, Ap, ks, B, T, d = 100, 96, 80, 3, 2, 130, 5
+    K1 = ks * R + Ap
+    m = dict(R=R, S=S, Ap=Ap, ks=ks, B=B, T=T, d=d, K1=K1)
+    m["xin"], m["haux"] = _rand(g, B, T, R), _rand(g, B, T, Ap)
+    m["w1"], m["b1"] = _rand(g, 2 * R, K1, scale=2 * K1 ** -0.5), _rand(g, 2 * R, scale=0.2)
+    m["w2"], m["b2"] = _rand(g, R + S, R, scale=R ** -0.5), _rand(g, R + S, scale=0.1)
+    m["dout"], m["dskip"] = _rand(g, B, T, R), _rand(g, B, T, S)
+    m["init"] = _rand(g, 2 * R, K1)
+    return m
+
+
+def test_fp32_planted_faults_are_reported():
+    m = _fp32_model()
+    R, Ap, ks, B, T, d, K1 = m["R"], m["Ap"], m["ks"], m["B"], m["T"], m["d"], m["K1"]
+    x, haux, w1, b1, w2, b2 = m["xin"], m["haux"], m["w1"], m["b1"], m["w2"], m["b2"]
+    zref = ref.gate_fwd(x, haux, w1, b1, d, ks, **_FP32_KW)
+    ref.assert_within(zref[0].float(), *zref, "z")
+    # 1. the last (partial) 16-term K chunk dropped from the pre-activations
+    w = w1.clone()
+    w[:, K1 // 16 * 16:] = 0
+    _raises(ref.gate_fwd(x, haux, w, b1, d, ks, **_FP32_KW)[0], zref, "z, last K chunk dropped")
+    # 2. a dropped K chunk in the middle (the 16 channels of tap 1 starting at 112)
+    w = w1.clone()
+    w[:, 112:128] = 0
+    _raises(ref.gate_fwd(x, haux, w, b1, d, ks, **_FP32_KW)[0], zref, "z, middle K chunk dropped")
+    # 3. the second 64-channel gate pass reads the first pass's weight rows
+    w = w1.clone()
+    w[64:R], w[R + 64:] = w1[0:R - 64], w1[R:2 * R - 64]
+    _raises(ref.gate_fwd(x, haux, w, b1, d, ks, **_FP32_KW)[0], zref, "z, gate pass 2", "ch=")
+    # 4. the last partial time tile not written (left at the previous content, here 0)
+    bad = zref[0].clone()
+    bad[:, 128:] = 0
+    _raises(bad, zref, "z, last time tile dropped", "time tile 2")
+    # 5. tap 0 (the oldest) dropped: in the gate and in dx
+    w = w1.clone()
+    w[:, :R] = 0
+    _raises(ref.gate_fwd(x, haux, w, b1, d, ks, **_FP32_KW)[0], zref, "z, tap 0 dropped")
+    dz, e_dz = ref.dz_perblock(m["dout"], m["dskip"], w2, cv=ref.exact)
+    dpre_ref = ref.gate_bwd(x, haux, w1, b1, d, ks, dz, e_dz, **_FP32_KW)
+    _raises(ref.gate_bwd(x, haux, w, b1, d, ks, dz, e_dz, **_FP32_KW)[0], dpre_ref, "dpre, tap 0 dropped")
+    dpre = dpre_ref[0].float()
+    dxref = ref.dx_stage(dpre, w1, d, ks, m["dout"], cv=ref.exact)
+    _raises(ref.dx_stage(dpre, w, d, ks, m["dout"], cv=ref.exact)[0], dxref, "dx, tap 0 dropped")
+    # 6. dz without the dout rows (the last-layer K offset applied to an inner block)
+    _raises(ref.dz_perblock(None, m["dskip"], w2, cv=ref.exact)[0], (dz, e_dz), "dz, dout rows skipped")
+    # 7. the skip rows of W2 offset by one row
+    skref = ref.skip_gemm(zref[0].float(), w2[R:], b2[R:], False, cv=ref.exact)
+    _raises(ref.skip_gemm(zref[0].float(), w2[R - 1:-1], b2[R:], False, cv=ref.exact)[0], skref, "skip, row offset")
+    # 8. the weight gradient without its last time range (T = 130: one range of 64 rows of batch 1, 2 rows short)
+    taps = ref.taps(x, ks, d) + [haux]
+    want, wb = ref.wgrad(dpre, taps, m["init"], cv=ref.exact, nsm=6)
+    a = dpre.clone()
+    a[B - 1, 128:] = 0
+    _raises(ref.wgrad(a, taps, m["init"], cv=ref.exact)[0][0], want, "dW1, last time range dropped")
+    with pytest.raises(AssertionError, match="db1, last row block dropped"):
+        ref.assert_within(ref.wgrad(a, taps, m["init"], cv=ref.exact)[1][0], *wb, "db1, last row block dropped")
+    # 9. one slot added twice
+    a = dpre.clone()
+    a[0, 64:128] *= 2
+    _raises(ref.wgrad(a, taps, m["init"], cv=ref.exact)[0][0], want, "dW1, slot counted twice")
