@@ -20,7 +20,8 @@
 // fp32 residual slice and the running skip sum stay in registers in the res+skip accumulator layout for the whole step;
 // the skip sum is added in layer order starting from the first block (python `0 + s0 + s1 ...`, like the fp32 decoders).
 //
-// Rounding points (the float64 emulation in tests/decode_bf16_reference.py restates them): every weight except the
+// Rounding points (the float64 emulation in tests/decode_bf16_reference.py restates them, and the layer-by-layer
+// checker tests/decode_bf16_layers.py checks each stage against them from the queues): every weight except the
 // front embedding is rounded to bf16 on the host (round to nearest even); the A operands of the products are bf16 of
 // the fp32 values: aux, layer input x_l (both as the current column and as dilated taps), z, relu(skip sum) and
 // relu(post-1).  Accumulation, biases, the residual stream, the skip sum, the gate (precise expf / tanhf) and the logits

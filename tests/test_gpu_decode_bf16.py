@@ -41,6 +41,7 @@ CASES = {
     "ljspeech_ks3": ((256, 80, 512, 256, 10, 1, 3, 256), 3, [72, 1, 40]),
     "shallow_256_B70": ((256, 28, 256, 256, 4, 2, 2, 4), 70, None),      # two clusters of 35
     "speaker_A31_U0": ((256, 31, 256, 256, 4, 2, 2, 0), 5, None),
+    "r512_s512": ((256, 28, 512, 512, 10, 1, 2, 80), 4, None),            # decode_bf16_kernel<512, 512>
 }
 _MODELS = {}
 

@@ -8,7 +8,8 @@
   dilation range (queues of up to 2 x 512 slots that wrap);
 * 10 000-step runs in sampling mode with in-kernel Philox (the bench's mode) on the cluster and single-CTA warp forms,
   the streaming and the direct kernel: the error must not grow with time;
-* a CDF-boundary sweep: uniforms that put the sampling target within +-8 ulps of every lane boundary.
+* a CDF-boundary sweep: uniforms that put the sampling target within +-8 ulps of every lane boundary, for these forms
+  and for the bf16 decoder's own pick.
 
 Every case gives each utterance its own multi-sample seed and aux, ragged lengths (1 and max_n among them, different
 inside one CTA) and a batch that is not a multiple of the utterances per CTA.  Every step's logits are compared with
@@ -266,8 +267,11 @@ def test_long_sampling_run_vs_fp64(which):
 # ---------------------------------------------------------------------------------------------------------------------
 # CDF-boundary sweep
 # ---------------------------------------------------------------------------------------------------------------------
+# the bf16 decoder's own pick (decode_bf16.cu): arctic at B = 64, where every CTA's 4 warps pick 2 rows each, and
+# 256/256 at B = 70, two clusters of 35
+BF16_SWEEP = {"arctic_B64": ((256, 28, 512, 256, 10, 3, 2, 80), 64), "r256_B70": ((256, 28, 256, 256, 4, 2, 2, 4), 70)}
 SWEEP = [("warp", f) for f in WARP_FORMS if f not in ("speaker_A31_U0", "A32", "split8")] + \
-        [(k, "nu%d" % nu) for k in ("stream", "direct") for nu in (1, 2, 4)]
+        [(k, "nu%d" % nu) for k in ("stream", "direct") for nu in (1, 2, 4)] + [("bf16", f) for f in BF16_SWEEP]
 
 
 @pytest.mark.parametrize("kernel,form_id", SWEEP)
@@ -277,6 +281,10 @@ def test_sampling_cdf_boundary_sweep(kernel, form_id, monkeypatch):
     uniform for every utterance of a batch.  Every pick must be admissible, so of nonzero probability."""
     if kernel == "warp":
         cfg, net, p64, B, form = _setup_warp(form_id, monkeypatch)
+    elif kernel == "bf16":
+        t, B = BF16_SWEEP[form_id]
+        cfg, net, p64 = _model(t)
+        form = form_id
     else:
         cfg, net, p64 = _model(SHALLOW)
         nsm = _nsm()
