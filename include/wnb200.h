@@ -183,12 +183,22 @@ WNB_API int wnb_zero(void* p, size_t bytes, void* stream);
 #define WNB_PROF_DZALL_GEMM 2  /* dZ_all = dskip Wskip */
 #define WNB_PROF_GATE_BWD 3    /* gate recompute + dz + dpre */
 #define WNB_PROF_DX_GEMM 4     /* dx (+ dhaux) */
-#define WNB_PROF_DW1 5         /* dW1, db1 */
-#define WNB_PROF_DW2RES 6      /* dW2res, db2res */
-#define WNB_PROF_DWSKIP 7      /* dWskip, dbskip */
-#define WNB_PROF_KINDS 8
+#define WNB_PROF_DW1 5         /* dW1, db1 (no longer launched on its own: part of WNB_PROF_WGRAD) */
+#define WNB_PROF_DW2RES 6      /* dW2res, db2res (part of WNB_PROF_WGRAD) */
+#define WNB_PROF_DWSKIP 7      /* dWskip, dbskip (part of WNB_PROF_WGRAD) */
+#define WNB_PROF_WGRAD 8       /* every weight gradient of the stack (dW1, dW2res, dWskip + biases): one launch + reduce */
+#define WNB_PROF_KINDS 9
 WNB_API int wnb_profile_enable(int on);
 WNB_API int wnb_profile_read(int kind, double* total_ms, int* launches);
+
+/* The static work split of the weight-gradient kernel (a host function; no device needed): problem i has stages[i]
+ * stages of cost[i] each, cut into nchunk[i] time chunks of ceil(stages / nchunk) stages (one CTA sums a chunk from
+ * zero, so the chunks fix the summation order); lock[i] != 0 marks problems that share operands through L2, whose chunks
+ * run side by side.  CTA j (of sms) runs the pieces cta_first[j] .. cta_first[j+1]-1; piece q is the stages
+ * pieces[3q+1] .. pieces[3q+2]-1 of problem pieces[3q].  Returns the number of pieces (pieces may be NULL to count
+ * them), or WNB_ERR_INVALID (bad input, or more than max_pieces). */
+WNB_API int wnb_wgrad_partition(const int* stages, const int* nchunk, const double* cost, const int* lock, int nprob,
+                                int sms, int* cta_first, int* pieces, int max_pieces);
 
 /* ---- residual stack in deferred-skip form (training path of WaveNet.forward, wavenet.py:229-236 over :525-536) ----
  * The skip sum over all L blocks is one GEMM over the concatenated gate outputs,

@@ -39,7 +39,7 @@ static int alternate_dir() {
 
 static bool stack_supported(int R, int S, int Ap, int ks, int L) {
   if (!resblock_fwd_z_supported(R, Ap, ks)) return false;
-  if (L < 1 || L > 64 /* wnb_stack_bwd's segment table, wgrad kMaxSeg */) return false;
+  if (L < 1 || L > 64 /* wnb_stack_bwd's segment shift table */) return false;
   if (S % 32 != 0 || S < 32 || (S > 256 && S != 512)) return false;
   return true;
 }
@@ -198,54 +198,49 @@ WNB_API int wnb_stack_bwd(const float* xs, const float* haux, const float* zall,
     dout = dxin;
   }
 
+  // The three weight gradients only read tensors that exist by now and do not depend on each other: ONE problem list,
+  // one launch over every SM (wgrad_tc_multi), so the streaming-bound dW1 / dW2res stages run beside the
+  // consumer-bound dWskip stages instead of after them.
   int seg_shift[64];
   for (int l = 0; l < L; l++) seg_shift[l] = -dilations[l];
-  {  // every block's dW1 (128 x 160) += dpre_l^T [x_l(t-d_l) | x_l(t) | aux(t)], db1 = column sums of dpre_l: one launch
-    WgBlock blk;
-    blk.nops = 1;
-    blk.ops[0] = WgOperand{dpre_all, 2 * R, 0, 4, 0, WG_LAYERED, 0};
-    blk.c = dw1; blk.m_valid = 128; blk.db = db1;
-    const WgOperand b[3] = {{xs, R, 0, 2, 0, WG_LAYERED | WG_SEG_SHIFT, 0}, {xs, R, 0, 2, 0, WG_LAYERED, 0},
-                            {haux, Ap, 0, 1, 0, 0, 0}};
-    const WgOpts o{1, L, seg_shift, 2 * R * K1, 2 * R};
-    ProfScope ps(WNB_PROF_DW1, st);
-    if ((rc = wgrad_tc_blocks(&blk, 1, b, 3, K1, B, T, st, &o)) != WNB_OK) return rc;
+  WgCall calls[3];
+  int ncalls = 0;
+  // every block's dW1 (128 x 160) += dpre_l^T [x_l(t-d_l) | x_l(t) | aux(t)], db1 = column sums of dpre_l: L segments
+  WgBlock blk1;
+  blk1.nops = 1;
+  blk1.ops[0] = WgOperand{dpre_all, 2 * R, 0, 4, 0, WG_LAYERED, 0};
+  blk1.c = dw1; blk1.m_valid = 128; blk1.db = db1;
+  const WgOperand b1op[3] = {{xs, R, 0, 2, 0, WG_LAYERED | WG_SEG_SHIFT, 0}, {xs, R, 0, 2, 0, WG_LAYERED, 0},
+                             {haux, Ap, 0, 1, 0, 0, 0}};
+  calls[ncalls++] = WgCall{&blk1, 1, b1op, 3, K1, WgOpts{1, L, seg_shift, 2 * R * K1, 2 * R, 0}};
+  // every block's dW2res (R x R) += dout_l^T z_l with dout_l = dx_{l+1} (an M = 64 problem: only its 2 sub-tiles are
+  // loaded), db2res = column sums of dout_l; the last block has no residual output, hence L-1 segments
+  WgBlock blk2;
+  blk2.nops = 1;
+  blk2.ops[0] = WgOperand{dx_all + xsz, R, 0, 4, 0, WG_LAYERED, 0};
+  blk2.c = dw2res; blk2.m_valid = R; blk2.db = db2res;
+  const WgOperand b2op[1] = {{zall, ldz, 0, R / 32, 0, 0, R}};
+  if (L > 1) calls[ncalls++] = WgCall{&blk2, 1, b2op, 1, R, WgOpts{1, L - 1, seg_shift, R * R, R, 0}};
+  // dWskip (S x L*R) += dskip^T Z_all, dbskip = column sums of dskip: every 128-row M-block of dskip, the L*R columns
+  // of Z_all in column groups of up to 7 x 32
+  const int groups = ldz / 32;
+  const int nmb = (S + 127) / 128;
+  int nB = 0;
+  for (int c = 7; c >= 1 && !nB; c--)
+    if (groups % c == 0 && groups / c <= 128) nB = c;
+  WNB_REQUIRE(nB > 0, "stack_bwd: cannot split L*R into column groups");
+  WNB_REQUIRE(nmb <= 5, "stack_bwd: at most 5 skip M-blocks");
+  WgBlock blks[5];
+  for (int i = 0; i < nmb; i++) {
+    const int r = 128 * i;
+    blks[i].nops = 1;
+    blks[i].ops[0] = WgOperand{dskip, S, r, 4, 0, 0, 0};
+    blks[i].c = dwskip + (size_t)r * ldz;
+    blks[i].m_valid = (S - r) < 128 ? (S - r) : 128;
+    blks[i].db = dbskip + r;
   }
-  if (L > 1) {  // every block's dW2res (R x R) += dout_l^T z_l with dout_l = dx_{l+1} (rows 64..127 of the M-block: TMA
-                // zero fill), db2res = column sums of dout_l; the last block has no residual output, hence L-1 segments
-    WgBlock blk;
-    blk.nops = 1;
-    blk.ops[0] = WgOperand{dx_all + xsz, R, 0, 4, 0, WG_LAYERED, 0};
-    blk.c = dw2res; blk.m_valid = R; blk.db = db2res;
-    const WgOperand bz[1] = {{zall, ldz, 0, R / 32, 0, 0, R}};
-    const WgOpts o{1, L - 1, seg_shift, R * R, R};
-    ProfScope ps(WNB_PROF_DW2RES, st);
-    if ((rc = wgrad_tc_blocks(&blk, 1, bz, 1, R, B, T, st, &o)) != WNB_OK) return rc;
-  }
-
-  {  // dWskip (S x L*R) += dskip^T Z_all, dbskip = column sums of dskip: every 128-row M-block of dskip in one launch,
-     // the L*R columns of Z_all in groups of up to 7 x 32 handled by different CTAs
-    const int groups = ldz / 32;
-    const int nmb = (S + 127) / 128;
-    int nB = 0;
-    for (int c = 7; c >= 1 && !nB; c--)
-      if (groups % c == 0 && groups / c <= 128) nB = c;
-    WNB_REQUIRE(nB > 0, "stack_bwd: cannot split L*R into column groups");
-    for (int r0 = 0; r0 < S; r0 += 128 * nmb) {
-      WgBlock blk[4];
-      int nblk = 0;
-      for (int r = r0; r < S && nblk < nmb; r += 128, nblk++) {
-        blk[nblk].nops = 1;
-        blk[nblk].ops[0] = WgOperand{dskip, S, r, 4, 0};
-        blk[nblk].c = dwskip + (size_t)r * ldz;
-        blk[nblk].m_valid = (S - r) < 128 ? (S - r) : 128;
-        blk[nblk].db = dbskip + r;
-      }
-      const WgOperand bz[1] = {{zall, ldz, 0, nB, 0}};
-      const WgOpts o{groups / nB};
-      ProfScope ps(WNB_PROF_DWSKIP, st);
-      if ((rc = wgrad_tc_blocks(blk, nblk, bz, 1, ldz, B, T, st, &o)) != WNB_OK) return rc;
-    }
-  }
-  return WNB_OK;
+  const WgOperand bsop[1] = {{zall, ldz, 0, nB, 0, 0, 0}};
+  calls[ncalls++] = WgCall{blks, nmb, bsop, 1, ldz, WgOpts{groups / nB, 1, nullptr, 0, 0, 0}};
+  ProfScope ps(WNB_PROF_WGRAD, st);
+  return wgrad_tc_multi(calls, ncalls, B, T, st);
 }

@@ -13,18 +13,30 @@ struct WgOperand { const float* base; int C; int c0; int groups; int shift; int 
 // (seg_cstride: segment mode, channel offset added per segment -- a block's slice of a concatenated tensor)
 // One M-block: 128 output rows = 4 groups taken from up to 2 operands (TMA zero fill past a tensor's channels).
 struct WgBlock { WgOperand ops[2]; int nops; float* c; int m_valid; float* db; };
-// n_split > 1: the B operand holds n_split consecutive column groups of 32*sum(groups_b) channels each; CTA
-// (g, s) = (blockIdx % n_split, blockIdx / n_split) accumulates column group g over time split s, so that the A
-// operand (read by every group) is shared through L2.  Bias gradients are flushed by group 0 only.
-// nseg > 1: nseg independent problems of identical structure in one launch (every residual block's dW1, say):
-// operands pick their per-segment batch / shift / channel offsets with the WG_* flags, block i's C and db are at
-// c + i*c_seg_stride, db + i*db_seg_stride; CTAs split the flattened (segment, time tile) space evenly.
+// n_split > 1: the B operand holds n_split consecutive column groups of 32*sum(groups_b) channels each, one problem
+// per (M-block, column group); the problems of a call with several M-blocks or column groups share their operands
+// through L2, so they are cut into equal time chunks that run side by side.  Bias gradients: column group 0 only.
+// nseg > 1: nseg independent problems of identical structure (every residual block's dW1, say): operands pick their
+// per-segment batch / shift / channel offsets with the WG_* flags, block i's C and db are at c + i*c_seg_stride,
+// db + i*db_seg_stride.
 // bf16: both operands are rounded to bf16 (nearest even) and multiplied by bf16 wgmma, fp32 accumulate.
 struct WgOpts { int n_split; int nseg; const int* seg_shift; int c_seg_stride; int db_seg_stride; int bf16; };
+// One call = the M-blocks of one B operand list.  wgrad_tc_multi runs the problems of all calls (same bf16 flag) as
+// one launch of device_sms() CTAs plus one reduce; wgrad_tc_blocks / wgrad_tc are one-call lists.
+struct WgCall { const WgBlock* blocks; int nblocks; const WgOperand* b_ops; int nb_ops; int ldc; WgOpts opts; };
+int wgrad_tc_multi(const WgCall* calls, int ncalls, int B, int T, cudaStream_t st);
 int wgrad_tc_blocks(const WgBlock* blocks, int nblocks, const WgOperand* b_ops, int nb_ops, int ldc, int B, int T,
                     cudaStream_t st, const WgOpts* opts = nullptr);
 int wgrad_tc(const WgOperand* a_ops, int na_ops, const WgOperand* b_ops, int nb_ops, float* c, int ldc, int m_valid,
              float* db, int B, int T, cudaStream_t st);
+// The static work split of one launch: problem i has stages[i] stages of cost[i] each, cut into nchunk[i] time chunks
+// of ceil(stages / nchunk) stages (the unit one CTA sums from zero: it fixes the summation order); lock[i] != 0 marks
+// problems that share operands through L2.  Writes CTA j's pieces (one chunk each) to pieces[cta_first[j] ..
+// cta_first[j + 1]) (cta_first has sms + 1 entries; pieces may be null to count them) and returns the piece count, or
+// -1 (bad input, or more than max_pieces).  A pure function of its arguments.
+struct WgPiece { int prob, s0, s1; };
+int wgrad_partition(const int* stages, const int* nchunk, const double* cost, const int* lock, int nprob, int sms,
+                    int* cta_first, WgPiece* pieces, int max_pieces);
 
 // ---- NT GEMM (gemm_nt_tc.cu):  out[b,t,n] = sum_seg sum_k A_seg[b,t+shift,k] W_seg[n0+n][k0+k]  (+ epilogues) ----
 // One segment: activation tensor (B,T,CA) read at rows t+shift, channels [0,K); weight matrix w (rows x ldw,
