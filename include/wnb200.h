@@ -150,6 +150,24 @@ WNB_API int wnb_adam_flat(float* p, const float* g, float* m, float* v, int64_t 
 WNB_API int wnb_mlsa_filter(const void* x, int x_is_i16, const long long* offsets, int n_utts, const double* coef, int order,
                             double alpha, int pd, double gain, void* y, int y_is_i16, void* stream);
 
+/* Resumable MLSA filtering: wnb_mlsa_filter over n_segs segments, each carrying its filter state from one call to the
+ * next, so that a signal filtered in consecutive chunks gives, bit for bit, what one call over the whole signal gives.
+ *   states      caller-owned device table of n_slots slots of wnb_mlsa_state_doubles(order, pd) doubles each; slot s
+ *               at states + s * wnb_mlsa_state_doubles(order, pd), laid out as d1[1..pd], pt1[0..pd], pt20,
+ *               pt[1..pd] (each Pade stage's previous output), then stage k's all-pass chain e[1..order] for
+ *               k = 1..pd (SPTK mlsadf's recursion state in the kernel's form, csrc/mlsa.cu).
+ *   slots       host int32 array of n_segs: segment u loads slot slots[u] and stores into it the state after its own last
+ *               sample (an empty segment leaves its slot unchanged).  The slots are distinct, 0 <= slots[u] < n_slots.
+ *   zero_start  host int32 array of n_segs or NULL: segment u with zero_start[u] != 0 starts from a zero state instead
+ *               of loading its slot (a new signal in a reused slot).
+ * Everything else as wnb_mlsa_filter; 1 <= n_segs <= WNB_MLSA_MAX_STATE_SEGMENTS.  WNB_ERR_INVALID for a bad shape,
+ * pointer or slot, before any device work.  wnb_mlsa_state_doubles returns 0 for an order or pd wnb_mlsa_filter rejects. */
+#define WNB_MLSA_MAX_STATE_SEGMENTS 1024
+WNB_API size_t wnb_mlsa_state_doubles(int order, int pd);
+WNB_API int wnb_mlsa_filter_state(const void* x, int x_is_i16, const long long* offsets, int n_segs, const double* coef,
+                                  int order, double alpha, int pd, double gain, void* y, int y_is_i16, double* states,
+                                  int n_slots, const int32_t* slots, const int32_t* zero_start, void* stream);
+
 /* ---- pack_weights: state_dict layout <-> kernel layout as one launch per direction (SURVEY.md 8b) ----------
  * A table of strided 3-D copies dst[i0*ds0 + i1*ds1 + i2*ds2] = scale * f(src[i0*ss0 + i1*ss1 + i2*ss2]) executed by
  * one kernel (one block row per entry).  `src` / `src2` are absolute device pointers (WNB_PACK_SRC_ABS: the

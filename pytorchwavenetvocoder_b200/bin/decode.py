@@ -35,6 +35,8 @@ from pytorchwavenetvocoder_b200.utils import have_soundfile
 from pytorchwavenetvocoder_b200.utils import write_wav
 from pytorchwavenetvocoder_b200.utils import write_wav_pcm16
 from pytorchwavenetvocoder_b200.utils import WavWriter
+from pytorchwavenetvocoder_b200.utils import check_hdf5
+from pytorchwavenetvocoder_b200.utils.mlsa import MlsaStreamFilter
 
 
 def pad_list(batch_list, pad_value=0.0):
@@ -124,21 +126,42 @@ def get_parser():
     parser.add_argument("--chunk_frames", default=0, type=int,
                         help="decode through a resumable session, feeding this many aux frames per call and writing each "
                              "wav as its samples arrive (0: one launch per batch); the files are the same either way")
+    parser.add_argument("--noise_shaping", action="store_true",
+                        help="restore noise-shaped output with the MLSA filter of --stats (/mlsa/coef, /mlsa/alpha), as "
+                             "noise_shaping.py --inv false does on the wav files; with --chunk_frames each chunk is "
+                             "filtered as it arrives")
     return parser
 
 
-def _decode_chunked(model, x, h, n_samples_list, chunk_frames, paths, fs, n_quantize, pcm16):
+def _restoration_filter(stats):
+    """(coef, alpha) of the noise-shaping restoration (``noise_shaping.py --inv false``: +coef, pd 4)."""
+    if not check_hdf5(stats, "/mlsa/coef"):
+        raise KeyError("\"/mlsa/coef\" is not found in %s." % stats)
+    return np.array(read_hdf5(stats, "/mlsa/coef"), dtype=np.float64), float(read_hdf5(stats, "/mlsa/alpha"))
+
+
+def _decode_chunked(model, x, h, n_samples_list, chunk_frames, paths, fs, n_quantize, pcm16, shaping=None):
     """Decode one batch through ``WaveNet.decode_session`` in chunks of ``chunk_frames`` aux frames and append every
-    utterance's new samples to its wav as they arrive.  Same samples (hence same files) as the one-shot path."""
+    utterance's new samples to its wav as they arrive.  Same samples (hence same files) as the one-shot path.
+
+    ``shaping`` = (coef, alpha): pass each chunk's PCM_16 samples through the MLSA restoration filter on the device
+    first (``MlsaStreamFilter``, rows as keys), which gives the samples ``noise_shaping.py --inv false`` gives for the
+    whole file."""
     sess = model.decode_session(x, n_samples_list, "sampling")
+    filt = MlsaStreamFilter(shaping[0], shaping[1], 4, x.device) if shaping is not None else None
     writers = [WavWriter(p, fs) for p in paths]
     try:
         for f0 in range(0, h.size(2), chunk_frames):
             if sess.done:
                 break
-            out = (sess.step_pcm16 if pcm16 else sess.step)(h[:, :, f0:f0 + chunk_frames])
+            out = (sess.step_pcm16 if pcm16 or filt is not None else sess.step)(h[:, :, f0:f0 + chunk_frames])
             counts = sess.last_counts
             if max(counts) == 0:
+                continue
+            if filt is not None:
+                ys = filt.filter({b: out[b, :c] for b, c in enumerate(counts) if c > 0})
+                for b, y in ys.items():
+                    writers[b].write_pcm16(y.cpu().numpy())
                 continue
             out = out.cpu().numpy()
             for b, w in enumerate(writers):
@@ -191,13 +214,16 @@ def gpu_decode(feat_list, gpu, args, config):
                 use_upsampling_layer=config.use_upsampling_layer,
                 use_speaker_code=config.use_speaker_code)
             chunk = getattr(args, "chunk_frames", 0)
+            # noise shaping filters the decoder's own PCM_16 samples (device quantisation, with or without soundfile);
+            # without --chunk_frames the batch is decoded as one chunk holding every frame, i.e. one-shot decoding
+            shaping = _restoration_filter(args.stats) if getattr(args, "noise_shaping", False) else None
             if args.batch_size > 1:
                 for feat_ids, (batch_x, batch_h, n_samples_list) in generator:
                     logging.info("decoding start")
-                    if chunk > 0:
-                        _decode_chunked(model, batch_x, batch_h, n_samples_list, chunk,
+                    if chunk > 0 or shaping is not None:
+                        _decode_chunked(model, batch_x, batch_h, n_samples_list, chunk or batch_h.size(2),
                                         [args.outdir + "/" + f + ".wav" for f in feat_ids], args.fs, config.n_quantize,
-                                        not have_soundfile())
+                                        not have_soundfile(), shaping)
                         logging.info("wrote %d wavs in %s." % (len(feat_ids), args.outdir))
                         continue
                     # batch_fast_generate returns completion order = ascending length, ties by batch index
@@ -218,9 +244,9 @@ def gpu_decode(feat_list, gpu, args, config):
             else:
                 for feat_id, (x, h, n_samples) in generator:
                     logging.info("decoding %s (length = %d)" % (feat_id, n_samples))
-                    if chunk > 0:
-                        _decode_chunked(model, x, h, [n_samples], chunk, [args.outdir + "/" + feat_id + ".wav"], args.fs,
-                                        config.n_quantize, False)
+                    if chunk > 0 or shaping is not None:
+                        _decode_chunked(model, x, h, [n_samples], chunk or h.size(2),
+                                        [args.outdir + "/" + feat_id + ".wav"], args.fs, config.n_quantize, False, shaping)
                         logging.info("wrote %s.wav in %s." % (feat_id, args.outdir))
                         continue
                     samples = model.fast_generate(x, h, n_samples, args.intervals)
