@@ -467,6 +467,28 @@ WNB_API int wnb_decode_bf16_pool_inputs(const float* frames, const float* up_w, 
                                         float* aux, float* uniforms, int B, int A, int F, int n, int U, uint64_t seed,
                                         void* stream_handle);
 
+/* ---- parking pool streams (csrc/decode_bf16_park.cu, nets/wavenet.py::DecodePool with park_below) -------------------
+ * A parked stream's queues live in a store of its own: [sum_l (ks-1) d_l slots][R] bf16, layer l's slots after those
+ * of layers 0 .. l-1, slot s of layer l holding x_l of the stream's positions v = s mod (ks-1) d_l (the slots an
+ * admission prefill leaves).  wnb_decode_bf16_park_bytes gives its size (0 for a bad shape or a dilation < 1).
+ *
+ * wnb_decode_bf16_pool_park copies n pool rows into stores: row slots[i] of `queues` (the pool's workspace, B =
+ * capacity) goes to stores[i], layer l's row slot s to store slot (s + rotations[i]) mod (ks-1) d_l, with rotations[i] =
+ * v - g for a stream whose next position v is the pool's step g.  wnb_decode_bf16_pool_unpark copies stores[i] back into
+ * row slots[i], store slot s to row slot (s + rotations[i]) mod (ks-1) d_l, with rotations[i] = g' - v for a stream whose
+ * next position v is to be the pool's step g'.  Both copy bit for bit and write every slot of their destination; one
+ * launch per call.
+ *   slots, rotations   host int32 arrays of n (1 <= n <= 64); the slots must be distinct;
+ *   stores             host array of n device pointers, 16-byte aligned, park_bytes each.
+ * WNB_ERR_INVALID for a bad shape, slot, dilation or pointer, before any device work. */
+WNB_API size_t wnb_decode_bf16_park_bytes(int R, int ks, const int32_t* host_dilations, int L);
+WNB_API int wnb_decode_bf16_pool_park(const void* queues, int capacity, const int32_t* slots, void* const* stores,
+                                      const int32_t* rotations, int n, int R, int ks, const int32_t* host_dilations,
+                                      int L, void* stream_handle);
+WNB_API int wnb_decode_bf16_pool_unpark(const void* const* stores, void* queues, int capacity, const int32_t* slots,
+                                        const int32_t* rotations, int n, int R, int ks, const int32_t* host_dilations,
+                                        int L, void* stream_handle);
+
 #ifdef __cplusplus
 }
 #endif

@@ -865,12 +865,12 @@ POOL_MAX_STEPS = 8192
 # streams one admission prefill takes at most: one cluster of the bf16 decoder
 POOL_ADMIT_ROWS = 64
 
-PoolCall = collections.namedtuple("PoolCall", "g0 n admit rows finished")
+PoolCall = collections.namedtuple("PoolCall", "g0 n admit rows finished park resume")
 
 
 class PoolStream(object):
     """One stream of a decode pool: seed length T0 (P = max(T0, rf), n_pad = P - T0), length, aux frames received,
-    samples decoded and the pool slot it occupies (None while it waits)."""
+    samples decoded and the pool slot it occupies (None while it waits or is parked)."""
 
     def __init__(self, sid, T0, total, rf):
         self.sid, self.T0, self.total = sid, T0, total
@@ -887,6 +887,11 @@ class PoolStream(object):
         """The aux column (sample rate) of sample i: position P - 1 + i less the n_pad replicated columns."""
         return self.T0 - 1 + i
 
+    @property
+    def position(self):
+        """The stream's next decoder position: P - 1 + samples decoded."""
+        return self.P - 1 + self.done
+
 
 class PoolSchedule(object):
     """The host arithmetic of a ``DecodePool``, with no device work: which streams enter which slots, how many steps a
@@ -896,10 +901,22 @@ class PoolSchedule(object):
       * ``admit``: groups ``(T0, [stream, ...])`` of at most POOL_ADMIT_ROWS streams with one seed length, each one
         prefill; a stream's queue slots rotate by ``g0 - (P - 1)`` (its first sample is step g0);
       * ``rows``: ``(slot, stream, i0, count)`` for every occupied slot: samples i0 .. i0 + count - 1;
-      * ``finished``: the ids of the streams this call completes (their slots are free for the next call)."""
+      * ``finished``: the ids of the streams this call completes (their slots are free for the next call);
+      * ``park``: ``(slot, stream, rotation)`` for every stream that leaves its slot for a store before the call;
+        ``rotation = v - g0`` for its next position v (the store's slot s holds position v' = s mod qlen);
+      * ``resume``: ``(slot, stream, rotation)`` for every parked stream that enters a free slot after the admissions;
+        ``rotation = g0 - v`` (its next sample is step g0).
 
-    def __init__(self, capacity, receptive_field, dilations, ks, U):
+    ``park_below=None`` is lock step: every stream in a slot stays there until it finishes, and a stream whose aux has not
+    arrived bounds the whole call.  With ``park_below=m`` (an int >= 1), a stream needs ``min(m, samples left)``
+    runnable samples to hold a slot: a stream in a slot with fewer is parked, and a parked stream that has them again is
+    resumed into any free slot, ahead of the waiting streams.  A stream whose aux is complete is never parked."""
+
+    def __init__(self, capacity, receptive_field, dilations, ks, U, park_below=None):
+        if park_below is not None and (not isinstance(park_below, int) or park_below < 1):
+            raise ValueError("park_below should be None or an int >= 1, got %r" % (park_below,))
         self.capacity, self.rf, self.ks, self.U = capacity, receptive_field, ks, U
+        self.park_below = park_below
         self.period = 1                      # lcm of the queue lengths (ks - 1) d_l
         for d in dilations:
             q = (ks - 1) * d
@@ -907,8 +924,9 @@ class PoolSchedule(object):
         self.g = ks - 1                      # the front gather reads g - (ks - 1) .. g: never a position below 0
         self.slots = [None] * capacity
         self.waiting = []                    # FIFO
-        self.streams = {}                    # id -> PoolStream, until it finishes
-        self.finished = set()
+        self.parked = []                     # in the order they were parked
+        self.streams = {}                    # id -> PoolStream, until it finishes or is cancelled
+        self.finished = set()                # ids of the streams that finished or were cancelled
 
     def add(self, sid, T0, total):
         st = PoolStream(sid, T0, total, self.rf)
@@ -916,11 +934,39 @@ class PoolSchedule(object):
         self.waiting.append(st)
         return st
 
+    def cancel(self, sid):
+        """Remove a waiting, active or parked stream; an active stream's slot is free for the next call."""
+        st = self.streams.pop(sid)
+        if st in self.waiting:
+            self.waiting.remove(st)
+        elif st in self.parked:
+            self.parked.remove(st)
+        else:
+            self.slots[st.slot] = None
+        st.slot = None
+        self.finished.add(sid)
+        return st
+
+    def _fits(self, st):
+        """Under park_below: the stream can run the samples it needs to hold a slot."""
+        return st.runnable(self.U, self.ks) >= min(self.park_below, st.total - st.done)
+
     def next_call(self, max_samples=None):
         U, ks = self.U, self.ks
-        free = [s for s, st in enumerate(self.slots) if st is None]
-        ready = [st for st in self.waiting if st.runnable(U, ks) > 0][:len(free)]
-        active = [st for st in self.slots if st is not None] + ready
+        # the plan works on a copy: a call that launches nothing changes nothing
+        slots, park, resume = list(self.slots), [], []
+        if self.park_below is None:
+            free = [s for s, st in enumerate(slots) if st is None]
+            ready = [st for st in self.waiting if st.runnable(U, ks) > 0][:len(free)]
+        else:
+            for s, st in enumerate(slots):
+                if st is not None and not self._fits(st):
+                    park.append((s, st))
+                    slots[s] = None
+            free = [s for s, st in enumerate(slots) if st is None]
+            resume = [st for st in self.parked if self._fits(st)][:len(free)]
+            ready = [st for st in self.waiting if self._fits(st)][:len(free) - len(resume)]
+        active = [st for st in slots if st is not None] + resume + ready
         if not active:
             return None
         # one launch for every row: a stream whose aux is still incomplete bounds the call by what it can run
@@ -938,6 +984,18 @@ class PoolSchedule(object):
                 raise ValueError("POOL_COUNTER_LIMIT %d leaves no step after a rebase to %d"
                                  % (POOL_COUNTER_LIMIT, self.g))
             n = min(n, POOL_COUNTER_LIMIT - self.g)
+        # rotations from g0: a rebase moves g by a multiple of every queue length, so a parked row's slots do not care
+        park_calls, resume_calls = [], []
+        for s, st in park:
+            park_calls.append((s, st, st.position - self.g))
+            self.slots[s], st.slot = None, None
+            self.parked.append(st)
+        free = iter(free)
+        for st in resume:
+            s = next(free)
+            resume_calls.append((s, st, self.g - st.position))
+            self.parked.remove(st)
+            st.slot, self.slots[s] = s, st
         groups = collections.OrderedDict()
         for st, s in zip(ready, free):
             self.waiting.remove(st)
@@ -959,7 +1017,7 @@ class PoolSchedule(object):
                 self.finished.add(st.sid)
         g0 = self.g
         self.g += n
-        return PoolCall(g0, n, admit, rows, finished)
+        return PoolCall(g0, n, admit, rows, finished, park_calls, resume_calls)
 
 
 def _pinned_int32(values, dev):
@@ -978,12 +1036,17 @@ class DecodePool(object):
     (``wnb_decode_bf16_pool_inputs``).  Stream k of a pool with seed S decodes exactly what row k of
     ``net._decode(X, H, n_list, mode, seed=S, kernel="bf16")`` decodes, bit for bit.
 
-    ``step`` runs one launch for every row, so it advances in lock step: a stream whose aux frames have not arrived
-    holds back the whole launch (the call runs only what that stream can run, and nothing if it can run nothing).  The
-    bf16 decoder is much slower than real time (about 1.6 k samples/s per stream at arctic 512/256), so an acoustic model
-    feeding it stays ahead.  The pool snapshots the weights at its creation."""
+    ``step`` runs one launch for every row.  By default (``park_below=None``) it advances in lock step: a stream whose
+    aux frames have not arrived holds back the whole launch (the call runs only what that stream can run, and nothing if
+    it can run nothing).  That suits a local acoustic model, which stays ahead of the bf16 decoder (about 1.6 k samples/s
+    per stream at arctic 512/256).  With ``park_below=m``, a stream that cannot run ``min(m, samples left)`` samples is
+    parked instead: its queues move out of its row into a store of its own (``wnb_decode_bf16_pool_park``), its row
+    serves other streams, and once its frames arrive it is resumed into any free row (``wnb_decode_bf16_pool_unpark``),
+    ahead of the waiting streams, with the same codes.  ``m = 1`` parks only streams that can run nothing; a larger m
+    keeps a slow stream from cutting every call short.  ``cancel`` drops a stream at once.  The pool snapshots the
+    weights at its creation."""
 
-    def __init__(self, net, capacity=64, mode="sampling", seed=None):
+    def __init__(self, net, capacity=64, mode="sampling", seed=None, park_below=None):
         if mode not in ("sampling", "argmax"):
             raise ValueError("mode should be sampling or argmax, got %r" % (mode,))
         capacity = int(capacity)
@@ -1010,9 +1073,11 @@ class DecodePool(object):
         self._admit_queues = torch.empty(lib.wnb_decode_bf16_workspace(POOL_ADMIT_ROWS, self.R, self.ks, self.dil,
                                                                        self.L), dtype=torch.uint8, device=dev)
         self._tail = torch.full((capacity, self.ks), self.Q // 2, dtype=torch.int32, device=dev)   # xs at g - ks + 1 .. g
-        self._sched = PoolSchedule(capacity, self.rf, net.dilations, self.ks, self.U)
+        self._sched = PoolSchedule(capacity, self.rf, net.dilations, self.ks, self.U, park_below)
+        self._park_bytes = lib.wnb_decode_bf16_park_bytes(self.R, self.ks, self.dil, self.L)
         self._x = {}        # id -> seed codes, until admitted
         self._h = {}        # id -> [aux frames (A, F) on the device, absolute frame of column 0]
+        self._parked = {}   # id -> (queue store, last ks codes), while parked
         self._admitted = 0
         self._pcm_tab = None
 
@@ -1026,8 +1091,23 @@ class DecodePool(object):
         """Ids of the admitted streams that wait for a row (or for the aux frames of their first sample), in order."""
         return [st.sid for st in self._sched.waiting]
 
+    @property
+    def parked(self):
+        """Ids of the parked streams, in the order they were parked."""
+        return [st.sid for st in self._sched.parked]
+
+    def cancel(self, stream):
+        """End ``stream`` at once, whether it waits, runs in a row (the row is free for the next call) or is parked.
+        Codes ``step`` returned before stay valid; afterwards ``finished(stream)`` is True, ``feed`` raises KeyError and
+        the id cannot be admitted again."""
+        if stream not in self._sched.streams:
+            raise KeyError("decode pool: unknown or finished stream %r" % (stream,))
+        self._sched.cancel(stream)
+        for d in (self._x, self._h, self._parked):
+            d.pop(stream, None)
+
     def finished(self, stream):
-        """True once every sample of ``stream`` has been returned by ``step``."""
+        """True once every sample of ``stream`` has been returned by ``step``, or once it was cancelled."""
         if stream in self._sched.finished:
             return True
         if stream not in self._sched.streams:
@@ -1076,7 +1156,9 @@ class DecodePool(object):
     def step(self, max_samples=None):
         """Admit the waiting streams whose first aux frames have arrived and run one launch of at most ``max_samples``
         steps.  Returns ``{stream: new codes}`` (int32 device tensors, without synchronising) for every stream in a row;
-        ``{}`` and no launch when no stream can run."""
+        ``{}`` and no launch when no stream can run.  In lock step the launch runs only as many steps as the least-fed
+        stream in a row can run.  With ``park_below`` the call first parks the streams that cannot keep up, then admits
+        waiting streams and resumes parked ones into the free rows (parked ones first), then runs the launch."""
         call, gen = self._call(max_samples)
         return {} if call is None else {st.sid: gen[slot, :c] for slot, st, _, c in call.rows}
 
@@ -1113,6 +1195,39 @@ class DecodePool(object):
         for k, st in enumerate(group):
             self._tail[st.slot] = xs[k, P - ks:]
 
+    def _park(self, lib, park):
+        """Copy the parked streams' rows into stores of their own (one launch per POOL_ADMIT_ROWS streams) and keep their
+        last ks codes.  An active stream that has not finished ran every step of the last call, so its tail row ends at
+        its last sample."""
+        stores = [torch.empty(self._park_bytes, dtype=torch.uint8, device=self.device) for _ in park]
+        for k0 in range(0, len(park), POOL_ADMIT_ROWS):
+            part = park[k0:k0 + POOL_ADMIT_ROWS]
+            n = len(part)
+            check(lib.wnb_decode_bf16_pool_park(ptr(self.queues), self.capacity, (ctypes.c_int32 * n)(*[s for s, _, _ in part]),
+                                                (ctypes.c_void_p * n)(*[ptr(t) for t in stores[k0:k0 + n]]),
+                                                (ctypes.c_int32 * n)(*[r for _, _, r in part]), n, self.R, self.ks,
+                                                self.dil, self.L, stream()),
+                  "decode_bf16_pool_park")
+        tails = self._tail.index_select(0, _pinned_int32([s for s, _, _ in park], self.device).long())
+        for k, (_, st, _) in enumerate(park):
+            self._parked[st.sid] = (stores[k], tails[k])
+
+    def _unpark(self, lib, resume):
+        """Copy the resumed streams' stores into their new rows (one launch per POOL_ADMIT_ROWS streams) and restore
+        their last ks codes."""
+        kept = [self._parked.pop(st.sid) for _, st, _ in resume]
+        for k0 in range(0, len(resume), POOL_ADMIT_ROWS):
+            part = resume[k0:k0 + POOL_ADMIT_ROWS]
+            n = len(part)
+            check(lib.wnb_decode_bf16_pool_unpark((ctypes.c_void_p * n)(*[ptr(q) for q, _ in kept[k0:k0 + n]]),
+                                                  ptr(self.queues), self.capacity,
+                                                  (ctypes.c_int32 * n)(*[s for s, _, _ in part]),
+                                                  (ctypes.c_int32 * n)(*[r for _, _, r in part]), n, self.R, self.ks,
+                                                  self.dil, self.L, stream()),
+                  "decode_bf16_pool_unpark")
+        self._tail.index_copy_(0, _pinned_int32([s for s, _, _ in resume], self.device).long(),
+                               torch.stack([t for _, t in kept]))
+
     def _call(self, max_samples):
         """One pool call: (PoolCall, (capacity, n) int32 codes of steps g0 .. g0 + n - 1), or (None, None)."""
         if max_samples is not None and int(max_samples) < 1:
@@ -1122,8 +1237,13 @@ class DecodePool(object):
             return None, None
         lib = _lib.load()
         C, A, ks, Uc, n = self.capacity, self.A, self.ks, max(self.U, 1), call.n
+        # parking first: a row it frees may take an admitted or a resumed stream in this same call
+        if call.park:
+            self._park(lib, call.park)
         for T0, group in call.admit:
             self._admit_group(lib, T0, group, call.g0)
+        if call.resume:
+            self._unpark(lib, call.resume)
         # each row's frames from the one of its first step, and the table of wnb_decode_bf16_pool_inputs
         table = [[0] * C for _ in range(5)]
         spans = []
@@ -1543,11 +1663,13 @@ class WaveNet(nn.Module):
         with torch.no_grad():
             return DecodeSession(self, x, n_samples_list, mode, seed)
 
-    def decode_pool(self, capacity=64, mode="sampling", seed=None):
+    def decode_pool(self, capacity=64, mode="sampling", seed=None, park_below=None):
         """Start a continuous-batching decode pool of ``capacity`` rows on the bf16 decoder (``decode_math="bf16"``):
         ``admit`` streams at any time, ``feed`` their aux frames and ``step`` to decode; a stream takes a free row as
-        soon as its first frames arrive and leaves it when it finishes.  Stream k of a pool with ``seed`` S decodes
-        what row k of a one-shot bf16 decode with seed S decodes, bit for bit (``DecodePool``).  The pool snapshots the
-        weights now; ``seed`` is drawn from torch's generator when not given."""
+        soon as its first frames arrive and leaves it when it finishes or is cancelled.  Stream k of a pool with
+        ``seed`` S decodes what row k of a one-shot bf16 decode with seed S decodes, bit for bit (``DecodePool``).  The
+        pool runs in lock step, unless ``park_below=m`` lets it park a stream that cannot run min(m, samples left)
+        samples until its frames arrive.  The pool snapshots the weights now; ``seed`` is drawn from torch's generator
+        when not given."""
         with torch.no_grad():
-            return DecodePool(self, capacity, mode, seed)
+            return DecodePool(self, capacity, mode, seed, park_below)
