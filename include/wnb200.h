@@ -168,6 +168,39 @@ WNB_API int wnb_mlsa_filter_state(const void* x, int x_is_i16, const long long* 
                                   int order, double alpha, int pd, double gain, void* y, int y_is_i16, double* states,
                                   int n_slots, const int32_t* slots, const int32_t* zero_start, void* stream);
 
+/* ---- f5: mel-spectrogram features for a batch of utterances (bin/feature_extract.py --feature_type melspc:
+ * low_cut_filter, then librosa.feature.melspectrogram(x / 32768, power=1.0, center=True) and log10(max(1e-10, .)))
+ * in float64 throughout, one float32 rounding at the end; fixed operation order, no atomics: two runs are bit-identical.
+ *
+ * wnb_melspc_lowcut: the low-cut FIR of every utterance, y[n] = sum_{k < n_taps} taps[k] x[n - k] with x[< 0] = 0
+ * (scipy lfilter(taps, 1, x)), one fma chain in ascending k per output sample.
+ *   x        the utterances concatenated, int16 (x_is_i16 = 1: the wav samples, converted like np.float64(x)) or float64;
+ *   offsets  (n_utts + 1 int64, device): utterance u is [offsets[u], offsets[u+1]); max_len = the longest utterance;
+ *   taps     (n_taps float64, device): scipy firwin(255, cutoff / (fs // 2), pass_zero=False) in the recipes;
+ *   y        float64, same layout as x;  y16  NULL or int16, same layout: np.int16(y) (truncation toward zero to int32,
+ *            out-of-range values giving INT_MIN, then the low 16 bits; the reference's filtered wav).
+ *
+ * wnb_melspc: log mel-spectrogram of every utterance.  The input is in int16 units (int16 samples, or the float64 output
+ * of wnb_melspc_lowcut) and is divided by 32768.  Utterance u has n_u = offsets[u+1] - offsets[u] >= 1 samples and
+ * 1 + n_u / hop frames, frames [frame_offsets[u], frame_offsets[u+1]) of out; n_frames = frame_offsets[n_utts] (the host
+ * computes both tables).  Frame t reads positions [t hop, t hop + fftl) of np.pad(x, fftl / 2, mode="reflect"), times
+ * `window` (fftl float64: scipy get_window("hann", fftl)), real FFT (radix-2 Stockham, float64, `twiddles` = fftl / 2
+ * pairs (cos, -sin)(2 pi m / fftl), interleaved), S[k] = hypot(Re, Im) for k <= fftl / 2, then for each mel filter m
+ * E = sum_{mel_lo[m] <= k < mel_hi[m]} (double)mel_basis[m][k] S[k] in ascending k (mel_basis (n_mels, fftl / 2 + 1)
+ * float32, the filters' nonzero ranges in mel_lo / mel_hi, int32), out[frame][m] = (float)log10(max(1e-10, E)).
+ * fftl must be a power of two in [WNB_MELSPC_MIN_FFTL, WNB_MELSPC_MAX_FFTL], else WNB_ERR_UNSUPPORTED.
+ *
+ * Both: WNB_ERR_INVALID for a bad shape or pointer, before any device work. */
+#define WNB_MELSPC_MAX_TAPS 1024
+#define WNB_MELSPC_MIN_FFTL 64
+#define WNB_MELSPC_MAX_FFTL 4096
+WNB_API int wnb_melspc_lowcut(const void* x, int x_is_i16, const long long* offsets, int n_utts, long long max_len,
+                              const double* taps, int n_taps, double* y, int16_t* y16, void* stream);
+WNB_API int wnb_melspc(const void* x, int x_is_i16, const long long* offsets, const long long* frame_offsets, int n_utts,
+                       long long n_frames, int fftl, int hop, const double* window, const double* twiddles,
+                       const float* mel_basis, const int32_t* mel_lo, const int32_t* mel_hi, int n_mels, float* out,
+                       void* stream);
+
 /* ---- pack_weights: state_dict layout <-> kernel layout as one launch per direction (SURVEY.md 8b) ----------
  * A table of strided 3-D copies dst[i0*ds0 + i1*ds1 + i2*ds2] = scale * f(src[i0*ss0 + i1*ss1 + i2*ss2]) executed by
  * one kernel (one block row per entry).  `src` / `src2` are absolute device pointers (WNB_PACK_SRC_ABS: the

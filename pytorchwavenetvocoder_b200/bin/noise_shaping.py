@@ -12,7 +12,8 @@ import sys
 
 import numpy as np
 
-from pytorchwavenetvocoder_b200.utils import check_hdf5, find_files, read_hdf5, read_txt, write_hdf5
+from pytorchwavenetvocoder_b200.utils import (check_hdf5, find_files, read_hdf5, read_txt, read_wav_int16, write_hdf5,
+                                             write_wav_int16)
 from pytorchwavenetvocoder_b200.utils.mlsa import convert_mcep_to_mlsa_coef, mlsa_filter_batch
 
 
@@ -23,26 +24,6 @@ def _strtobool(v):
     if v in ("n", "no", "f", "false", "off", "0"):
         return 0
     raise ValueError("invalid truth value %r" % (v,))
-
-
-def _read_wav_int16(path):
-    """``scipy.io.wavfile.read`` as the reference does (noise_shaping.py:70); stdlib ``wave`` when scipy is missing."""
-    try:
-        from scipy.io import wavfile
-        return wavfile.read(path)
-    except ImportError:
-        import wave
-        with wave.open(path, "rb") as w:
-            return w.getframerate(), np.frombuffer(w.readframes(w.getnframes()), dtype="<i2")
-
-
-def _write_wav_int16(path, fs, x):
-    try:
-        from scipy.io import wavfile
-        wavfile.write(path, fs, x)
-    except ImportError:
-        from pytorchwavenetvocoder_b200.utils import write_wav_pcm16
-        write_wav_pcm16(path, x, fs)
 
 
 def noise_shaping(wav_list, args):
@@ -60,7 +41,7 @@ def noise_shaping(wav_list, args):
         xs = []
         for i, wav_name in enumerate(names):
             logging.info("now processing %s (%d/%d)" % (wav_name, i0 + i + 1, len(wav_list)))
-            fs, x = _read_wav_int16(wav_name)
+            fs, x = read_wav_int16(wav_name)
             if x.dtype != np.int16:
                 logging.warning("wav file format is not 16 bit PCM.")
             if not fs == args.fs:
@@ -71,7 +52,7 @@ def noise_shaping(wav_list, args):
             xs = [np.float64(x) for x in xs]
         ys = mlsa_filter_batch(xs, mlsa_coef, alpha, pd=4, out_int16=True)
         for wav_name, y in zip(names, ys):
-            _write_wav_int16(args.outdir + "/" + os.path.basename(wav_name), args.fs, y)
+            write_wav_int16(args.outdir + "/" + os.path.basename(wav_name), args.fs, y)
 
 
 def main(argv=None):

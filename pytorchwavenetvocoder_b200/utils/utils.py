@@ -207,6 +207,27 @@ def write_wav_pcm16(path, pcm, fs):
         w.writeframes(np.ascontiguousarray(pcm, dtype="<i2").tobytes())
 
 
+def read_wav_int16(path):
+    """``scipy.io.wavfile.read`` as the reference's feature extraction and noise shaping call it: (fs, samples in the
+    file's dtype); the stdlib ``wave`` reader (16-bit PCM) when scipy is missing."""
+    try:
+        from scipy.io import wavfile
+        return wavfile.read(path)
+    except ImportError:
+        import wave
+        with wave.open(path, "rb") as w:
+            return w.getframerate(), np.frombuffer(w.readframes(w.getnframes()), dtype="<i2")
+
+
+def write_wav_int16(path, fs, x):
+    """``scipy.io.wavfile.write(path, fs, x)`` of int16 samples; ``write_wav_pcm16`` when scipy is missing."""
+    try:
+        from scipy.io import wavfile
+        wavfile.write(path, fs, x)
+    except ImportError:
+        write_wav_pcm16(path, x, fs)
+
+
 def write_wav(path, x, fs):
     """``sf.write(path, x, fs, "PCM_16")`` (reference bin/decode.py:319)."""
     try:
