@@ -201,6 +201,39 @@ WNB_API int wnb_melspc(const void* x, int x_is_i16, const long long* offsets, co
                        const float* mel_basis, const int32_t* mel_lo, const int32_t* mel_hi, int n_mels, float* out,
                        void* stream);
 
+/* ---- f6: STFT mel-cepstra for a batch of utterances (bin/feature_extract.py --feature_type mcep: stft_mcep, then
+ * pysptk.mcep(frame, order, alpha, eps=1e-10, etype=1) per frame) in float64 throughout, one float32 rounding at the end;
+ * fixed operation order, no atomics: two runs are bit-identical.
+ *
+ * wnb_mcep: the input is in int16 units (int16 samples, or the float64 output of wnb_melspc_lowcut), NOT divided by
+ * 32768.  Utterance u has n_u = offsets[u+1] - offsets[u] >= fftl samples and (n_u - fftl) / hop + 1 frames, frames
+ * [frame_offsets[u], frame_offsets[u+1]) of out; n_frames = frame_offsets[n_utts] (the host computes both tables).
+ * Frame t is x[t hop, t hop + fftl) (no padding) times `window` (fftl float64: scipy get_window("hamming", fftl)), real
+ * FFT (the Stockham FFT of wnb_melspc, same `twiddles` layout), P_k = |X_k|^2 + eps for k <= fftl / 2, then SPTK mcep's
+ * Newton-Raphson for the mel-cepstrum of order `order` on the axis warped by alpha, every warp a sum over the bins:
+ *   warp_cos      (fftl / 2 + 1 float64): cos w~_k, w~_k = w_k + 2 atan(alpha sin w_k / (1 - alpha cos w_k)),
+ *                 w_k = 2 pi k / fftl;
+ *   init_map      ((order + 2) x (fftl / 2 + 1) float64): rows 0 .. order map log P to SPTK's initial value (real
+ *                 cepstrum of log P, c[0] and c[fftl/2] halved, freqt to the order); row order + 1 gives the halved
+ *                 c[0] that seeds the convergence test;
+ *   neg_alpha_pow (order + 1 float64): (-alpha)^m.
+ * From iteration miniter on, |(r0 - s) / r0| < threshold (r0 the zeroth warped autocorrelation of P / |H|^2, s the
+ * previous checked r0) stops before that iteration's update; at most maxiter updates.  out[frame][m] = (float)c_m,
+ * iters[frame] = the number of updates applied, or -j when iteration j's Cholesky pivot falls below min_det.
+ * Supported: fftl a power of two in [WNB_MCEP_MIN_FFTL, WNB_MCEP_MAX_FFTL], 1 <= order <= WNB_MCEP_MAX_ORDER,
+ * 0 <= alpha <= WNB_MCEP_MAX_ALPHA (there the bin sums equal SPTK's truncated recursions to 1e-13), else
+ * WNB_ERR_UNSUPPORTED.  WNB_ERR_INVALID for a bad shape or pointer, before any device work. */
+#define WNB_MCEP_MIN_FFTL 1024
+#define WNB_MCEP_MAX_FFTL 4096
+#define WNB_MCEP_MAX_ORDER 40
+#define WNB_MCEP_MAX_ALPHA 0.6
+#define WNB_MCEP_MAX_ITER 1000
+WNB_API int wnb_mcep(const void* x, int x_is_i16, const long long* offsets, const long long* frame_offsets, int n_utts,
+                     long long n_frames, int fftl, int hop, int order, double alpha, const double* window,
+                     const double* twiddles, const double* warp_cos, const double* init_map,
+                     const double* neg_alpha_pow, int miniter, int maxiter, double threshold, double eps,
+                     double min_det, float* out, int32_t* iters, void* stream);
+
 /* ---- pack_weights: state_dict layout <-> kernel layout as one launch per direction (SURVEY.md 8b) ----------
  * A table of strided 3-D copies dst[i0*ds0 + i1*ds1 + i2*ds2] = scale * f(src[i0*ss0 + i1*ss1 + i2*ss2]) executed by
  * one kernel (one block row per entry).  `src` / `src2` are absolute device pointers (WNB_PACK_SRC_ABS: the

@@ -9,15 +9,16 @@
 //
 // Frames (melspc_kernel): one block per frame.  Frame t of an utterance of length n reads padded positions
 // [t hop, t hop + fftl) of np.pad(x / 32768, fftl / 2, mode="reflect") through a closed-form index map, multiplies by the
-// window, runs a radix-2 Stockham FFT of length fftl in shared memory (separate re / im arrays, ping-pong, natural-order
-// output, host float64 twiddles), takes |X[k]| with hypot for k = 0 .. fftl / 2, and sums each mel filter's nonzero bins
-// [lo, hi) in ascending order against the float32 filterbank widened to float64.  Then log10(max(1e-10, .)) in float64
+// window, runs a radix-2 Stockham FFT of length fftl in shared memory (stockham.cuh: separate re / im arrays, ping-pong,
+// natural-order output, host float64 twiddles), takes |X[k]| with hypot for k = 0 .. fftl / 2, and sums each mel
+// filter's nonzero bins [lo, hi) in ascending order against the float32 filterbank widened to float64.  Then log10(max(1e-10, .)) in float64
 // and one float32 rounding; the row goes to out[frame_offsets[u] + t][m].  No atomics: two runs are bit-identical.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include "../../include/wnb200.h"
 #include "common.cuh"
+#include "stockham.cuh"
 
 namespace wnb {
 
@@ -102,27 +103,7 @@ __global__ void __launch_bounds__(MS_THREADS_MAX) melspc_kernel(
     im[n] = 0.0;
   }
   __syncthreads();
-  // Stockham radix-2: stage s (Ns = 2^s) combines pairs j, j + N/2 with twiddle exp(-2 pi i k / (2 Ns)), k = j mod Ns,
-  // = twiddles[k * N / (2 Ns)], and writes the natural-order positions (j - k) * 2 + k and that + Ns.
-  for (int s = 0; s < log2n; s++) {
-    const int Ns = 1 << s;
-    for (int j = threadIdx.x; j < half; j += blockDim.x) {
-      const int k = j & (Ns - 1);
-      const int m = k << (log2n - 1 - s);
-      const double wr = twiddles[2 * m], wi = twiddles[2 * m + 1];
-      const double ar = re[j], ai = im[j], br = re[j + half], bi = im[j + half];
-      const double tr = fma(br, wr, -(bi * wi));
-      const double ti = fma(br, wi, bi * wr);
-      const int o = ((j - k) << 1) + k;
-      re2[o] = ar + tr;
-      im2[o] = ai + ti;
-      re2[o + Ns] = ar - tr;
-      im2[o + Ns] = ai - ti;
-    }
-    __syncthreads();
-    double* t = re; re = re2; re2 = t;
-    t = im; im = im2; im2 = t;
-  }
+  stockham_fft(re, im, re2, im2, N, log2n, twiddles);
   double* S = re2;                        // |X[k]|, k = 0 .. N/2
   for (int k = threadIdx.x; k < nb; k += blockDim.x) S[k] = hypot(re[k], im[k]);
   __syncthreads();
