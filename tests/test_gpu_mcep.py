@@ -1,18 +1,8 @@
 # -*- coding: utf-8 -*-
 """GPU tier: STFT mel-cepstra (wnb_mcep, utils/mcep.py mcep_batch, bin/feature_extract.py --feature_type mcep) frame by
-frame against oracle/mcep_oracle.c, and the sd-melspc recipe's noise-shaping stages end to end through the CLIs.
-
-The bar.  The kernel and the oracle run the same Newton iteration in float64 but evaluate its pieces differently: a
-Stockham FFT against a bit-reversed one, sums over the bins with Clenshaw and a Chebyshev recurrence against SPTK's
-FFTs and freqt / frqtr recursions (equal to 1e-13 inside the supported range), a different Cholesky summation order.
-These rounding differences are ~ (2M)^2 eps ~ 1e-12 relative in the warped autocorrelations r(i) (the recurrence to
-order 2M = 80 dominates); Newton's step divides them by the Hessian T + H, whose condition number stays below 1e3 on
-speech-like frames, so the coefficients differ by at most TOL = 1e-9 (1 + |c|).  Where the iteration counts agree, each
-float32 coefficient must lie in [np.float32(oracle - TOL), np.float32(oracle + TOL)]: np.float32(oracle), or its
-neighbour where the oracle lies within TOL of a float32 rounding boundary.  Where they differ, the convergence test sat on its threshold: the oracle's statistic at the first iteration
-the two disagree on must lie within DELTA = 1e-9 of the threshold (the statistics differ by rounding of r(0) only), and
-the GPU row must pass the same bar against the oracle forced to the GPU's count.  Each check prints how many frames took
-that branch and how many coefficients needed the neighbour."""
+frame against oracle/mcep_oracle.c, and the sd-melspc recipe's noise-shaping stages end to end through the CLIs.  The
+bar and the checker are in tests/mcep_check.py; the corners of the supported range and every exit of the Newton loop
+are in tests/test_gpu_mcep_edges.py."""
 import glob
 import os
 import subprocess
@@ -22,72 +12,13 @@ import numpy as np
 import pytest
 
 from oracle import mcep_oracle as MO
+from tests.mcep_check import _check, _speechlike
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-TOL = 1e-9
-DELTA = 1e-9
 ARCTIC = dict(fs=16000, fftl=1024, hop=80, order=25, alpha=0.41)
 LJSPEECH = dict(fs=22050, fftl=1024, hop=256, order=35, alpha=0.455)
 CLI_DEFAULT = dict(fs=16000, fftl=1024, hop=80, order=24, alpha=0.41)
-
-
-def _speechlike(rng, n, amp=8000.0):
-    """a pulse train through a drifting all-pole filter plus noise: formant-like peaks and deep valleys"""
-    from scipy.signal import lfilter
-    e = rng.randn(n) * 300.0
-    e[::int(rng.randint(60, 140))] += amp
-    y = np.zeros(n)
-    for s in range(0, n, 4000):
-        a1 = 1.1 + 0.3 * np.sin(s * 1e-4)             # poles inside |z| < 0.81 for a1 in [0.8, 1.4]
-        seg = lfilter([1.0], [1.0, -a1, 0.75, -0.15], e[s:s + 4000])
-        y[s:s + 4000] = seg / (np.abs(seg).max() + 1e-9) * amp * (0.3 + 0.7 * rng.rand())
-    return y
-
-
-def _allowed(got, want):
-    """got (float32) lies in [np.float32(want - TOL'), np.float32(want + TOL')], TOL' = TOL (1 + |want|): it is
-    np.float32(want), or a neighbour only where the oracle lies within TOL' of a float32 rounding boundary (coefficients
-    much smaller than TOL', of frames with a flat spectrum, may be any float32 in the interval); returns (ok, n_other)"""
-    tol = TOL * (1.0 + np.abs(want))
-    exact = got == np.float32(want)
-    ok = exact | ((got >= np.float32(want - tol)) & (got <= np.float32(want + tol)))
-    return ok, int((ok & ~exact).sum())
-
-
-def _check(xs, fs, fftl, hop, order, alpha, cutoff=0, which=None, stride=1, label=""):
-    """mcep_batch of the whole list against the oracle for the utterances in ``which`` (every ``stride``-th frame)."""
-    from pytorchwavenetvocoder_b200.utils.mcep import mcep_batch
-    from pytorchwavenetvocoder_b200.utils.melspc import lowcut_filter_batch
-    feats, iters = mcep_batch(xs, fs, fftl, hop, order, alpha, highpass_cutoff=cutoff, return_iters=True)
-    xf = lowcut_filter_batch(xs, fs, cutoff)[0] if cutoff else xs
-    n_frames = n_branch = n_neigh = 0
-    hist = np.zeros(31, dtype=np.int64)
-    for u in (range(len(xs)) if which is None else which):
-        fr = MO.frames(xf[u], fftl, hop)
-        assert feats[u].shape == (len(fr), order + 1) and feats[u].dtype == np.float32, (label, u, feats[u].shape)
-        assert np.all(iters[u] >= 0)
-        for t in range(0, len(fr), stride):
-            where = "%s utterance %d (length %d) frame %d" % (label, u, len(xs[u]), t)
-            want, n, st = MO.mcep(fr[t], order, alpha)
-            g = int(iters[u][t])
-            hist[g] += 1
-            if g != n:
-                j = min(g, n) + 1
-                assert abs(st[j] - 1e-3) <= DELTA, "%s: GPU %d updates, oracle %d, oracle statistic %r at iteration " \
-                    "%d is not within %g of the threshold" % (where, g, n, st[j], j, DELTA)
-                want = MO.mcep(fr[t], order, alpha, force_iters=g)[0]
-                n_branch += 1
-            ok, nn = _allowed(feats[u][t], want)
-            if not ok.all():
-                m = int(np.argmin(ok))
-                raise AssertionError("%s coefficient %d: GPU %r, np.float32(oracle) %r (oracle64 %r, %d updates)"
-                                     % (where, m, feats[u][t][m], np.float32(want[m]), want[m], g))
-            n_neigh += nn
-            n_frames += 1
-    print("%s: %d frames checked, %d with a different iteration count, %d coefficients took the neighbour; update "
-          "counts %s" % (label, n_frames, n_branch, n_neigh, {i: int(c) for i, c in enumerate(hist) if c}))
-    return n_frames
 
 
 @pytest.mark.parametrize("cfg,name", [(ARCTIC, "arctic"), (LJSPEECH, "ljspeech"), (CLI_DEFAULT, "cli-default")])
