@@ -201,6 +201,58 @@ WNB_API int wnb_melspc(const void* x, int x_is_i16, const long long* offsets, co
                        const float* mel_basis, const int32_t* mel_lo, const int32_t* mel_hi, int n_mels, float* out,
                        void* stream);
 
+/* ---- f7: streaming mel-spectrogram.  wnb_melspc_stream advances n_segs keyed signals by one chunk each and writes every
+ * frame no later sample can change; concatenated, a signal's frames equal wnb_melspc (after wnb_melspc_lowcut when
+ * n_taps > 0) of the whole signal bit for bit, whatever the chunking.  Frame t reads signal indices
+ * [t hop - fftl / 2, t hop + fftl / 2) through the reflect map of the signal's length; the host decides which frames
+ * are final and which filtered samples to keep (utils/melspc.py melspc_frames_ready, melspc_carry_start).
+ *   states   device table of n_slots slots of wnb_melspc_stream_state_doubles(fftl, n_taps) doubles: the last
+ *            n_taps - 1 input samples (FIR history), then the carry, filtered samples [carry start, n) of a signal that
+ *            has had n samples (at most fftl - 1).
+ *   segs     host table of n_segs rows of WNB_MELSPC_SEG_FIELDS int64, and segs_dev, the same table in device memory
+ *            (the kernels read segs_dev; the library validates segs):
+ *              SLOT      the slot; distinct within a call.
+ *              FLAGS     NEW: exactly when N_BEFORE = 0 (zero history, no carry); STORE: store the new state (a key
+ *                        that does not end with this chunk and has samples in it).
+ *              X_OFF, X_LEN  the chunk, x[X_OFF, X_OFF + X_LEN) (int16 when x_is_i16, else float64, int16 units).
+ *              N_BEFORE  samples the key had before this chunk;  CARRY0  the carry's start index before it.
+ *              SCRATCH   offset of the segment's scratch region (doubles): [old carry | filtered chunk | new history
+ *                        when STORE], N_BEFORE - CARRY0 + X_LEN (+ n_taps - 1) doubles.
+ *              R0, R1    frames [R0, R1) to write, rows OUT_ROW .. OUT_ROW + R1 - R0 of out; OUT_ROW is the running sum
+ *                        of R1 - R0 over the previous segments, n_frames the total.
+ *              CARRY1    the carry's new start index (STORE).
+ *   out      (n_frames, n_mels) float32 raw features.  aux NULL or float32: segment u's frames scaled,
+ *            (x - mean) / scale, transposed to (n_mels, R1 - R0) at aux + OUT_ROW n_mels.  scaler_mode 0: float64
+ *            subtract, round to float32, float64 divide, round; 2: float32 subtract and divide with mean and scale
+ *            rounded to float32 (StandardScaler.transform of float32 features, scikit-learn 0.22 and >= 1.x).
+ * Two launches (the first reads slots and writes scratch, the second reads scratch and writes frames and slots, so no
+ * block reads a slot another block of the call has stored), none when no segment has frames or state to store; no host
+ * synchronisation, no atomics.  WNB_ERR_INVALID for a bad table or pointer, WNB_ERR_UNSUPPORTED for an fftl wnb_melspc
+ * rejects, both before any device work.  wnb_melspc_stream_state_doubles returns 0 for such an fftl or n_taps outside
+ * [0, WNB_MELSPC_MAX_TAPS]. */
+#define WNB_MELSPC_MAX_STREAM_SEGMENTS 1024
+#define WNB_MELSPC_SEG_SLOT 0
+#define WNB_MELSPC_SEG_FLAGS 1
+#define WNB_MELSPC_SEG_X_OFF 2
+#define WNB_MELSPC_SEG_X_LEN 3
+#define WNB_MELSPC_SEG_N_BEFORE 4
+#define WNB_MELSPC_SEG_CARRY0 5
+#define WNB_MELSPC_SEG_SCRATCH 6
+#define WNB_MELSPC_SEG_R0 7
+#define WNB_MELSPC_SEG_R1 8
+#define WNB_MELSPC_SEG_OUT_ROW 9
+#define WNB_MELSPC_SEG_CARRY1 10
+#define WNB_MELSPC_SEG_FIELDS 11
+#define WNB_MELSPC_SEG_NEW 1
+#define WNB_MELSPC_SEG_STORE 2
+WNB_API size_t wnb_melspc_stream_state_doubles(int fftl, int n_taps);
+WNB_API int wnb_melspc_stream(const void* x, int x_is_i16, int n_segs, const long long* segs, const long long* segs_dev,
+                              long long n_frames, int fftl, int hop, const double* taps, int n_taps,
+                              const double* window, const double* twiddles, const float* mel_basis,
+                              const int32_t* mel_lo, const int32_t* mel_hi, int n_mels, double* states, int n_slots,
+                              double* scratch, long long scratch_doubles, float* out, const double* mean,
+                              const double* scale, int scaler_mode, float* aux, void* stream);
+
 /* ---- f6: STFT mel-cepstra for a batch of utterances (bin/feature_extract.py --feature_type mcep: stft_mcep, then
  * pysptk.mcep(frame, order, alpha, eps=1e-10, etype=1) per frame) in float64 throughout, one float32 rounding at the end;
  * fixed operation order, no atomics: two runs are bit-identical.

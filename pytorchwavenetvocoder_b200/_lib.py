@@ -88,6 +88,9 @@ SIGNATURES = {
     "wnb_mlsa_filter_state": (_I, [_P, _I, _P, _I, _P, _I, _c.c_double, _I, _c.c_double, _P, _I, _P, _I, _P, _P, _P]),
     "wnb_melspc_lowcut": (_I, [_P, _I, _P, _I, _L, _P, _I, _P, _P, _P]),
     "wnb_melspc": (_I, [_P, _I, _P, _P, _I, _L, _I, _I] + [_P] * 5 + [_I, _P, _P]),
+    "wnb_melspc_stream_state_doubles": (_c.c_size_t, [_I, _I]),
+    "wnb_melspc_stream": (_I, [_P, _I, _I, _P, _P, _L, _I, _I, _P, _I] + [_P] * 5 + [_I, _P, _I, _P, _L, _P, _P, _P, _I,
+                                                                                      _P, _P]),
     "wnb_mcep": (_I, [_P, _I, _P, _P, _I, _L, _I, _I, _I, _c.c_double] + [_P] * 5
                  + [_I, _I] + [_c.c_double] * 3 + [_P, _P, _P]),
 }

@@ -140,42 +140,88 @@ def _restoration_filter(stats):
     return np.array(read_hdf5(stats, "/mlsa/coef"), dtype=np.float64), float(read_hdf5(stats, "/mlsa/alpha"))
 
 
-def _decode_chunked(model, x, h, n_samples_list, chunk_frames, paths, fs, n_quantize, pcm16, shaping=None):
-    """Decode one batch through ``WaveNet.decode_session`` in chunks of ``chunk_frames`` aux frames and append every
-    utterance's new samples to its wav as they arrive.  Same samples (hence same files) as the one-shot path.
+class SessionWriter(object):
+    """A ``WaveNet.decode_session`` over one batch whose new samples are appended to each utterance's wav as they
+    arrive: ``feed(h_chunk)`` runs one session step and writes what it returned.
 
     ``shaping`` = (coef, alpha): pass each chunk's PCM_16 samples through the MLSA restoration filter on the device
     first (``MlsaStreamFilter``, rows as keys), which gives the samples ``noise_shaping.py --inv false`` gives for the
     whole file."""
-    sess = model.decode_session(x, n_samples_list, "sampling")
-    filt = MlsaStreamFilter(shaping[0], shaping[1], 4, x.device) if shaping is not None else None
-    writers = [WavWriter(p, fs) for p in paths]
+
+    def __init__(self, model, x, n_samples_list, paths, fs, n_quantize, pcm16, shaping=None):
+        self.sess = model.decode_session(x, n_samples_list, "sampling")
+        self.filt = MlsaStreamFilter(shaping[0], shaping[1], 4, x.device) if shaping is not None else None
+        self.writers = [WavWriter(p, fs) for p in paths]
+        self.n_quantize, self.pcm16 = n_quantize, pcm16
+
+    def feed(self, h_chunk):
+        sess, filt = self.sess, self.filt
+        out = (sess.step_pcm16 if self.pcm16 or filt is not None else sess.step)(h_chunk)
+        counts = sess.last_counts
+        if max(counts) == 0:
+            return
+        if filt is not None:
+            ys = filt.filter({b: out[b, :c] for b, c in enumerate(counts) if c > 0})
+            for b, y in ys.items():
+                self.writers[b].write_pcm16(y.cpu().numpy())
+            return
+        out = out.cpu().numpy()
+        for b, w in enumerate(self.writers):
+            if counts[b] == 0:
+                continue
+            if self.pcm16:
+                w.write_pcm16(out[b, :counts[b]])
+            else:
+                w.write(decode_mu_law(out[b, :counts[b]].astype(np.int64), self.n_quantize))
+
+    def close(self):
+        for w in self.writers:
+            w.close()
+
+
+def _decode_chunked(model, x, h, n_samples_list, chunk_frames, paths, fs, n_quantize, pcm16, shaping=None):
+    """Decode one batch through ``WaveNet.decode_session`` in chunks of ``chunk_frames`` aux frames and append every
+    utterance's new samples to its wav as they arrive (``SessionWriter``).  Same samples (hence same files) as the
+    one-shot path."""
+    sw = SessionWriter(model, x, n_samples_list, paths, fs, n_quantize, pcm16, shaping)
     try:
         for f0 in range(0, h.size(2), chunk_frames):
-            if sess.done:
+            if sw.sess.done:
                 break
-            out = (sess.step_pcm16 if pcm16 or filt is not None else sess.step)(h[:, :, f0:f0 + chunk_frames])
-            counts = sess.last_counts
-            if max(counts) == 0:
-                continue
-            if filt is not None:
-                ys = filt.filter({b: out[b, :c] for b, c in enumerate(counts) if c > 0})
-                for b, y in ys.items():
-                    writers[b].write_pcm16(y.cpu().numpy())
-                continue
-            out = out.cpu().numpy()
-            for b, w in enumerate(writers):
-                if counts[b] == 0:
-                    continue
-                if pcm16:
-                    w.write_pcm16(out[b, :counts[b]])
-                else:
-                    w.write(decode_mu_law(out[b, :counts[b]].astype(np.int64), n_quantize))
-        if not sess.done:   # the one-shot path raises the same way instead of writing short files
+            sw.feed(h[:, :, f0:f0 + chunk_frames])
+        if not sw.sess.done:   # the one-shot path raises the same way instead of writing short files
             raise ValueError("aux features too short: %d frames for %d samples" % (h.size(2), max(n_samples_list)))
     finally:
-        for w in writers:
-            w.close()
+        sw.close()
+
+
+def load_model(args, config):
+    """The WaveNet of ``args.checkpoint`` built from ``config`` (model.conf), in eval mode on the current device, with
+    ``args.decode_math``."""
+    upsampling_factor = config.upsampling_factor if config.use_upsampling_layer else 0
+    model = WaveNet(
+        n_quantize=config.n_quantize,
+        n_aux=config.n_aux,
+        n_resch=config.n_resch,
+        n_skipch=config.n_skipch,
+        dilation_depth=config.dilation_depth,
+        dilation_repeat=config.dilation_repeat,
+        kernel_size=config.kernel_size,
+        upsampling_factor=upsampling_factor)
+    model.load_state_dict(torch.load(
+        args.checkpoint, map_location=lambda storage, loc: storage, weights_only=False)["model"])
+    model.eval()
+    model.cuda()
+    model.decode_math = getattr(args, "decode_math", "fp32")
+    return model
+
+
+def load_scaler(stats, feature_type):
+    """The ``StandardScaler`` of ``stats`` (``/<feature_type>/mean`` and ``/scale``)."""
+    scaler = StandardScaler()
+    scaler.mean_ = read_hdf5(stats, "/" + feature_type + "/mean")
+    scaler.scale_ = read_hdf5(stats, "/" + feature_type + "/scale")
+    return scaler
 
 
 def gpu_decode(feat_list, gpu, args, config):
@@ -186,24 +232,8 @@ def gpu_decode(feat_list, gpu, args, config):
     torch.manual_seed(args.seed + gpu)
     with torch.cuda.device(gpu):
         with torch.no_grad():
-            upsampling_factor = config.upsampling_factor if config.use_upsampling_layer else 0
-            model = WaveNet(
-                n_quantize=config.n_quantize,
-                n_aux=config.n_aux,
-                n_resch=config.n_resch,
-                n_skipch=config.n_skipch,
-                dilation_depth=config.dilation_depth,
-                dilation_repeat=config.dilation_repeat,
-                kernel_size=config.kernel_size,
-                upsampling_factor=upsampling_factor)
-            model.load_state_dict(torch.load(
-                args.checkpoint, map_location=lambda storage, loc: storage, weights_only=False)["model"])
-            model.eval()
-            model.cuda()
-            model.decode_math = getattr(args, "decode_math", "fp32")
-            scaler = StandardScaler()
-            scaler.mean_ = read_hdf5(args.stats, "/" + config.feature_type + "/mean")
-            scaler.scale_ = read_hdf5(args.stats, "/" + config.feature_type + "/scale")
+            model = load_model(args, config)
+            scaler = load_scaler(args.stats, config.feature_type)
             generator = decode_generator(
                 feat_list,
                 batch_size=args.batch_size,

@@ -18,7 +18,7 @@
 
 #include "../../include/wnb200.h"
 #include "common.cuh"
-#include "stockham.cuh"
+#include "melspc_frame.cuh"
 
 namespace wnb {
 
@@ -55,23 +55,10 @@ __global__ void __launch_bounds__(LC_THREADS) lowcut_kernel(const void* __restri
   for (int r = threadIdx.x; r < LC_TILE; r += LC_THREADS) {
     const long long n = tile0 + r;
     if (n >= len) break;
-    const double* xr = xs + r + (n_taps - 1);   // xr[-k] = x[n - k]
-    double acc = 0.0;
-#pragma unroll 5
-    for (int k = 0; k < n_taps; k++) acc = fma(b[k], xr[-k], acc);
+    const double acc = lowcut_fma(b, n_taps, xs + r + (n_taps - 1));   // xr[-k] = x[n - k]
     y[off + n] = acc;
     if (y16 != nullptr) y16[off + n] = np_int16(acc);
   }
-}
-
-// np.pad(x, pad, mode="reflect") index map for a signal of length n >= 1 and a position i in [-pad, n + pad): numpy's
-// reflection (edge sample not repeated) is periodic with period 2 (n - 1); a one-sample signal repeats its sample.
-__device__ __forceinline__ long long reflect_index(long long i, long long n) {
-  if (n == 1) return 0;
-  const long long p = 2 * (n - 1);
-  long long j = i % p;
-  if (j < 0) j += p;
-  return j < n ? j : p - j;
 }
 
 __global__ void __launch_bounds__(MS_THREADS_MAX) melspc_kernel(
@@ -96,23 +83,13 @@ __global__ void __launch_bounds__(MS_THREADS_MAX) melspc_kernel(
   const long long start = (f - frame_offsets[lo]) * hop - half;   // signal index of the frame's first sample
   const int16_t* x16 = reinterpret_cast<const int16_t*>(xin);
   const double* x64 = reinterpret_cast<const double*>(xin);
-  for (int n = threadIdx.x; n < N; n += blockDim.x) {
-    const long long j = off + reflect_index(start + n, len);
-    const double v = (x_i16 ? (double)x16[j] : x64[j]) * 0x1p-15;   // x / 32768: exact
-    re[n] = v * window[n];
-    im[n] = 0.0;
-  }
-  __syncthreads();
-  stockham_fft(re, im, re2, im2, N, log2n, twiddles);
-  double* S = re2;                        // |X[k]|, k = 0 .. N/2
-  for (int k = threadIdx.x; k < nb; k += blockDim.x) S[k] = hypot(re[k], im[k]);
-  __syncthreads();
-  for (int m = threadIdx.x; m < n_mels; m += blockDim.x) {
-    const float* w = mel_basis + (size_t)m * nb;
-    double acc = 0.0;
-    for (int k = mel_lo[m]; k < mel_hi[m]; k++) acc = fma((double)w[k], S[k], acc);
-    out[(size_t)f * n_mels + m] = __double2float_rn(log10(fmax(1e-10, acc)));
-  }
+  melspc_frame(
+      [&](int n) {
+        const long long j = off + reflect_index(start + n, len);
+        return x_i16 ? (double)x16[j] : x64[j];
+      },
+      [&](int m, float v) { out[(size_t)f * n_mels + m] = v; }, re, im, re2, im2, N, nb, log2n, window, twiddles,
+      mel_basis, mel_lo, mel_hi, n_mels);
 }
 
 }  // namespace wnb

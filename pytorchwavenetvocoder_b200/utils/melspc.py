@@ -7,7 +7,10 @@ Mirrors the reference's ``melspectrogram_extract`` (bin/feature_extract.py): the
 semantics of librosa 0.6.2-0.9 (``center=True`` reflect padding, periodic Hann window, Slaney mel filterbank stored as
 float32) and ``np.float32(np.log10(np.maximum(1e-10, mspc.T)))``.  librosa is not needed: its filterbank is restated
 here, and the window and FIR taps come from scipy, the functions the reference calls.  A batch of utterances is one
-launch per stage (csrc/melspc.cu), float64 throughout with one float32 rounding at the end; there is no CPU fallback."""
+launch per stage (csrc/melspc.cu), float64 throughout with one float32 rounding at the end; there is no CPU fallback.
+``MelspcStream`` extracts the same features from signals that arrive in chunks (row f7, csrc/melspc_stream.cu),
+bit-identical to ``melspc_batch`` of each whole signal."""
+import ctypes
 import functools
 
 import numpy as np
@@ -213,3 +216,187 @@ def melspc_batch(signals, fs, fftl, hop, n_mels, fmin=None, fmax=None, highpass_
     if filtered_int16:
         return feats, [wavs[off[i]:off[i + 1]] for i in range(len(signals))]
     return feats
+
+
+# ---- streaming (DESIGN.md §6 row f7) --------------------------------------------------------------------------------
+MELSPC_MAX_STREAM_SEGMENTS = 1024   # WNB_MELSPC_MAX_STREAM_SEGMENTS (include/wnb200.h): keys per MelspcStream.push call
+SEG_FIELDS = 11                     # WNB_MELSPC_SEG_FIELDS and the column order of include/wnb200.h
+(SEG_SLOT, SEG_FLAGS, SEG_X_OFF, SEG_X_LEN, SEG_N_BEFORE, SEG_CARRY0, SEG_SCRATCH, SEG_R0, SEG_R1, SEG_OUT_ROW,
+ SEG_CARRY1) = range(SEG_FIELDS)
+SEG_NEW, SEG_STORE = 1, 2
+
+
+def melspc_frames_ready(n, fftl, hop):
+    """Frames of a centred STFT (reflect padding, ``half = fftl // 2``) that no later sample and no end position can
+    change once a signal has had ``n`` samples: frame t reads ``[t hop - half, t hop + half)``, which lies in the known
+    samples and, for t hop >= half is not needed, reflects about index 0 only, once ``t hop + half <= n``."""
+    half = int(fftl) // 2
+    return 0 if n <= half else (int(n) - half) // int(hop) + 1
+
+
+def melspc_carry_start(n, fftl, hop):
+    """First filtered sample the frames still pending after ``n`` samples can read, whatever the signal's final length:
+    the next frame's first sample ``ready(n) hop - half``, or, if the signal ends now, the earliest sample the last
+    frames reach by reflection about the end, ``n - 1 - half``.  Fewer than ``fftl`` samples are kept from here."""
+    half = int(fftl) // 2
+    return max(0, min(melspc_frames_ready(n, fftl, hop) * int(hop) - half, int(n) - 1 - half))
+
+
+def melspc_stream_plan(segments, fftl, hop, n_taps):
+    """The segment table of one ``wnb_melspc_stream`` call, from host counts only (a pure function: the numpy executor
+    of tests/test_melspc_stream_host.py runs the same table on the CPU).
+
+    segments: (slot, samples before this chunk, chunk length, key ends now) per key.  A key with no samples before
+    this chunk is new: zero history and no carry, whatever its slot held.  Returns (table (n, SEG_FIELDS) int64,
+    frames written, scratch doubles).  A key that ends without a sample raises ValueError."""
+    hist = max(int(n_taps) - 1, 0)
+    tab = np.zeros((len(segments), SEG_FIELDS), dtype=np.int64)
+    x_off = rows = scratch = 0
+    for u, (slot, n0, m, final) in enumerate(segments):
+        n1 = n0 + m
+        if final and n1 == 0:
+            raise ValueError("melspc stream: a signal needs at least one sample")
+        r0 = melspc_frames_ready(n0, fftl, hop)
+        r1 = n_frames(n1, hop) if final else melspc_frames_ready(n1, fftl, hop)
+        cs0 = melspc_carry_start(n0, fftl, hop)
+        store = not final and m > 0
+        flags = (SEG_NEW if n0 == 0 else 0) | (SEG_STORE if store else 0)
+        tab[u] = (slot, flags, x_off, m, n0, cs0, scratch, r0, r1, rows, melspc_carry_start(n1, fftl, hop))
+        if r1 > r0 or store:
+            scratch += n0 - cs0 + m + (hist if store else 0)
+        x_off += m
+        rows += r1 - r0
+    return tab, rows, scratch
+
+
+class MelspcStream(object):
+    """Log mel-spectrogram features of signals that arrive in chunks: ``push`` takes the next chunk of any number of
+    signals, keyed by the caller, and returns every frame that no later sample can change.  Concatenated, the frames of
+    a key equal ``melspc_batch`` of its whole signal bit for bit, whatever the chunk sizes (``wnb_melspc_stream`` keeps
+    each key's FIR history and the filtered samples its pending frames still read on the device between calls).
+
+    With ``scaler=(mean, scale)`` (float64, n_mels) the frames come back scaled as ``StandardScaler.transform`` scales
+    the float32 features ``bin/decode.py`` reads, transposed to ``(n_mels, n)``: the aux chunk ``DecodePool.feed``
+    takes and, stacked over rows, ``DecodeSession.step``.  ``scaler_mode`` (0 or 2, see
+    ``device_loader._f32_scaler_mode``) defaults to what the installed scikit-learn does."""
+
+    def __init__(self, fs, fftl, hop, n_mels, fmin=None, fmax=None, highpass_cutoff=0, scaler=None, scaler_mode=None,
+                 device=None):
+        dev = torch.device(device if device is not None else "cuda")
+        self.device = torch.device("cuda", torch.cuda.current_device()) if dev.type == "cuda" and dev.index is None else dev
+        if hop <= 0:
+            raise ValueError("melspc stream: need a frame shift of at least one sample, got %d" % hop)
+        self.fs, self.fftl, self.hop, self.n_mels = int(fs), int(fftl), int(hop), int(n_mels)
+        self.n_taps = N_TAPS if highpass_cutoff else 0
+        self.state_doubles = int(load().wnb_melspc_stream_state_doubles(self.fftl, self.n_taps))
+        if self.state_doubles == 0:
+            raise ValueError("melspc stream: fftl %d is not supported (powers of two from 64 to 4096)" % fftl)
+        basis, lo, hi = mel_filterbank(fs, fftl, n_mels, 0 if fmin is None else fmin, fs // 2 if fmax is None else fmax)
+        d = self.device
+        self._taps = torch.from_numpy(lowcut_taps(fs, highpass_cutoff)).to(d) if highpass_cutoff else None
+        self._window = torch.from_numpy(hann_window(fftl)).to(d)
+        self._tw = torch.from_numpy(np.array(fft_twiddles(self.fftl))).to(d)
+        self._mel = torch.from_numpy(np.array(basis)).to(d)
+        self._lo, self._hi = torch.from_numpy(np.array(lo)).to(d), torch.from_numpy(np.array(hi)).to(d)
+        self._mean = self._scale = None
+        self.scaler_mode = 0
+        if scaler is not None:
+            mean, scale = (np.ascontiguousarray(a, dtype=np.float64) for a in scaler)
+            if mean.shape != (self.n_mels,) or scale.shape != (self.n_mels,):
+                raise ValueError("melspc stream: scaler mean and scale should have shape (%d,)" % self.n_mels)
+            if scaler_mode is None:
+                from .device_loader import _f32_scaler_mode
+                scaler_mode = _f32_scaler_mode()
+            if scaler_mode not in (0, 2):
+                raise ValueError("melspc stream: scaler_mode should be 0 or 2, got %r" % (scaler_mode,))
+            self.scaler_mode = int(scaler_mode)
+            self._mean, self._scale = torch.from_numpy(mean).to(d), torch.from_numpy(scale).to(d)
+        self._states = torch.empty(0, self.state_doubles, dtype=torch.float64, device=d)
+        self._slots = {}       # key -> state slot
+        self._count = {}       # key -> samples pushed so far
+        self._free = []        # slots of closed keys
+        self._used = 0         # slots handed out so far (the table may hold more)
+
+    def slot(self, key):
+        """The state slot of ``key``, or None when the key is not open."""
+        return self._slots.get(key)
+
+    def samples(self, key):
+        """Samples pushed for ``key`` so far (None when the key is not open)."""
+        return self._count.get(key)
+
+    def push(self, chunks, final=()):
+        """``{key: 1-D int16 or float64 CUDA tensor}`` (one dtype per call, int16 units) -> ``{key: frames}`` for every
+        key in ``chunks`` or ``final``: float32 ``(n, n_mels)`` rows, or with a scaler the scaled ``(n_mels, n)`` aux.
+        Keys in ``final`` end with this call (their chunk may be left out or empty): their remaining frames come back
+        and their slot is freed.  A new key starts from zero state.  Two library launches, none when no key has samples
+        or frames; the host is not synchronised."""
+        final = set(final)
+        keys = list(chunks) + [k for k in final if k not in chunks]
+        if not keys:
+            return {}
+        if len(keys) > MELSPC_MAX_STREAM_SEGMENTS:
+            raise ValueError("melspc stream: at most %d keys per call" % MELSPC_MAX_STREAM_SEGMENTS)
+        xs = [chunks[k] for k in keys if k in chunks]
+        dt = xs[0].dtype if xs else torch.int16
+        if dt not in (torch.int16, torch.float64) or any(x.dtype != dt for x in xs):
+            raise ValueError("melspc stream: chunks should all be int16 or all float64")
+        if any(x.dim() != 1 or x.device != self.device for x in xs):
+            raise ValueError("melspc stream: chunks should be 1-D tensors on %s" % self.device)
+        for k in keys:
+            if k in final and self._count.get(k, 0) + (chunks[k].numel() if k in chunks else 0) == 0:
+                raise ValueError("melspc stream: key %r ends without a sample" % (k,))
+        for k in keys:
+            if k not in self._slots:
+                self._open(k)
+        lens = [chunks[k].numel() if k in chunks else 0 for k in keys]
+        tab, rows, scratch = melspc_stream_plan([(self._slots[k], self._count[k], m, k in final)
+                                                 for k, m in zip(keys, lens)], self.fftl, self.hop, self.n_taps)
+        d = self.device
+        out = torch.empty(rows, self.n_mels, dtype=torch.float32, device=d)
+        aux = torch.empty(rows * self.n_mels, dtype=torch.float32, device=d) if self._mean is not None else None
+        if rows > 0 or (tab[:, SEG_FLAGS] & SEG_STORE).any():
+            x = torch.cat([chunks[k] for k in keys if k in chunks]) if sum(lens) > 0 else None
+            xp = ptr(x)   # raises for CPU tensors: there is no CPU fallback
+            with torch.cuda.device(d):
+                host = torch.from_numpy(tab)
+                segs = host.pin_memory().to(d, non_blocking=True)
+                buf = torch.empty(max(scratch, 1), dtype=torch.float64, device=d)
+                check(load().wnb_melspc_stream(
+                    xp, 1 if dt == torch.int16 else 0, len(keys), tab.ctypes.data_as(ctypes.c_void_p), ptr(segs),
+                    rows, self.fftl, self.hop, ptr(self._taps), self.n_taps, ptr(self._window), ptr(self._tw),
+                    ptr(self._mel), ptr(self._lo), ptr(self._hi), self.n_mels, ptr(self._states),
+                    self._states.size(0), ptr(buf), max(scratch, 1), ptr(out), ptr(self._mean), ptr(self._scale),
+                    self.scaler_mode, ptr(aux), stream()), "melspc_stream")
+        res = {}
+        for u, (k, m) in enumerate(zip(keys, lens)):
+            row, nf = int(tab[u, SEG_OUT_ROW]), int(tab[u, SEG_R1] - tab[u, SEG_R0])
+            if aux is not None:
+                res[k] = aux[row * self.n_mels:(row + nf) * self.n_mels].view(self.n_mels, nf)
+            else:
+                res[k] = out[row:row + nf]
+            self._count[k] += m
+        for k in final:
+            self.close(k)
+        return res
+
+    def close(self, key):
+        """Forget ``key`` without output; its slot goes to the next new key (which starts from zero state)."""
+        s = self._slots.pop(key, None)
+        if s is None:
+            raise KeyError("melspc stream: unknown key %r" % (key,))
+        del self._count[key]
+        self._free.append(s)
+
+    def _open(self, key):
+        if self._free:
+            s = min(self._free)
+            self._free.remove(s)
+        else:
+            s, self._used = self._used, self._used + 1
+            if s == self._states.size(0):   # grow the table; a new key's slot is written before it is read
+                grown = torch.empty(max(2 * s, 64), self.state_doubles, dtype=torch.float64, device=self.device)
+                grown[:s] = self._states
+                self._states = grown
+        self._slots[key] = s
+        self._count[key] = 0
