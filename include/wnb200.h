@@ -577,7 +577,9 @@ WNB_API int wnb_decode_bf16_prefill(const int32_t* xs, const float* h, const flo
  *            (frames[b][a][j - [0]] when U = 0), the fp32 value the decoder computes in-kernel; 0 for k >= [4];
  *   uniforms (B, n) out, or NULL (argmax): column k = (r0 >> 8) * 2^-24 of Philox4x32-10((sample [2] + k, stream id [3],
  *            0, 0), seed), the decoder's own draw; 0 for k >= [4].
- * WNB_ERR_INVALID for a bad shape or pointer, before any device work. */
+ * WNB_ERR_INVALID for a bad shape or pointer, before any device work.
+ * wnb_decode_bf16_pool_inputs does not depend on the decoder: the fp32 decoders compute the same fmaf up-sampling and
+ * the same draw in-kernel, and the pool on the fp32 warp decoder (below) uses it unchanged. */
 WNB_API int wnb_decode_bf16_pool_transplant(const void* src_queues, int src_B, const int32_t* src_rows, void* dst_queues,
                                             int capacity, const int32_t* dst_slots, const int32_t* rotations, int n,
                                             int R, int ks, const int32_t* host_dilations, int L, void* stream_handle);
@@ -606,6 +608,29 @@ WNB_API int wnb_decode_bf16_pool_park(const void* queues, int capacity, const in
 WNB_API int wnb_decode_bf16_pool_unpark(const void* const* stores, void* queues, int capacity, const int32_t* slots,
                                         const int32_t* rotations, int n, int R, int ks, const int32_t* host_dilations,
                                         int L, void* stream_handle);
+
+/* ---- continuous batching on the fp32 warp decoder (csrc/decode_pool.cu, nets/wavenet.py::DecodePool) ----------------
+ * The same pool on wnb_decode_warp_at: B = capacity, P = 1, n_pad = 0, U = 0, pos0 = g0, xs_base = g0 - 1,
+ * h_frame0 = g0, Th = max_n = n, W / CL of the capacity, inputs from wnb_decode_bf16_pool_inputs.  The fp32 decoders
+ * read a tap of layer l only at positions >= d_l (a zero before, the causal padding), so the pool's step counter stays
+ * at or above the longest queue, (ks-1) max_l d_l.  An admitted stream's warm-up runs through wnb_decode_warp_prefill
+ * with the pool's CL (not the CL of the admitted group's size: the 2-CTA form sums half of the residual products in
+ * another order).
+ *
+ * The fp32 decoders keep one utterance's queues in one contiguous block of wnb_decode_workspace(1, R, ks, dilations, L)
+ * bytes, [sum_l (ks-1) d_l slots][R] fp32, slot t mod (ks-1) d_l of layer l holding x_l(t).  A pool row, a row of an
+ * admission workspace and a parked stream's store all have this layout, so admission, parking and resuming are one
+ * operation: wnb_decode_pool_move copies n queue blocks src[i] -> dst[i], layer l's slot s to slot
+ * (s + rotations[i]) mod (ks-1) d_l, bit for bit, every slot of the destination written, one launch per call.  Admission
+ * rotates by g_a - (P - 1) (the stream's first sample is the pool's step g_a), parking by v - g (its next position v is
+ * the pool's step g), resuming by g' - v.
+ *   src, dst   host arrays of n device pointers to one utterance's block (workspace + b * block bytes) or to a store of
+ *              that size, 16-byte aligned;
+ *   rotations  host int32 array of n, any sign;  1 <= n <= 64.
+ * WNB_ERR_INVALID, before any device work, for a bad shape (R a multiple of 4), a dilation < 1, a null or misaligned
+ * pointer, a destination given twice or one that overlaps any source (an in-place rotation would race). */
+WNB_API int wnb_decode_pool_move(const void* const* src, void* const* dst, const int32_t* rotations, int n, int R,
+                                 int ks, const int32_t* host_dilations, int L, void* stream_handle);
 
 #ifdef __cplusplus
 }

@@ -79,6 +79,7 @@ SIGNATURES = {
     "wnb_decode_bf16_park_bytes": (_c.c_size_t, [_I, _I, _P, _I]),
     "wnb_decode_bf16_pool_park": (_I, [_P, _I, _P, _P, _P] + [_I] * 3 + [_P, _I, _P]),
     "wnb_decode_bf16_pool_unpark": (_I, [_P, _P, _I, _P, _P] + [_I] * 3 + [_P, _I, _P]),
+    "wnb_decode_pool_move": (_I, [_P, _P, _P] + [_I] * 3 + [_P, _I, _P]),
     "wnb_pack_weights": (_I, [_P, _I, _P, _P, _P, _P]),
     "wnb_zero": (_I, [_P, _c.c_size_t, _P]),
     "wnb_make_train_batch": (_I, [_P, _P, _P, _L, _L, _I, _L, _L] + [_P] * 5 + [_I] * 6 + [_P]),

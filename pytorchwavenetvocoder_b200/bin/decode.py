@@ -8,6 +8,12 @@ Utterances are length-sorted and batched like the reference (``decode_generator`
 GPUs with ``np.array_split`` (:261-262), one process per GPU, no communication (:330-338).  Each batch
 is ONE persistent-kernel launch (``WaveNet.batch_fast_generate``); like the reference the decoding mode is
 "sampling".
+
+With ``--pool_capacity C`` each GPU worker instead decodes its whole file list through one continuous-batching pool
+of C rows (``WaveNet.decode_pool(C, "sampling")``, under either ``--decode_math``): files enter free rows longest
+first as others finish, so no row idles until the longest file of a batch ends.  The stream id of a file is its index
+in the worker's list and the pool seed is ``pool_seed(--seed, gpu)``; each ``{feat_id}.wav`` holds exactly the samples
+the pool API gives for the same model, seed and features (``decode_pool_files``).
 """
 from __future__ import division
 
@@ -130,7 +136,74 @@ def get_parser():
                         help="restore noise-shaped output with the MLSA filter of --stats (/mlsa/coef, /mlsa/alpha), as "
                              "noise_shaping.py --inv false does on the wav files; with --chunk_frames each chunk is "
                              "filtered as it arrives")
+    parser.add_argument("--pool_capacity", default=0, type=int,
+                        help="decode each GPU's files through one continuous-batching pool of this many rows, writing "
+                             "each wav as its samples arrive (0: length-sorted batches of --batch_size)")
     return parser
+
+
+def check_args(args):
+    """Refusals of flag combinations, before anything is written: an error message, or None."""
+    if args.pool_capacity < 0:
+        return "--pool_capacity should be 0 (off) or a positive number of rows, got %d" % args.pool_capacity
+    if args.pool_capacity > 0 and args.chunk_frames > 0:
+        return ("--pool_capacity and --chunk_frames do not combine: the pool already writes each wav as its samples "
+                "arrive, and every frame of a file is present when it is admitted")
+    return None
+
+
+def pool_seed(seed, gpu):
+    """The decode-pool seed of GPU worker ``gpu`` for ``--seed``: the first 64-bit draw of torch's generator after
+    ``torch.manual_seed(seed + gpu)``, the worker's own seeding."""
+    torch.manual_seed(seed + gpu)
+    return int(torch.empty((), dtype=torch.int64).random_().item())
+
+
+def decode_pool_files(model, frames, capacity, seed, load, paths, fs, n_quantize, pcm16, shaping=None):
+    """Decode files 0 .. len(frames) - 1 through one ``model.decode_pool(capacity, "sampling", seed)`` and append each
+    stream's samples to its wav (``paths[i]``) as calls return them; a writer closes when its stream finishes.
+
+    ``load(i)`` -> (h (n_aux, frames) on the GPU, n_samples) reads file i; the stream id is i.  Files are admitted
+    longest first (``frames[i]`` from the file shapes) and loaded lazily: at most 2 * capacity streams are admitted and
+    unfinished at a time.  A stream's codes do not depend on when or into which row it is admitted, so the files are
+    those of the pool API for the same seed and features.  ``pcm16`` or ``shaping``: PCM_16 from ``step_pcm16`` (and,
+    with ``shaping`` = (coef, alpha), through one ``MlsaStreamFilter`` keyed by stream id); otherwise ``decode_mu_law``
+    and the wav writer's quantisation."""
+    order = iter(sorted(range(len(frames)), key=lambda i: (-frames[i], i)))
+    pool = model.decode_pool(capacity, "sampling", seed)
+    filt = MlsaStreamFilter(shaping[0], shaping[1], 4) if shaping is not None else None
+    x = torch.full((1,), int(encode_mu_law(np.zeros(1), n_quantize)[0]), dtype=torch.int64, device="cuda")
+    writers = {}
+    try:
+        while True:
+            while len(writers) < 2 * capacity:
+                i = next(order, None)
+                if i is None:
+                    break
+                h, n_samples = load(i)
+                writers[i] = WavWriter(paths[i], fs)
+                pool.admit(x, n_samples, h, stream=i)
+            if not writers:
+                return
+            out = (pool.step_pcm16 if pcm16 or filt is not None else pool.step)()
+            if not out:   # every frame of an admitted file is present, so some stream can always run
+                raise RuntimeError("decode pool: no stream could run")
+            if filt is not None:
+                out = filt.filter(out)
+            for sid, y in out.items():
+                y = y.cpu().numpy()
+                if pcm16 or filt is not None:
+                    writers[sid].write_pcm16(y)
+                else:
+                    writers[sid].write(decode_mu_law(y.astype(np.int64), n_quantize))
+                if pool.finished(sid):
+                    writers.pop(sid).close()
+                    if filt is not None:
+                        filt.close(sid)
+                    logging.info("wrote %s." % paths[sid])
+    finally:
+        for w in writers.values():
+            w.close()
 
 
 def _restoration_filter(stats):
@@ -230,10 +303,28 @@ def gpu_decode(feat_list, gpu, args, config):
     # re-seed here so that --seed controls the Philox stream of every GPU (distinct per GPU, reproducible)
     np.random.seed(args.seed + gpu)
     torch.manual_seed(args.seed + gpu)
+    capacity = getattr(args, "pool_capacity", 0)
+    seed = pool_seed(args.seed, gpu) if capacity > 0 else None
     with torch.cuda.device(gpu):
         with torch.no_grad():
             model = load_model(args, config)
             scaler = load_scaler(args.stats, config.feature_type)
+            if capacity > 0:
+                logging.info("decoding %d files through a pool of %d rows (seed %d); --batch_size is not used"
+                             % (len(feat_list), capacity, seed))
+
+                def load(i):
+                    h, n = _load_feat(feat_list[i], config.feature_type, config.upsampling_factor,
+                                      config.use_upsampling_layer, config.use_speaker_code, scaler.transform)
+                    return torch.from_numpy(np.asarray(h)).float().t().contiguous().cuda(), n
+
+                frames = [shape_hdf5(f, "/" + config.feature_type)[0] for f in feat_list]
+                paths = [args.outdir + "/" + os.path.basename(f).replace(".h5", "").replace(".npz", "") + ".wav"
+                         for f in feat_list]
+                shaping = _restoration_filter(args.stats) if getattr(args, "noise_shaping", False) else None
+                decode_pool_files(model, frames, capacity, seed, load, paths, args.fs, config.n_quantize,
+                                  not have_soundfile(), shaping)
+                return
             generator = decode_generator(
                 feat_list,
                 batch_size=args.batch_size,
@@ -297,6 +388,10 @@ def main():
         logging.warning("logging is disabled.")
     for key, value in vars(args).items():
         logging.info("%s = %s" % (key, str(value)))
+    refusal = check_args(args)
+    if refusal is not None:
+        logging.error(refusal)
+        sys.exit(1)
     if args.stats is None:
         args.stats = os.path.dirname(args.checkpoint) + "/stats.h5"      # reference decode.py:226-227
     if args.config is None:

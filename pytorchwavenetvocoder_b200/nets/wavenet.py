@@ -910,9 +910,12 @@ class PoolSchedule(object):
     ``park_below=None`` is lock step: every stream in a slot stays there until it finishes, and a stream whose aux has not
     arrived bounds the whole call.  With ``park_below=m`` (an int >= 1), a stream needs ``min(m, samples left)``
     runnable samples to hold a slot: a stream in a slot with fewer is parked, and a parked stream that has them again is
-    resumed into any free slot, ahead of the waiting streams.  A stream whose aux is complete is never parked."""
+    resumed into any free slot, ahead of the waiting streams.  A stream whose aux is complete is never parked.
 
-    def __init__(self, capacity, receptive_field, dilations, ks, U, park_below=None):
+    ``g_base`` is the lowest step counter (default ks - 1: the front gather reads g - (ks - 1) .. g, never a position
+    below 0); the counter starts there and a rebase stays at or above it."""
+
+    def __init__(self, capacity, receptive_field, dilations, ks, U, park_below=None, g_base=None):
         if park_below is not None and (not isinstance(park_below, int) or park_below < 1):
             raise ValueError("park_below should be None or an int >= 1, got %r" % (park_below,))
         self.capacity, self.rf, self.ks, self.U = capacity, receptive_field, ks, U
@@ -921,7 +924,10 @@ class PoolSchedule(object):
         for d in dilations:
             q = (ks - 1) * d
             self.period = self.period * q // math.gcd(self.period, q)
-        self.g = ks - 1                      # the front gather reads g - (ks - 1) .. g: never a position below 0
+        self.g_base = ks - 1 if g_base is None else int(g_base)
+        if self.g_base < ks - 1:
+            raise ValueError("g_base should be at least ks - 1 = %d, got %d" % (ks - 1, self.g_base))
+        self.g = self.g_base
         self.slots = [None] * capacity
         self.waiting = []                    # FIFO
         self.parked = []                     # in the order they were parked
@@ -979,7 +985,7 @@ class PoolSchedule(object):
         if n <= 0:
             return None
         if self.g + n > POOL_COUNTER_LIMIT:
-            self.g = ks - 1 + (self.g - (ks - 1)) % self.period
+            self.g = self.g_base + (self.g - self.g_base) % self.period
             if self.g >= POOL_COUNTER_LIMIT:
                 raise ValueError("POOL_COUNTER_LIMIT %d leaves no step after a rebase to %d"
                                  % (POOL_COUNTER_LIMIT, self.g))
@@ -1020,28 +1026,52 @@ class PoolSchedule(object):
         return PoolCall(g0, n, admit, rows, finished, park_calls, resume_calls)
 
 
+def warp_pool_form(net, capacity):
+    """(NU, W, CL): the form ``wnb_decode_warp_at`` runs for a pool of ``capacity`` rows on the fp32 warp decoder
+    (``wnb_decode_warp_form``).  The thresholds are the library's and follow the device's SM count: on a 132-SM H100 one
+    utterance per 2-CTA cluster up to 66 rows, one per CTA up to 132, two up to 264, four beyond.  Raises ``WnbError``
+    for a model or capacity the warp decoder does not cover."""
+    lib = _lib.load()
+    Q, A, Ap, R, S, ks, L = (net.n_quantize, net.n_aux, net.n_aux_pad, net.n_resch, net.n_skipch, net.kernel_size,
+                             len(net.dilations))
+    form = (ctypes.c_int32 * 4)()
+    if not lib.wnb_decode_warp_supported(Q, Ap, R, S, ks, L) or lib.wnb_decode_warp_form(capacity, L, form) != 0:
+        raise _lib.WnbError("decode_math='fp32' pools run the warp decoder, which does not cover this model (n_quantize "
+                            "%d, n_aux %d, n_resch %d, n_skipch %d, kernel_size %d, %d layers) at capacity %d: it covers "
+                            "n_quantize 256, n_aux <= 32, n_resch 64, n_skipch 512, kernel_size 2; decode_math='bf16' "
+                            "pools cover the recipe sizes" % (Q, A, R, S, ks, L, capacity))
+    return form[0], form[1], form[2]
+
+
 def _pinned_int32(values, dev):
     """A host list as an int32 device tensor, copied without synchronising the host (pinned staging)."""
     return torch.tensor(values, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
 
 
 class DecodePool(object):
-    """Continuous batching on the bf16 decoder (``WaveNet.decode_pool``): streams join a free row of a running batch and
-    leave it the moment they finish, so requests that arrive at different times share one cluster's weight read.
+    """Continuous batching (``WaveNet.decode_pool``): streams join a free row of a running batch and leave it the moment
+    they finish, so requests that arrive at different times share one weight read.  Under ``decode_math="bf16"`` the
+    pool runs the bf16 decoder, under "fp32" the fp32 warp decoder (``warp_pool_form``: the BASELINE shape, 64 res /
+    512 skip, ks 2; another shape raises ``WnbError``).
 
-    The pool is one ``wnb_decode_bf16_at`` batch of ``capacity`` rows, launched once per ``step`` over the pool's global
-    steps g0 .. g0 + n - 1 with P = 1, n_pad = 0, U = 0 (include/wnb200.h, DESIGN §3.7).  A stream's warm-up runs as the
-    usual parallel prefill when it is admitted, and its queues are moved into its row, rotated so that its first sample
-    is the pool's step of admission; each call's aux window and uniforms are written per row for the row's own stream
-    (``wnb_decode_bf16_pool_inputs``).  Stream k of a pool with seed S decodes exactly what row k of
-    ``net._decode(X, H, n_list, mode, seed=S, kernel="bf16")`` decodes, bit for bit.
+    The pool is one decoder batch of ``capacity`` rows (``wnb_decode_bf16_at`` or ``wnb_decode_warp_at``), launched once
+    per ``step`` over the pool's global steps g0 .. g0 + n - 1 with P = 1, n_pad = 0, U = 0 (include/wnb200.h, DESIGN
+    §3.7).  A stream's warm-up runs as the usual parallel prefill when it is admitted, and its queues are moved into its
+    row, rotated so that its first sample is the pool's step of admission (``wnb_decode_bf16_pool_transplant``, or
+    ``wnb_decode_pool_move`` on the warp decoder, whose prefill runs with the pool's CL); each call's aux window and
+    uniforms are written per row for the row's own stream (``wnb_decode_bf16_pool_inputs``, shared by both decoders).
+    Stream k of a bf16 pool with seed S decodes exactly what row k of ``net._decode(X, H, n_list, mode, seed=S,
+    kernel="bf16")`` decodes, bit for bit.  Stream k of an fp32 pool with seed S decodes what row k of
+    ``net._decode(X, H, n_list, mode, seed=S, kernel="warp")`` decodes, bit for bit, for a one-shot batch whose warp form
+    (``wnb_decode_warp_form``: NU, W, CL) equals the pool's: the form sets the order of some fp32 sums.
 
     ``step`` runs one launch for every row.  By default (``park_below=None``) it advances in lock step: a stream whose
     aux frames have not arrived holds back the whole launch (the call runs only what that stream can run, and nothing if
     it can run nothing).  That suits a local acoustic model, which stays ahead of the bf16 decoder (about 1.6 k samples/s
     per stream at arctic 512/256).  With ``park_below=m``, a stream that cannot run ``min(m, samples left)`` samples is
-    parked instead: its queues move out of its row into a store of its own (``wnb_decode_bf16_pool_park``), its row
-    serves other streams, and once its frames arrive it is resumed into any free row (``wnb_decode_bf16_pool_unpark``),
+    parked instead: its queues move out of its row into a store of its own (``wnb_decode_bf16_pool_park``, or
+    ``wnb_decode_pool_move`` on the warp decoder), its row serves other streams, and once its frames arrive it is
+    resumed into any free row (``wnb_decode_bf16_pool_unpark``, or ``wnb_decode_pool_move``),
     ahead of the waiting streams, with the same codes.  ``m = 1`` parks only streams that can run nothing; a larger m
     keeps a slow stream from cutting every call short.  ``cancel`` drops a stream at once.  The pool snapshots the
     weights at its creation."""
@@ -1052,29 +1082,42 @@ class DecodePool(object):
         capacity = int(capacity)
         if capacity < 1:
             raise ValueError("a decode pool needs a capacity of at least 1, got %d" % capacity)
-        if getattr(net, "decode_math", "fp32") != "bf16":
-            raise _lib.WnbError("decode pools run the bf16 decoder: set decode_math='bf16' (got %r)"
-                                % (getattr(net, "decode_math", "fp32"),))
+        decode_math = getattr(net, "decode_math", "fp32")
+        if decode_math not in ("fp32", "bf16"):
+            raise _lib.WnbError("decode pools run the bf16 decoder (decode_math='bf16') or the fp32 warp decoder "
+                                "(decode_math='fp32'), got %r" % (decode_math,))
         lib = _lib.load()
         self.device = dev = _device()
         self.Q, self.A, self.Ap, self.R, self.S, self.ks, self.U = (
             net.n_quantize, net.n_aux, net.n_aux_pad, net.n_resch, net.n_skipch, net.kernel_size, net.upsampling_factor)
         self.rf, self.L, self.capacity = net.receptive_field, len(net.dilations), capacity
         self.dil = (ctypes.c_int32 * self.L)(*net.dilations)
-        self.wstream = _bf16_weight_stream(lib, net)
+        self.kernel = "bf16" if decode_math == "bf16" else "warp"
+        g_base = None
+        if self.kernel == "bf16":
+            self.wstream = _bf16_weight_stream(lib, net)
+            qbytes = lib.wnb_decode_bf16_workspace(capacity, self.R, self.ks, self.dil, self.L)
+            admit_bytes = lib.wnb_decode_bf16_workspace(POOL_ADMIT_ROWS, self.R, self.ks, self.dil, self.L)
+            self._park_bytes = lib.wnb_decode_bf16_park_bytes(self.R, self.ks, self.dil, self.L)
+        else:
+            _, self.W, self.CL = warp_pool_form(net, capacity)
+            self.wstream = net._decode_warp_pack(self.W, self.CL)
+            assert self.wstream.numel() == lib.wnb_decode_warp_floats(self.L, self.CL)
+            # one utterance's queue block: a pool row, a row of the admission workspace and a parked stream's store
+            self._block = lib.wnb_decode_workspace(1, self.R, self.ks, self.dil, self.L)
+            qbytes, admit_bytes, self._park_bytes = capacity * self._block, POOL_ADMIT_ROWS * self._block, self._block
+            # the fp32 decoders read layer l's tap only at positions >= d_l (a zero before): keep g at or above that
+            g_base = (self.ks - 1) * max(net.dilations)
         self.w, self.upw, self.upb = _decode_snapshot(net)
         self.mode = MODE_ARGMAX if mode == "argmax" else MODE_SAMPLING
         if seed is None:
             seed = int(torch.empty((), dtype=torch.int64).random_().item())  # follows torch.manual_seed, like _decode
         self.seed = ctypes.c_uint64(seed & 0xFFFFFFFFFFFFFFFF)
         # zeroed once: the decoder is never launched with pos0 = 0 here, so it never clears them
-        self.queues = torch.zeros(lib.wnb_decode_bf16_workspace(capacity, self.R, self.ks, self.dil, self.L),
-                                  dtype=torch.uint8, device=dev)
-        self._admit_queues = torch.empty(lib.wnb_decode_bf16_workspace(POOL_ADMIT_ROWS, self.R, self.ks, self.dil,
-                                                                       self.L), dtype=torch.uint8, device=dev)
+        self.queues = torch.zeros(qbytes, dtype=torch.uint8, device=dev)
+        self._admit_queues = torch.empty(admit_bytes, dtype=torch.uint8, device=dev)
         self._tail = torch.full((capacity, self.ks), self.Q // 2, dtype=torch.int32, device=dev)   # xs at g - ks + 1 .. g
-        self._sched = PoolSchedule(capacity, self.rf, net.dilations, self.ks, self.U, park_below)
-        self._park_bytes = lib.wnb_decode_bf16_park_bytes(self.R, self.ks, self.dil, self.L)
+        self._sched = PoolSchedule(capacity, self.rf, net.dilations, self.ks, self.U, park_below, g_base)
         self._x = {}        # id -> seed codes, until admitted
         self._h = {}        # id -> [aux frames (A, F) on the device, absolute frame of column 0]
         self._parked = {}   # id -> (queue store, last ks codes), while parked
@@ -1184,6 +1227,15 @@ class DecodePool(object):
         xs[:, n_pad:] = torch.stack([self._x.pop(st.sid) for st in group])
         Fg = min(self._h[st.sid][0].size(1) for st in group)
         h = torch.stack([self._h[st.sid][0][:, :Fg] for st in group]).contiguous()
+        if self.kernel == "warp":
+            # the pool's CL, not the group's: the 2-CTA form sums half of the residual products in another order
+            _warp_prefill(lib, xs, P, h, self.upw, self.upb, self.w, self.dil, self.L, self._admit_queues, n_pad, self.A,
+                          self.U, self.CL)
+            base = ptr(self._admit_queues)
+            self._move(lib, [(base + k * self._block, self._row(st.slot), g0 - (P - 1)) for k, st in enumerate(group)])
+            for k, st in enumerate(group):
+                self._tail[st.slot] = xs[k, P - ks:]
+            return
         _bf16_prefill(lib, xs, P, h, self.upw, self.upb, self.w, self.wstream, self.dil, self.L, self._admit_queues,
                       n_pad, self.A, self.Ap, self.R, self.S, ks, self.U)
         check(lib.wnb_decode_bf16_pool_transplant(ptr(self._admit_queues), Bg, (ctypes.c_int32 * Bg)(*range(Bg)),
@@ -1200,6 +1252,15 @@ class DecodePool(object):
         last ks codes.  An active stream that has not finished ran every step of the last call, so its tail row ends at
         its last sample."""
         stores = [torch.empty(self._park_bytes, dtype=torch.uint8, device=self.device) for _ in park]
+        if self.kernel == "warp":
+            self._move(lib, [(self._row(s), ptr(q), r) for (s, _, r), q in zip(park, stores)])
+        else:
+            self._bf16_park(lib, park, stores)
+        tails = self._tail.index_select(0, _pinned_int32([s for s, _, _ in park], self.device).long())
+        for k, (_, st, _) in enumerate(park):
+            self._parked[st.sid] = (stores[k], tails[k])
+
+    def _bf16_park(self, lib, park, stores):
         for k0 in range(0, len(park), POOL_ADMIT_ROWS):
             part = park[k0:k0 + POOL_ADMIT_ROWS]
             n = len(part)
@@ -1208,14 +1269,19 @@ class DecodePool(object):
                                                 (ctypes.c_int32 * n)(*[r for _, _, r in part]), n, self.R, self.ks,
                                                 self.dil, self.L, stream()),
                   "decode_bf16_pool_park")
-        tails = self._tail.index_select(0, _pinned_int32([s for s, _, _ in park], self.device).long())
-        for k, (_, st, _) in enumerate(park):
-            self._parked[st.sid] = (stores[k], tails[k])
 
     def _unpark(self, lib, resume):
         """Copy the resumed streams' stores into their new rows (one launch per POOL_ADMIT_ROWS streams) and restore
         their last ks codes."""
         kept = [self._parked.pop(st.sid) for _, st, _ in resume]
+        if self.kernel == "warp":
+            self._move(lib, [(ptr(q), self._row(s), r) for (s, _, r), (q, _) in zip(resume, kept)])
+        else:
+            self._bf16_unpark(lib, resume, kept)
+        self._tail.index_copy_(0, _pinned_int32([s for s, _, _ in resume], self.device).long(),
+                               torch.stack([t for _, t in kept]))
+
+    def _bf16_unpark(self, lib, resume, kept):
         for k0 in range(0, len(resume), POOL_ADMIT_ROWS):
             part = resume[k0:k0 + POOL_ADMIT_ROWS]
             n = len(part)
@@ -1225,8 +1291,21 @@ class DecodePool(object):
                                                   (ctypes.c_int32 * n)(*[r for _, _, r in part]), n, self.R, self.ks,
                                                   self.dil, self.L, stream()),
                   "decode_bf16_pool_unpark")
-        self._tail.index_copy_(0, _pinned_int32([s for s, _, _ in resume], self.device).long(),
-                               torch.stack([t for _, t in kept]))
+
+    def _row(self, slot):
+        """Device address of pool row ``slot``'s queue block (fp32 pool)."""
+        return ptr(self.queues) + slot * self._block
+
+    def _move(self, lib, moves):
+        """``wnb_decode_pool_move`` of ``(src, dst, rotation)`` queue blocks, one launch per POOL_ADMIT_ROWS moves."""
+        for k0 in range(0, len(moves), POOL_ADMIT_ROWS):
+            part = moves[k0:k0 + POOL_ADMIT_ROWS]
+            n = len(part)
+            check(lib.wnb_decode_pool_move((ctypes.c_void_p * n)(*[s for s, _, _ in part]),
+                                           (ctypes.c_void_p * n)(*[d for _, d, _ in part]),
+                                           (ctypes.c_int32 * n)(*[r for _, _, r in part]), n, self.R, self.ks, self.dil,
+                                           self.L, stream()),
+                  "decode_pool_move")
 
     def _call(self, max_samples):
         """One pool call: (PoolCall, (capacity, n) int32 codes of steps g0 .. g0 + n - 1), or (None, None)."""
@@ -1267,11 +1346,18 @@ class DecodePool(object):
         xs = torch.empty(C, ks + n, dtype=torch.int32, device=self.device)
         xs[:, :ks] = self._tail
         w, g0 = self.w, call.g0
-        check(lib.wnb_decode_bf16_at(ptr(xs), ptr(aux), None, None, ptr(w["wf"]), ptr(w["bf"]), ptr(self.wstream),
-                                     self.dil, self.L, ptr(self.queues), ptr(tab[4]), ptr(uni), None, C, 1, n, 0, n,
-                                     self.Q, A, self.Ap, self.R, self.S, ks, 0, self.mode, self.seed, g0, g0 - (ks - 1),
-                                     g0, st_),
-              "decode_bf16_at")
+        if self.kernel == "warp":
+            check(lib.wnb_decode_warp_at(ptr(xs), ptr(aux), None, None, ptr(w["wf"]), ptr(w["bf"]), ptr(self.wstream),
+                                         ptr(w["b1"]), ptr(w["b2"]), ptr(w["bp1"]), ptr(w["bp2"]), self.dil, self.L,
+                                         ptr(self.queues), ptr(tab[4]), ptr(uni), None, C, 1, n, 0, n, A, 0, self.mode,
+                                         self.seed, self.W, self.CL, g0, g0 - (ks - 1), g0, st_),
+                  "decode_warp_at")
+        else:
+            check(lib.wnb_decode_bf16_at(ptr(xs), ptr(aux), None, None, ptr(w["wf"]), ptr(w["bf"]), ptr(self.wstream),
+                                         self.dil, self.L, ptr(self.queues), ptr(tab[4]), ptr(uni), None, C, 1, n, 0, n,
+                                         self.Q, A, self.Ap, self.R, self.S, ks, 0, self.mode, self.seed, g0,
+                                         g0 - (ks - 1), g0, st_),
+                  "decode_bf16_at")
         self._tail = xs[:, n:].contiguous()
         # frames before each stream's next sample are no longer needed
         for slot, st, f0, f1 in spans:
@@ -1664,12 +1750,13 @@ class WaveNet(nn.Module):
             return DecodeSession(self, x, n_samples_list, mode, seed)
 
     def decode_pool(self, capacity=64, mode="sampling", seed=None, park_below=None):
-        """Start a continuous-batching decode pool of ``capacity`` rows on the bf16 decoder (``decode_math="bf16"``):
-        ``admit`` streams at any time, ``feed`` their aux frames and ``step`` to decode; a stream takes a free row as
-        soon as its first frames arrive and leaves it when it finishes or is cancelled.  Stream k of a pool with
-        ``seed`` S decodes what row k of a one-shot bf16 decode with seed S decodes, bit for bit (``DecodePool``).  The
-        pool runs in lock step, unless ``park_below=m`` lets it park a stream that cannot run min(m, samples left)
-        samples until its frames arrive.  The pool snapshots the weights now; ``seed`` is drawn from torch's generator
-        when not given."""
+        """Start a continuous-batching decode pool of ``capacity`` rows, on the bf16 decoder under ``decode_math="bf16"``
+        and on the fp32 warp decoder under "fp32" (the 64 res / 512 skip, ks 2 shape; another shape raises
+        ``WnbError``): ``admit`` streams at any time, ``feed`` their aux frames and ``step`` to decode; a stream takes a
+        free row as soon as its first frames arrive and leaves it when it finishes or is cancelled.  Stream k of a pool
+        with ``seed`` S decodes what row k of a one-shot decode with seed S decodes, bit for bit: on the bf16 decoder,
+        and on the warp decoder for a one-shot batch of the pool's warp form (``DecodePool``).  The pool runs in lock
+        step, unless ``park_below=m`` lets it park a stream that cannot run min(m, samples left) samples until its frames
+        arrive.  The pool snapshots the weights now; ``seed`` is drawn from torch's generator when not given."""
         with torch.no_grad():
             return DecodePool(self, capacity, mode, seed, park_below)
