@@ -461,8 +461,12 @@ WNB_API int wnb_decode_at(int32_t* xs, const float* h, const float* up_w, const 
  * with cp.async.bulk while the consumer warps run the recurrence):
  *   per layer l: W1d [K1][O1] | W2res [R][Or] | W2skip [R][Os]   then  wp1d [S][Sp] | wp2d [S][Qp]
  * with O1 = 2R, Or = R, Os = Sp = S, Qp = Q each rounded up to a multiple of 4 (zero padded).
- * Returns WNB_ERR_UNSUPPORTED when the shape does not fit, before any device work (the caller may run wnb_decode_at). */
+ * Returns WNB_ERR_UNSUPPORTED when the shape does not fit, before any device work (the caller may run wnb_decode_at).
+ * wnb_decode_stream_supported answers the same question without a device: 1 when covered (every padded width fits the
+ * consumer threads and a 32 KB ring chunk, R, S and Ap are multiples of 4, L <= 64, and the work area of one utterance
+ * plus two ring slots fits shared memory), else 0.  Whether it is covered does not depend on B. */
 WNB_API size_t wnb_decode_stream_floats(int Q, int Ap, int R, int S, int ks, int L);
+WNB_API int wnb_decode_stream_supported(int Q, int Ap, int R, int S, int ks, int L);
 WNB_API int wnb_decode_stream_at(int32_t* xs, const float* h, const float* up_w, const float* up_b,
                                  const float* wf, const float* bf, const float* stream, const float* b1,
                                  const float* b2, const float* bp1, const float* bp2,
@@ -536,6 +540,23 @@ WNB_API int wnb_decode_warp_prefill(const int32_t* xs, const float* h, const flo
                                     const float* w2d, const float* b2, const int32_t* host_dilations, int L,
                                     void* queues, void* scratch, int B, int P, int n_pad, int Th, int A, int U, int CL,
                                     void* stream_handle);
+/* wnb_decode_stream_prefill: the same for the streaming decoder (csrc/decode_stream_prefill.cu).  After the call `queues`
+ * (the workspace of wnb_decode_stream_at, same B, wnb_decode_workspace() bytes) holds exactly what
+ * wnb_decode_stream_at(pos0 = 0) leaves there after the warm-up positions 0 .. P - 2, bit for bit; the caller then runs
+ * wnb_decode_stream_at with pos0 = P - 1, xs_base = 0, h_frame0 = 0 and the same xs, h, stream.  Slots of positions < 0
+ * are left as they are.
+ *   xs      (B, P) int32, the padded seed prefix;
+ *   h, up_w, up_b, wf, bf, b1, b2, n_pad, Th, Q, A, Ap, R, S, ks, U   as for wnb_decode_stream_at (h_frame0 = 0);
+ *   stream  the packed stream of wnb_decode_stream_at (its W1d and W2res are read), 16-byte aligned;
+ *   scratch wnb_decode_prefill_workspace(min(B, 64), P, R, ks, dilations, L) bytes: batches run in groups of at most 64
+ *           utterances (0 bytes, and scratch may be NULL, when P == 1 or ks == 1).
+ * Launches 1 + (L - 1) kernels per group of 64.  Covers every shape of wnb_decode_stream_supported and any dilations >= 1;
+ * WNB_ERR_UNSUPPORTED for another shape and WNB_ERR_INVALID for a bad shape or pointer, before any device work. */
+WNB_API int wnb_decode_stream_prefill(const int32_t* xs, const float* h, const float* up_w, const float* up_b,
+                                      const float* wf, const float* bf, const float* stream, const float* b1,
+                                      const float* b2, const int32_t* host_dilations, int L, void* queues,
+                                      void* scratch, int B, int P, int n_pad, int Th, int Q, int A, int Ap, int R,
+                                      int S, int ks, int U, void* stream_handle);
 /* wnb_decode_bf16_prefill: the same for the bf16 decoder (csrc/decode_bf16_prefill.cu).  After the call `queues` (the
  * workspace of wnb_decode_bf16_at, same B, wnb_decode_bf16_workspace() bytes) holds exactly what wnb_decode_bf16_at(pos0 = 0)
  * leaves there after the warm-up positions 0 .. P - 2, bit for bit, padding rows of each cluster included; the caller

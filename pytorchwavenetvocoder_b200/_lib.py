@@ -56,6 +56,7 @@ SIGNATURES = {
     "wnb_cross_entropy": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "wnb_decode_workspace": (_c.c_size_t, [_I, _I, _I, _P, _I]),
     "wnb_decode_stream_floats": (_c.c_size_t, [_I] * 6),
+    "wnb_decode_stream_supported": (_I, [_I] * 6),
     "wnb_decode_warp_floats": (_c.c_size_t, [_I, _I]),
     "wnb_decode_warp_set_timing": (None, [_P]),
     "wnb_decode_warp_supported": (_I, [_I] * 6),
@@ -72,6 +73,7 @@ SIGNATURES = {
     "wnb_decode_prefill_windows": (_I, [_P, _I, _I, _P]),
     "wnb_decode_prefill_workspace": (_c.c_size_t, [_I] * 4 + [_P, _I]),
     "wnb_decode_warp_prefill": (_I, [_P] * 11 + [_I] + [_P] * 2 + [_I] * 7 + [_P]),
+    "wnb_decode_stream_prefill": (_I, [_P] * 9 + [_P, _I] + [_P] * 2 + [_I] * 11 + [_P]),
     "wnb_decode_bf16_prefill_workspace": (_c.c_size_t, [_I] * 4 + [_P, _I]),
     "wnb_decode_bf16_prefill": (_I, [_P] * 7 + [_P, _I] + [_P] * 2 + [_I] * 10 + [_P]),
     "wnb_decode_bf16_pool_transplant": (_I, [_P, _I, _P, _P, _I, _P, _P] + [_I] * 3 + [_P, _I, _P]),

@@ -10,7 +10,8 @@ is ONE persistent-kernel launch (``WaveNet.batch_fast_generate``); like the refe
 "sampling".
 
 With ``--pool_capacity C`` each GPU worker instead decodes its whole file list through one continuous-batching pool
-of C rows (``WaveNet.decode_pool(C, "sampling")``, under either ``--decode_math``): files enter free rows longest
+of C rows (``WaveNet.decode_pool(C, "sampling")``, under either ``--decode_math``; under fp32 a model the warp decoder
+does not cover runs on the streaming decoder, ``kernel="stream"``): files enter free rows longest
 first as others finish, so no row idles until the longest file of a batch ends.  The stream id of a file is its index
 in the worker's list and the pool seed is ``pool_seed(--seed, gpu)``; each ``{feat_id}.wav`` holds exactly the samples
 the pool API gives for the same model, seed and features (``decode_pool_files``).
@@ -32,6 +33,7 @@ from sklearn.preprocessing import StandardScaler
 from pytorchwavenetvocoder_b200.nets import decode_mu_law
 from pytorchwavenetvocoder_b200.nets import encode_mu_law
 from pytorchwavenetvocoder_b200.nets import WaveNet
+from pytorchwavenetvocoder_b200.nets.wavenet import warp_pool_supported
 from pytorchwavenetvocoder_b200.utils import extend_time
 from pytorchwavenetvocoder_b200.utils import find_files
 from pytorchwavenetvocoder_b200.utils import read_hdf5
@@ -159,9 +161,18 @@ def pool_seed(seed, gpu):
     return int(torch.empty((), dtype=torch.int64).random_().item())
 
 
-def decode_pool_files(model, frames, capacity, seed, load, paths, fs, n_quantize, pcm16, shaping=None):
-    """Decode files 0 .. len(frames) - 1 through one ``model.decode_pool(capacity, "sampling", seed)`` and append each
-    stream's samples to its wav (``paths[i]``) as calls return them; a writer closes when its stream finishes.
+def pool_kernel_for(model, capacity):
+    """The decoder of ``--pool_capacity``: "stream" under fp32 when the warp decoder does not cover the model, else
+    "auto" (the warp decoder under fp32, the bf16 decoder under bf16)."""
+    if getattr(model, "decode_math", "fp32") == "fp32" and not warp_pool_supported(model, capacity):
+        return "stream"
+    return "auto"
+
+
+def decode_pool_files(model, frames, capacity, seed, load, paths, fs, n_quantize, pcm16, shaping=None, kernel="auto"):
+    """Decode files 0 .. len(frames) - 1 through one ``model.decode_pool(capacity, "sampling", seed, kernel=kernel)``
+    and append each stream's samples to its wav (``paths[i]``) as calls return them; a writer closes when its stream
+    finishes.
 
     ``load(i)`` -> (h (n_aux, frames) on the GPU, n_samples) reads file i; the stream id is i.  Files are admitted
     longest first (``frames[i]`` from the file shapes) and loaded lazily: at most 2 * capacity streams are admitted and
@@ -170,7 +181,7 @@ def decode_pool_files(model, frames, capacity, seed, load, paths, fs, n_quantize
     with ``shaping`` = (coef, alpha), through one ``MlsaStreamFilter`` keyed by stream id); otherwise ``decode_mu_law``
     and the wav writer's quantisation."""
     order = iter(sorted(range(len(frames)), key=lambda i: (-frames[i], i)))
-    pool = model.decode_pool(capacity, "sampling", seed)
+    pool = model.decode_pool(capacity, "sampling", seed, kernel=kernel)
     filt = MlsaStreamFilter(shaping[0], shaping[1], 4) if shaping is not None else None
     x = torch.full((1,), int(encode_mu_law(np.zeros(1), n_quantize)[0]), dtype=torch.int64, device="cuda")
     writers = {}
@@ -323,7 +334,7 @@ def gpu_decode(feat_list, gpu, args, config):
                          for f in feat_list]
                 shaping = _restoration_filter(args.stats) if getattr(args, "noise_shaping", False) else None
                 decode_pool_files(model, frames, capacity, seed, load, paths, args.fs, config.n_quantize,
-                                  not have_soundfile(), shaping)
+                                  not have_soundfile(), shaping, pool_kernel_for(model, capacity))
                 return
             generator = decode_generator(
                 feat_list,

@@ -400,27 +400,47 @@ static size_t stream_work_floats(int NU, int R, int S, int Qp, int Ap, int ks, i
   return (size_t)NU * (K1 + 2 * R + 2 * S + Qp + Ap + (size_t)(ks - 1) * L * R + omax);
 }
 
-// returns WNB_ERR_UNSUPPORTED when the shape does not fit this kernel (the caller may run wnb_decode_at instead)
-int decode_stream_launch(StreamParams& p, cudaStream_t st) {
-  const int widths[5] = {p.O1, p.Or, p.Os, p.Sp, p.Qp};
+// The streaming kernel's coverage and shared-memory rule: every padded width fits the consumer threads and a ring chunk,
+// L <= kMaxLayersS, R, S and Ap are multiples of 4, and the work area of NU utterances plus at least two ring slots fits
+// shared memory (NU halves down to 1 until it does).  Returns the ring slots (2 .. 6) with *NU and *work set, or 0 when
+// the shape is not covered.
+static int stream_plan(int Q, int Ap, int R, int S, int ks, int L, int NU, int* NU_out, size_t* work_out) {
+  const int O1 = (2 * R + 3) & ~3, Or = (R + 3) & ~3, Os = (S + 3) & ~3, Sp = Os, Qp = (Q + 3) & ~3;
+  const int widths[5] = {O1, Or, Os, Sp, Qp};
   for (int i = 0; i < 5; i++)
-    if (widths[i] % 4 != 0 || widths[i] / 4 > kConsThreads || widths[i] * 4 > kChunkBytes) return WNB_ERR_UNSUPPORTED;
-  if (p.L > kMaxLayersS || p.R % 4 != 0 || p.S % 4 != 0 || p.Ap % 4 != 0) return WNB_ERR_UNSUPPORTED;
-  int NU = 1;
-  if (p.B > device_sms() * 2) NU = 4; else if (p.B > device_sms()) NU = 2;
-  size_t work = 0, smem = 0;
+    if (widths[i] % 4 != 0 || widths[i] / 4 > kConsThreads || widths[i] * 4 > kChunkBytes) return 0;
+  if (L > kMaxLayersS || R % 4 != 0 || S % 4 != 0 || Ap % 4 != 0) return 0;
+  size_t work = 0;
   int nslot = 0;
   for (;;) {
-    work = stream_work_floats(NU, p.R, p.S, p.Qp, p.Ap, p.ks, p.L, p.O1, p.Os, p.Sp) * sizeof(float);
+    work = stream_work_floats(NU, R, S, Qp, Ap, ks, L, O1, Os, Sp) * sizeof(float);
     const size_t avail = 227 * 1024 - 64 - work - 16 * 16;
     nslot = work + 2 * kChunkBytes + 512 > 227 * 1024 ? 0 : (int)(avail / kChunkBytes);
     if (nslot > 6) nslot = 6;
     if (nslot >= 2 || NU == 1) break;
     NU >>= 1;
   }
+  if (nslot < 2) return 0;
+  *NU_out = NU;
+  *work_out = work;
+  return nslot;
+}
+
+int decode_stream_supported_shape(int Q, int Ap, int R, int S, int ks, int L) {
+  int NU = 1;
+  size_t work = 0;
+  return Q > 0 && Ap > 0 && R > 0 && S > 0 && ks >= 1 && L >= 1 && stream_plan(Q, Ap, R, S, ks, L, 1, &NU, &work) > 0;
+}
+
+// returns WNB_ERR_UNSUPPORTED when the shape does not fit this kernel (the caller may run wnb_decode_at instead)
+int decode_stream_launch(StreamParams& p, cudaStream_t st) {
+  int NU = 1;
+  if (p.B > device_sms() * 2) NU = 4; else if (p.B > device_sms()) NU = 2;
+  size_t work = 0;
+  const int nslot = stream_plan(p.Q, p.Ap, p.R, p.S, p.ks, p.L, NU, &NU, &work);
   if (nslot < 2) return WNB_ERR_UNSUPPORTED;
   p.nslot = nslot;
-  smem = (size_t)nslot * kChunkBytes + 2 * nslot * sizeof(uint64_t) + work;
+  const size_t smem = (size_t)nslot * kChunkBytes + 2 * nslot * sizeof(uint64_t) + work;
   const int grid = cdiv(p.B, NU);
 #define WNB_LAUNCH_STREAM(N)                                                                                     \
   do {                                                                                                           \
@@ -446,6 +466,11 @@ WNB_API size_t wnb_decode_stream_floats(int Q, int Ap, int R, int S, int ks, int
   const size_t O1 = (2 * R + 3) & ~3, Or = (R + 3) & ~3, Os = (S + 3) & ~3, Sp = Os, Qp = (Q + 3) & ~3;
   const size_t K1 = (size_t)ks * R + Ap;
   return (size_t)L * (K1 * O1 + (size_t)R * Or + (size_t)R * Os) + (size_t)S * Sp + (size_t)S * Qp;
+}
+
+// 1 when wnb_decode_stream_at covers the configuration, else 0 (no device needed).
+WNB_API int wnb_decode_stream_supported(int Q, int Ap, int R, int S, int ks, int L) {
+  return decode_stream_supported_shape(Q, Ap, R, S, ks, L);
 }
 
 WNB_API int wnb_decode_stream_at(int32_t* xs, const float* h, const float* up_w, const float* up_b, const float* wf,

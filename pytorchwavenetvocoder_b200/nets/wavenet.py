@@ -677,6 +677,24 @@ def _bf16_prefill(lib, xs, P, h, upw, upb, w, wstream, dil, L, queues, n_pad, A,
           "decode_bf16_prefill")
 
 
+# utterances one streaming-decoder prefill launch sequence takes at most: the library groups larger batches, so the
+# scratch stays at 2 * 64 * R * min(S_0, P - 1) floats
+STREAM_PREFILL_ROWS = 64
+
+
+def _stream_prefill(lib, xs, P, h, upw, upb, w, wstream, dil, L, queues, n_pad, Q, A, Ap, R, S, ks, U):
+    """Run the warm-up positions 0 .. P - 2 of ``wnb_decode_stream_at`` in parallel over time
+    (wnb_decode_stream_prefill): the queues then hold what the sequential warm-up leaves there, and
+    ``wnb_decode_stream_at`` continues from P - 1."""
+    B = xs.size(0)
+    nbytes = lib.wnb_decode_prefill_workspace(min(B, STREAM_PREFILL_ROWS), P, R, ks, dil, L)
+    scratch = torch.empty(nbytes // 4, dtype=torch.float32, device=xs.device) if nbytes else None
+    check(lib.wnb_decode_stream_prefill(ptr(xs[:, :P].contiguous()), ptr(h), ptr(upw), ptr(upb), ptr(w["wf"]),
+                                        ptr(w["bf"]), ptr(wstream), ptr(w["b1"]), ptr(w["b2"]), dil, L, ptr(queues),
+                                        ptr(scratch), B, P, n_pad, h.size(2), Q, A, Ap, R, S, ks, U, stream()),
+          "decode_stream_prefill")
+
+
 class DecodeSession(object):
     """A resumable decode of a batch of utterances, fed with aux frames as they arrive (``WaveNet.decode_session``).
 
@@ -706,8 +724,6 @@ class DecodeSession(object):
             raise ValueError("unknown decode kernel %r" % (kernel,))
         if kernel == "auto" and decode_math == "bf16":
             kernel = "bf16"
-        # fp32 "auto" only: the streaming kernel finds out at its first launch whether it covers the shape
-        self._stream_fallback = kernel == "auto"
         self.device = dev = x.device
         B, T0 = x.shape
         self.totals = [int(n) for n in n_samples_list]
@@ -737,7 +753,7 @@ class DecodeSession(object):
                 elif kernel == "warp":
                     raise _lib.WnbError("decode kernel 'warp' does not cover this configuration")
                 else:
-                    kernel = "stream"
+                    kernel = "stream" if lib.wnb_decode_stream_supported(Q, Ap, R, S, ks, L) else "direct"
             if kernel == "warp":
                 self.W, self.CL = lib.wnb_decode_warp_plan(B), lib.wnb_decode_warp_cluster(B)
                 self.wstream = net._decode_warp_pack(self.W, self.CL)
@@ -745,6 +761,10 @@ class DecodeSession(object):
             elif kernel == "stream":
                 self.wstream = net._decode_stream_pack(self.w)
                 assert self.wstream.numel() == lib.wnb_decode_stream_floats(Q, Ap, R, S, ks, L)
+                # the parallel warm-up serves the models the streaming decoder runs by default, every fp32 shape outside
+                # the warp decoder; on a shape the warp decoder covers, "stream" runs only when named, and stays the
+                # one-launch sequential decode that cross-checks the other decoders
+                self._parallel_warmup = not lib.wnb_decode_warp_supported(Q, Ap, R, S, ks, L)
             qbytes = lib.wnb_decode_workspace(B, R, ks, self.dil, L)
         self.kernel = kernel
         self.queues = torch.empty(max(qbytes // 4, 1), dtype=torch.float32, device=dev)
@@ -819,22 +839,21 @@ class DecodeSession(object):
                                         ptr(self.wstream), ptr(w["b1"]), ptr(w["b2"]), ptr(w["bp1"]), ptr(w["bp2"]),
                                         self.dil, self.L, ptr(self.queues), ptr(nsm), ptr(uni), ptr(lg), *common, self.A,
                                         self.U, self.mode, self.seed, self.W, self.CL, *window)
+        elif self.kernel == "stream":
+            if win.pos0 == 0 and self._parallel_warmup:   # the warm-up in parallel over time, then this call from P - 1
+                _stream_prefill(lib, xs, self.P, h, self.upw, self.upb, w, self.wstream, self.dil, self.L, self.queues,
+                                self.n_pad, Q, self.A, self.Ap, self.R, self.S, self.ks, self.U)
+                window = (self.P - 1, 0, 0, st)
+            rc = lib.wnb_decode_stream_at(ptr(xs), ptr(h), ptr(self.upw), ptr(self.upb), ptr(w["wf"]), ptr(w["bf"]),
+                                          ptr(self.wstream), ptr(w["b1"]), ptr(w["b2"]), ptr(w["bp1"]), ptr(w["bp2"]),
+                                          self.dil, self.L, ptr(self.queues), ptr(nsm), ptr(uni), ptr(lg), *common, Q,
+                                          self.A, self.Ap, self.R, self.S, self.ks, self.U, self.mode, self.seed, *window)
         else:
-            rc = -3
-            if self.kernel == "stream":
-                rc = lib.wnb_decode_stream_at(ptr(xs), ptr(h), ptr(self.upw), ptr(self.upb), ptr(w["wf"]), ptr(w["bf"]),
-                                              ptr(self.wstream), ptr(w["b1"]), ptr(w["b2"]), ptr(w["bp1"]),
-                                              ptr(w["bp2"]), self.dil, self.L, ptr(self.queues), ptr(nsm), ptr(uni),
-                                              ptr(lg), *common, Q, self.A, self.Ap, self.R, self.S, self.ks, self.U,
-                                              self.mode, self.seed, *window)
-                if rc == -3 and self._stream_fallback and win.pos0 == 0:   # shape outside the streaming kernel
-                    self.kernel = "direct"
-            if self.kernel == "direct":
-                rc = lib.wnb_decode_at(ptr(xs), ptr(h), ptr(self.upw), ptr(self.upb), ptr(w["wf"]), ptr(w["bf"]),
-                                       ptr(w["w1d"]), ptr(w["b1"]), ptr(w["w2d"]), ptr(w["b2"]), ptr(w["wp1d"]),
-                                       ptr(w["bp1"]), ptr(w["wp2d"]), ptr(w["bp2"]), self.dil, self.L, ptr(self.queues),
-                                       ptr(nsm), ptr(uni), ptr(lg), *common, Q, self.A, self.Ap, self.R, self.S, self.ks,
-                                       self.U, self.mode, self.seed, *window)
+            rc = lib.wnb_decode_at(ptr(xs), ptr(h), ptr(self.upw), ptr(self.upb), ptr(w["wf"]), ptr(w["bf"]),
+                                   ptr(w["w1d"]), ptr(w["b1"]), ptr(w["w2d"]), ptr(w["b2"]), ptr(w["wp1d"]),
+                                   ptr(w["bp1"]), ptr(w["wp2d"]), ptr(w["bp2"]), self.dil, self.L, ptr(self.queues),
+                                   ptr(nsm), ptr(uni), ptr(lg), *common, Q, self.A, self.Ap, self.R, self.S, self.ks,
+                                   self.U, self.mode, self.seed, *window)
         check(rc, "decode_%s_at" % self.kernel)
         self._xs, self._xs_base = xs, win.xs_base
         self.pos = win.end
@@ -1026,6 +1045,15 @@ class PoolSchedule(object):
         return PoolCall(g0, n, admit, rows, finished, park_calls, resume_calls)
 
 
+def warp_pool_supported(net, capacity):
+    """True when the fp32 warp decoder covers ``net`` at a pool of ``capacity`` rows (``warp_pool_form`` would not
+    raise)."""
+    lib = _lib.load()
+    Q, Ap, R, S, ks, L = (net.n_quantize, net.n_aux_pad, net.n_resch, net.n_skipch, net.kernel_size, len(net.dilations))
+    return bool(lib.wnb_decode_warp_supported(Q, Ap, R, S, ks, L)
+                and lib.wnb_decode_warp_form(capacity, L, (ctypes.c_int32 * 4)()) == 0)
+
+
 def warp_pool_form(net, capacity):
     """(NU, W, CL): the form ``wnb_decode_warp_at`` runs for a pool of ``capacity`` rows on the fp32 warp decoder
     (``wnb_decode_warp_form``).  The thresholds are the library's and follow the device's SM count: on a 132-SM H100 one
@@ -1039,8 +1067,25 @@ def warp_pool_form(net, capacity):
         raise _lib.WnbError("decode_math='fp32' pools run the warp decoder, which does not cover this model (n_quantize "
                             "%d, n_aux %d, n_resch %d, n_skipch %d, kernel_size %d, %d layers) at capacity %d: it covers "
                             "n_quantize 256, n_aux <= 32, n_resch 64, n_skipch 512, kernel_size 2; decode_math='bf16' "
-                            "pools cover the recipe sizes" % (Q, A, R, S, ks, L, capacity))
+                            "pools cover the recipe sizes, and kernel='stream' runs an fp32 pool on the streaming "
+                            "decoder" % (Q, A, R, S, ks, L, capacity))
     return form[0], form[1], form[2]
+
+
+def pool_kernel(decode_math, kernel):
+    """The decoder a ``DecodePool`` runs: "auto" is "bf16" under ``decode_math="bf16"`` and "warp" under "fp32"; a named
+    kernel must belong to the pool's math ("bf16" to bf16, "warp" and "stream" to fp32).  Raises ``WnbError``
+    otherwise."""
+    if decode_math not in ("fp32", "bf16"):
+        raise _lib.WnbError("decode pools run the bf16 decoder (decode_math='bf16') or an fp32 decoder "
+                            "(decode_math='fp32'), got %r" % (decode_math,))
+    if kernel == "auto":
+        return "bf16" if decode_math == "bf16" else "warp"
+    if kernel not in ("warp", "stream", "bf16"):
+        raise ValueError("unknown decode pool kernel %r: 'auto', 'warp', 'stream' or 'bf16'" % (kernel,))
+    if (kernel == "bf16") != (decode_math == "bf16"):
+        raise _lib.WnbError("decode pool kernel %r does not run decode_math=%r" % (kernel, decode_math))
+    return kernel
 
 
 def _pinned_int32(values, dev):
@@ -1052,7 +1097,8 @@ class DecodePool(object):
     """Continuous batching (``WaveNet.decode_pool``): streams join a free row of a running batch and leave it the moment
     they finish, so requests that arrive at different times share one weight read.  Under ``decode_math="bf16"`` the
     pool runs the bf16 decoder, under "fp32" the fp32 warp decoder (``warp_pool_form``: the BASELINE shape, 64 res /
-    512 skip, ks 2; another shape raises ``WnbError``).
+    512 skip, ks 2; another shape raises ``WnbError``), or with ``kernel="stream"`` the fp32 streaming decoder, which
+    covers every shape ``wnb_decode_stream_supported`` accepts (``pool_kernel``).
 
     The pool is one decoder batch of ``capacity`` rows (``wnb_decode_bf16_at`` or ``wnb_decode_warp_at``), launched once
     per ``step`` over the pool's global steps g0 .. g0 + n - 1 with P = 1, n_pad = 0, U = 0 (include/wnb200.h, DESIGN
@@ -1063,7 +1109,10 @@ class DecodePool(object):
     Stream k of a bf16 pool with seed S decodes exactly what row k of ``net._decode(X, H, n_list, mode, seed=S,
     kernel="bf16")`` decodes, bit for bit.  Stream k of an fp32 pool with seed S decodes what row k of
     ``net._decode(X, H, n_list, mode, seed=S, kernel="warp")`` decodes, bit for bit, for a one-shot batch whose warp form
-    (``wnb_decode_warp_form``: NU, W, CL) equals the pool's: the form sets the order of some fp32 sums.
+    (``wnb_decode_warp_form``: NU, W, CL) equals the pool's: the form sets the order of some fp32 sums.  On
+    ``kernel="stream"`` (admission: ``wnb_decode_stream_prefill`` and ``wnb_decode_pool_move``) stream k equals row k of
+    ``net._decode(X, H, n_list, mode, seed=S, kernel="stream")`` for any one-shot batch size: the streaming decoder's sums
+    do not depend on its launch form.
 
     ``step`` runs one launch for every row.  By default (``park_below=None``) it advances in lock step: a stream whose
     aux frames have not arrived holds back the whole launch (the call runs only what that stream can run, and nothing if
@@ -1076,23 +1125,21 @@ class DecodePool(object):
     keeps a slow stream from cutting every call short.  ``cancel`` drops a stream at once.  The pool snapshots the
     weights at its creation."""
 
-    def __init__(self, net, capacity=64, mode="sampling", seed=None, park_below=None):
+    def __init__(self, net, capacity=64, mode="sampling", seed=None, park_below=None, kernel="auto"):
         if mode not in ("sampling", "argmax"):
             raise ValueError("mode should be sampling or argmax, got %r" % (mode,))
         capacity = int(capacity)
         if capacity < 1:
             raise ValueError("a decode pool needs a capacity of at least 1, got %d" % capacity)
-        decode_math = getattr(net, "decode_math", "fp32")
-        if decode_math not in ("fp32", "bf16"):
-            raise _lib.WnbError("decode pools run the bf16 decoder (decode_math='bf16') or the fp32 warp decoder "
-                                "(decode_math='fp32'), got %r" % (decode_math,))
+        kernel = pool_kernel(getattr(net, "decode_math", "fp32"), kernel)
         lib = _lib.load()
         self.device = dev = _device()
         self.Q, self.A, self.Ap, self.R, self.S, self.ks, self.U = (
             net.n_quantize, net.n_aux, net.n_aux_pad, net.n_resch, net.n_skipch, net.kernel_size, net.upsampling_factor)
         self.rf, self.L, self.capacity = net.receptive_field, len(net.dilations), capacity
         self.dil = (ctypes.c_int32 * self.L)(*net.dilations)
-        self.kernel = "bf16" if decode_math == "bf16" else "warp"
+        self.kernel = kernel
+        self.w, self.upw, self.upb = _decode_snapshot(net)
         g_base = None
         if self.kernel == "bf16":
             self.wstream = _bf16_weight_stream(lib, net)
@@ -1100,15 +1147,23 @@ class DecodePool(object):
             admit_bytes = lib.wnb_decode_bf16_workspace(POOL_ADMIT_ROWS, self.R, self.ks, self.dil, self.L)
             self._park_bytes = lib.wnb_decode_bf16_park_bytes(self.R, self.ks, self.dil, self.L)
         else:
-            _, self.W, self.CL = warp_pool_form(net, capacity)
-            self.wstream = net._decode_warp_pack(self.W, self.CL)
-            assert self.wstream.numel() == lib.wnb_decode_warp_floats(self.L, self.CL)
+            if self.kernel == "warp":
+                _, self.W, self.CL = warp_pool_form(net, capacity)
+                self.wstream = net._decode_warp_pack(self.W, self.CL)
+                assert self.wstream.numel() == lib.wnb_decode_warp_floats(self.L, self.CL)
+            else:
+                if not lib.wnb_decode_stream_supported(self.Q, self.Ap, self.R, self.S, self.ks, self.L):
+                    raise _lib.WnbError("kernel='stream' pools run the streaming decoder, which does not cover this "
+                                        "model (n_quantize %d, n_aux %d, n_resch %d, n_skipch %d, kernel_size %d, %d "
+                                        "layers)" % (self.Q, self.A, self.R, self.S, self.ks, self.L))
+                self.wstream = net._decode_stream_pack(self.w)
+                assert self.wstream.numel() == lib.wnb_decode_stream_floats(self.Q, self.Ap, self.R, self.S, self.ks,
+                                                                            self.L)
             # one utterance's queue block: a pool row, a row of the admission workspace and a parked stream's store
             self._block = lib.wnb_decode_workspace(1, self.R, self.ks, self.dil, self.L)
             qbytes, admit_bytes, self._park_bytes = capacity * self._block, POOL_ADMIT_ROWS * self._block, self._block
             # the fp32 decoders read layer l's tap only at positions >= d_l (a zero before): keep g at or above that
             g_base = (self.ks - 1) * max(net.dilations)
-        self.w, self.upw, self.upb = _decode_snapshot(net)
         self.mode = MODE_ARGMAX if mode == "argmax" else MODE_SAMPLING
         if seed is None:
             seed = int(torch.empty((), dtype=torch.int64).random_().item())  # follows torch.manual_seed, like _decode
@@ -1227,10 +1282,14 @@ class DecodePool(object):
         xs[:, n_pad:] = torch.stack([self._x.pop(st.sid) for st in group])
         Fg = min(self._h[st.sid][0].size(1) for st in group)
         h = torch.stack([self._h[st.sid][0][:, :Fg] for st in group]).contiguous()
-        if self.kernel == "warp":
-            # the pool's CL, not the group's: the 2-CTA form sums half of the residual products in another order
-            _warp_prefill(lib, xs, P, h, self.upw, self.upb, self.w, self.dil, self.L, self._admit_queues, n_pad, self.A,
-                          self.U, self.CL)
+        if self.kernel != "bf16":
+            if self.kernel == "warp":
+                # the pool's CL, not the group's: the 2-CTA form sums half of the residual products in another order
+                _warp_prefill(lib, xs, P, h, self.upw, self.upb, self.w, self.dil, self.L, self._admit_queues, n_pad,
+                              self.A, self.U, self.CL)
+            else:
+                _stream_prefill(lib, xs, P, h, self.upw, self.upb, self.w, self.wstream, self.dil, self.L,
+                                self._admit_queues, n_pad, self.Q, self.A, self.Ap, self.R, self.S, ks, self.U)
             base = ptr(self._admit_queues)
             self._move(lib, [(base + k * self._block, self._row(st.slot), g0 - (P - 1)) for k, st in enumerate(group)])
             for k, st in enumerate(group):
@@ -1252,7 +1311,7 @@ class DecodePool(object):
         last ks codes.  An active stream that has not finished ran every step of the last call, so its tail row ends at
         its last sample."""
         stores = [torch.empty(self._park_bytes, dtype=torch.uint8, device=self.device) for _ in park]
-        if self.kernel == "warp":
+        if self.kernel != "bf16":
             self._move(lib, [(self._row(s), ptr(q), r) for (s, _, r), q in zip(park, stores)])
         else:
             self._bf16_park(lib, park, stores)
@@ -1274,7 +1333,7 @@ class DecodePool(object):
         """Copy the resumed streams' stores into their new rows (one launch per POOL_ADMIT_ROWS streams) and restore
         their last ks codes."""
         kept = [self._parked.pop(st.sid) for _, st, _ in resume]
-        if self.kernel == "warp":
+        if self.kernel != "bf16":
             self._move(lib, [(ptr(q), self._row(s), r) for (s, _, r), (q, _) in zip(resume, kept)])
         else:
             self._bf16_unpark(lib, resume, kept)
@@ -1352,6 +1411,13 @@ class DecodePool(object):
                                          ptr(self.queues), ptr(tab[4]), ptr(uni), None, C, 1, n, 0, n, A, 0, self.mode,
                                          self.seed, self.W, self.CL, g0, g0 - (ks - 1), g0, st_),
                   "decode_warp_at")
+        elif self.kernel == "stream":
+            check(lib.wnb_decode_stream_at(ptr(xs), ptr(aux), None, None, ptr(w["wf"]), ptr(w["bf"]), ptr(self.wstream),
+                                           ptr(w["b1"]), ptr(w["b2"]), ptr(w["bp1"]), ptr(w["bp2"]), self.dil, self.L,
+                                           ptr(self.queues), ptr(tab[4]), ptr(uni), None, C, 1, n, 0, n, self.Q, A,
+                                           self.Ap, self.R, self.S, ks, 0, self.mode, self.seed, g0, g0 - (ks - 1), g0,
+                                           st_),
+                  "decode_stream_at")
         else:
             check(lib.wnb_decode_bf16_at(ptr(xs), ptr(aux), None, None, ptr(w["wf"]), ptr(w["bf"]), ptr(self.wstream),
                                          self.dil, self.L, ptr(self.queues), ptr(tab[4]), ptr(uni), None, C, 1, n, 0, n,
@@ -1679,7 +1745,7 @@ class WaveNet(nn.Module):
 
     def _decode(self, x, h, n_samples_list, mode, uniforms=None, return_logits=False, seed=None, kernel="auto"):
         """Decode every sample at once: one call of a ``DecodeSession`` given all the aux frames, i.e. one launch over
-        positions 0 .. P - 1 + max_n - 1 (after the parallel warm-up on ``warp`` and ``bf16``).  Returns the (B, max_n)
+        positions 0 .. P - 1 + max_n - 1 (after the parallel warm-up on ``warp``, ``stream`` and ``bf16``).  Returns the (B, max_n)
         int32 codes, and the (B, max_n, Q) teacher-check logits with ``return_logits``; ``last_decode_kernel`` names the
         decoder that ran.  ``x`` may be on the CPU, ``h`` may not."""
         if not h.is_cuda:
@@ -1749,7 +1815,7 @@ class WaveNet(nn.Module):
         with torch.no_grad():
             return DecodeSession(self, x, n_samples_list, mode, seed)
 
-    def decode_pool(self, capacity=64, mode="sampling", seed=None, park_below=None):
+    def decode_pool(self, capacity=64, mode="sampling", seed=None, park_below=None, kernel="auto"):
         """Start a continuous-batching decode pool of ``capacity`` rows, on the bf16 decoder under ``decode_math="bf16"``
         and on the fp32 warp decoder under "fp32" (the 64 res / 512 skip, ks 2 shape; another shape raises
         ``WnbError``): ``admit`` streams at any time, ``feed`` their aux frames and ``step`` to decode; a stream takes a
@@ -1757,6 +1823,8 @@ class WaveNet(nn.Module):
         with ``seed`` S decodes what row k of a one-shot decode with seed S decodes, bit for bit: on the bf16 decoder,
         and on the warp decoder for a one-shot batch of the pool's warp form (``DecodePool``).  The pool runs in lock
         step, unless ``park_below=m`` lets it park a stream that cannot run min(m, samples left) samples until its frames
-        arrive.  The pool snapshots the weights now; ``seed`` is drawn from torch's generator when not given."""
+        arrive.  The pool snapshots the weights now; ``seed`` is drawn from torch's generator when not given.
+        ``kernel``: "auto" (the decoder of ``decode_math``), "warp", "bf16", or "stream" for an fp32 pool on the
+        streaming decoder (any shape it covers; bit-identical to one-shot ``kernel="stream"`` decoding)."""
         with torch.no_grad():
-            return DecodePool(self, capacity, mode, seed, park_below)
+            return DecodePool(self, capacity, mode, seed, park_below, kernel)
