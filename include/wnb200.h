@@ -411,6 +411,17 @@ WNB_API int wnb_post_bwd(const float* skip, const float* r1, const float* dlogit
  * dlogits (B,T,Q) may be NULL (loss only); rows t < start get zero gradient. */
 WNB_API int wnb_cross_entropy(const float* logits, const int64_t* target /*(B,T)*/, double* loss_sum,
                       float* dlogits, int B, int T, int Q, int start, void* stream);
+/* ---- held-out scoring (WaveNet.score, DESIGN.md section 6): per-row summed cross entropy, one launch, no atomics.
+ * For each row b, adds -log softmax(logits[b, t])[target[b, t]] over start <= t < min(lengths[b], T) to nll[b]
+ * (accumulated into; the caller zeroes it) and that number of positions to count[b] (may be NULL).  A row with
+ * lengths[b] <= start is left untouched.  The value of each position is the one wnb_cross_entropy computes (its Q == 256
+ * register path when logits is 16-byte aligned).  The row is summed in one order that depends on the row alone
+ * (csrc/score.cu): segments [32 j, 32 j + 32) of its columns, each summed as a fixed lane tree, then added to nll[b]
+ * in ascending j.  So a row's result does not depend on B, T beyond its length, the other rows or the run, and chaining
+ * calls over windows whose first column is a multiple of 32 reproduces one call over the whole row bit for bit. */
+WNB_API int wnb_cross_entropy_rows(const float* logits /*(B,T,Q)*/, const int64_t* target /*(B,T)*/,
+                                   const int64_t* lengths /*(B)*/, int start, double* nll /*(B)*/,
+                                   int64_t* count /*(B)*/, int B, int T, int Q, void* stream);
 
 /* ---- a14/a15/a16: persistent fast-generate kernels (wavenet.py:309-395, 397-511, 538-549) ----------------------------
  * Four decoders, one entry point each: wnb_decode_at (weights read directly from L2), wnb_decode_stream_at,

@@ -54,6 +54,7 @@ SIGNATURES = {
     "wnb_post_fwd": (_I, [_P] * 7 + [_I] * 6 + [_P]),
     "wnb_post_bwd": (_I, [_P] * 11 + [_I] * 5 + [_P]),
     "wnb_cross_entropy": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "wnb_cross_entropy_rows": (_I, [_P, _P, _P, _I, _P, _P, _I, _I, _I, _P]),
     "wnb_decode_workspace": (_c.c_size_t, [_I, _I, _I, _P, _I]),
     "wnb_decode_stream_floats": (_c.c_size_t, [_I] * 6),
     "wnb_decode_stream_supported": (_I, [_I] * 6),

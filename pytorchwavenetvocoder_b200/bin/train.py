@@ -211,7 +211,36 @@ def get_parser():
                              "tensor-core path covers")
     parser.add_argument("--host_loader", default=False, type=_strtobool,
                         help="(H100 build) build the mini-batches on the host like the reference instead of on the GPU")
+    parser.add_argument("--dev_waveforms", default=None, type=str, help="directory or list of held-out wav files")
+    parser.add_argument("--dev_feats", default=None, type=str, help="directory or list of held-out aux feat files")
+    parser.add_argument("--dev_interval", default=0, type=int,
+                        help="log the held-out loss (utils/scoring.py) every this many iterations and at the end "
+                             "(0: off)")
+    parser.add_argument("--dev_batch_samples", default=1 << 19, type=int,
+                        help="samples per held-out scoring batch (rows x longest row)")
     return parser
+
+
+def check_dev_args(args):
+    """Refusals of the held-out flags, before anything is written: an error message, or None."""
+    if (args.dev_waveforms is None) != (args.dev_feats is None):
+        return "--dev_waveforms and --dev_feats go together"
+    if args.dev_interval < 0:
+        return "--dev_interval should be 0 (off) or a positive number of iterations, got %d" % args.dev_interval
+    if args.dev_interval > 0 and args.dev_waveforms is None:
+        return "--dev_interval %d needs --dev_waveforms and --dev_feats" % args.dev_interval
+    if args.dev_batch_samples <= 0:
+        return "--dev_batch_samples should be positive, got %d" % args.dev_batch_samples
+    return None
+
+
+def dev_loss(model, utts, batch_samples):
+    """Held-out loss of this rank's share ``utts`` gathered over ranks in list order (``parallel.gather_scores``):
+    (Σ nll, Σ count, nats per sample), the same bits on any number of ranks.  Draws from no random generator."""
+    from pytorchwavenetvocoder_b200.parallel import gather_scores
+    from pytorchwavenetvocoder_b200.utils.scoring import corpus_mean, score_utterances
+    nll, count = score_utterances(model, utts, batch_samples)
+    return corpus_mean(*gather_scores(nll, count))
 
 
 def _strtobool(v):
@@ -253,6 +282,10 @@ def main():
     if args.n_gpus > 1 and world != args.n_gpus:
         logging.error("--n_gpus %d but WORLD_SIZE is %d (launch with `torchrun --nproc-per-node %d`)."
                       % (args.n_gpus, world, args.n_gpus))
+        sys.exit(1)
+    refusal = check_dev_args(args)
+    if refusal is not None:
+        logging.error(refusal)
         sys.exit(1)
     if args.batch_length > 0 and args.batch_size % world != 0:
         # --batch_size stays the GLOBAL batch (the reference scatters one batch over the GPUs, train.py:449-454)
@@ -369,6 +402,23 @@ def main():
         from pytorchwavenetvocoder_b200.parallel import GradAllReduce
         sync = GradAllReduce(model)
 
+    dev_utts = None
+    if args.dev_interval > 0:
+        # this rank's np.array_split share of the held-out list, aligned once (utils/scoring.py); scoring it draws from
+        # no random generator and leaves the training generator alone, so the checkpoints do not change
+        from pytorchwavenetvocoder_b200.bin.evaluate import file_lists
+        from pytorchwavenetvocoder_b200.parallel import shard_utterances
+        from pytorchwavenetvocoder_b200.utils.scoring import load_utterance
+        dev_wavs, dev_feats = file_lists(args.dev_waveforms, args.dev_feats)
+        dev_utts = [load_utterance(w, f, args, scaler) for w, f in
+                    zip(shard_utterances(dev_wavs, world, rank), shard_utterances(dev_feats, world, rank))]
+        logging.info("number of held-out data = %d." % len(dev_wavs))
+
+    def log_dev(it):
+        s_, n_, mean = dev_loss(model, dev_utts, args.dev_batch_samples)
+        if rank == 0:
+            logging.info("(iter:%d) dev loss = %.6f (%d samples)" % (it, mean, n_))
+
     loss = torch.zeros((), device="cuda")    # summed on the device: no host sync per step (reference :540 syncs)
     total = 0
     debug = logging.getLogger().isEnabledFor(logging.DEBUG)
@@ -406,7 +456,11 @@ def main():
 
         if (i + 1) % args.checkpoint_interval == 0 and rank == 0:
             save_checkpoint(args.expdir, model, optimizer, i + 1)
+        if dev_utts is not None and (i + 1) % args.dev_interval == 0:
+            log_dev(i + 1)
 
+    if dev_utts is not None and (args.iters <= iterations or args.iters % args.dev_interval != 0):
+        log_dev(max(args.iters, iterations))
     if rank == 0:
         torch.save({"model": model.state_dict()}, args.expdir + "/checkpoint-final.pkl")
         logging.info("final checkpoint created.")

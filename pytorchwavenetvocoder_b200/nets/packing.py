@@ -230,6 +230,14 @@ class StackPlan(object):
         return torch.from_numpy(arr.view(np.uint8).copy()).to(self.device)
 
     # ---------------------------------------------------------------------------------------------
+    def autograd_params(self):
+        """The parameters handed to ``_StackTrainFn.apply``: the modules' own under grad mode, detached views
+        otherwise.  ``Function.forward`` runs with grad mode off whatever the caller's, so it tells a no-grad call
+        (ping-ponged activations, nothing saved) from a training call by ``needs_input_grad`` alone."""
+        if torch.is_grad_enabled():
+            return [p for _, p in self.params]
+        return [p.detach() for _, p in self.params]
+
     def pack(self, stream):
         lib = _lib.load()
         _lib.check(lib.wnb_pack_weights(self.pack_table.data_ptr(), self.n_pack, None, self.pbuf.data_ptr(), None,

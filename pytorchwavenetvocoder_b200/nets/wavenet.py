@@ -1588,7 +1588,55 @@ class WaveNet(nn.Module):
         plan = self._stack_plan(x.device)
         if plan is None:
             return cross_entropy(self._forward_impl(x, h), t, start)
-        return _StackTrainFn.apply(self, plan, x, h, t, start, *[p for _, p in plan.params])
+        return _StackTrainFn.apply(self, plan, x, h, t, start, *plan.autograd_params())
+
+    def score(self, x, h, t, lengths, start=None, out=None):
+        """Teacher-forced negative log-likelihood of held-out utterances (DESIGN.md section 6, row e1).
+
+        ``x`` (B, T) int64 input codes, ``h`` the aux features of ``forward``, ``t`` (B, T) int64 next-sample targets
+        (``utils.scoring.utterance_arrays`` aligns them as the training batches are), ``lengths`` (B,) the number of
+        valid positions of each row (an int64 CUDA tensor, or a host sequence).  Scores positions ``start <= p <
+        lengths[b]``; ``start`` defaults to ``receptive_field``, the training loss's start, after which no position sees
+        the causal zero padding.
+
+        Runs the forward of the model's ``math_mode`` under ``no_grad`` (two ping-ponged activation buffers; under
+        fp32 and bf16 the weights are first packed with torch ops, as ``forward`` packs them), then one
+        ``wnb_cross_entropy_rows`` launch.  Returns ``(nll_sum float64 (B,), count int64 (B,))`` on the device, without
+        synchronising: the summed NLL in nats and the number of scored positions of each row (0, and nll 0, for a row
+        with no scored position).  A row's result is bit-identical whatever else is in the batch and however far it is
+        padded.  ``out`` = (nll, count): add into these instead of fresh zeroed tensors (a chain of window calls,
+        ``utils.scoring.score_windows``)."""
+        start = self.receptive_field if start is None else int(start)
+        if not x.is_cuda:
+            raise _lib.WnbError("WaveNet.score needs CUDA tensors: this build has no CPU fallback")
+        lib = _lib.load()
+        B, T = x.shape
+        dev = x.device
+        if not torch.is_tensor(lengths):
+            lengths = torch.tensor([int(v) for v in lengths], dtype=torch.int64).to(dev)
+        t = t.contiguous()
+        if (t.dtype != torch.int64 or tuple(t.shape) != (B, T) or t.device != dev or lengths.dtype != torch.int64
+                or tuple(lengths.shape) != (B,) or lengths.device != dev):
+            raise ValueError("score: t should be an int64 (B, T) = %s tensor and lengths an int64 (B,) tensor on %s"
+                             % ((B, T), dev))
+        if start < 0:
+            raise ValueError("score: start should be >= 0, got %d" % start)
+        st = stream()
+        if out is None:
+            nll = torch.empty(B, device=dev, dtype=torch.float64)
+            count = torch.empty(B, device=dev, dtype=torch.int64)
+            check(lib.wnb_zero(ptr(nll), 8 * B, st), "zero")
+            check(lib.wnb_zero(ptr(count), 8 * B, st), "zero")
+        else:
+            nll, count = out
+            if (nll.dtype != torch.float64 or count.dtype != torch.int64 or tuple(nll.shape) != (B,)
+                    or tuple(count.shape) != (B,) or nll.device != dev or count.device != dev):
+                raise ValueError("score: out should be a float64 and an int64 (B,) = (%d,) tensor on %s" % (B, dev))
+        with torch.no_grad():
+            logits = self._forward_impl(x, h)
+            check(lib.wnb_cross_entropy_rows(ptr(logits), ptr(t), ptr(lengths), start, ptr(nll), ptr(count), B, T,
+                                             self.n_quantize, st), "cross_entropy_rows")
+        return nll, count
 
     def _forward_impl(self, x, h, upsample=True):
         if not x.is_cuda:
@@ -1596,7 +1644,7 @@ class WaveNet(nn.Module):
         if upsample and PROFILE_EVENTS is None:
             plan = self._stack_plan(x.device)
             if plan is not None:
-                return _StackTrainFn.apply(self, plan, x, h, None, 0, *[p for _, p in plan.params])
+                return _StackTrainFn.apply(self, plan, x, h, None, 0, *plan.autograd_params())
         haux = self._aux(h, upsample)
         if haux.size(1) != x.size(1):
             raise ValueError("aux length %d does not match waveform length %d" % (haux.size(1), x.size(1)))

@@ -57,3 +57,15 @@ def shard_utterances(items, world, rank):
     """bin/decode.py:261-262: ``np.array_split(feat_list, n_gpus)`` -> this rank's slice (order kept)."""
     parts = np.array_split(np.arange(len(items)), world)
     return [items[i] for i in parts[rank]]
+
+
+def gather_scores(nll, count, group=None):
+    """Per-utterance held-out scores (``utils.scoring``) of every rank, concatenated in rank order on every rank.  Each
+    rank scored its ``shard_utterances`` share of one list, so the result is in list order and its ``corpus_mean`` is
+    bit-identical to scoring the whole list in one process.  Without a process group, returns the arguments."""
+    nll, count = np.asarray(nll, dtype=np.float64), np.asarray(count, dtype=np.int64)
+    if not dist.is_initialized():
+        return nll, count
+    parts = [None] * dist.get_world_size(group)
+    dist.all_gather_object(parts, (nll, count), group=group)
+    return np.concatenate([p[0] for p in parts]), np.concatenate([p[1] for p in parts])
