@@ -33,6 +33,7 @@ struct DecodeParams {
   int dil[kMaxLayers];
   long long qoff[kMaxLayers];  // float offset of layer l's ring inside one utterance's queue block
   long long q_per_utt;
+  int partial_pad;  // 0 .. 3 floats between qtap's end and the 16-byte aligned partial (decode_partial_offset)
 };
 
 __device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
@@ -137,7 +138,8 @@ __global__ void __launch_bounds__(kDecThreads) decode_kernel(const DecodeParams 
   const int R = p.R, S = p.S, Q = p.Q, Ap = p.Ap, ks = p.ks, L = p.L;
   const int K1 = ks * R + Ap;
   const int ntap = (ks - 1) * L;
-  // shared memory carve-up (floats)
+  // shared memory carve-up (floats).  Only `partial` is accessed as float4; it starts at a multiple of 4 floats (16
+  // bytes, decode_partial_offset).  The regions before it are read and written as scalars and may have any length.
   float* xcat = smem;                          // [NU][K1]
   float* cur = xcat + NU * K1;                 // [NU][R]
   float* zs = cur + NU * R;                    // [NU][R]
@@ -146,7 +148,7 @@ __global__ void __launch_bounds__(kDecThreads) decode_kernel(const DecodeParams 
   float* logit = h1 + NU * S;                  // [NU][Qp]
   float* hcol = logit + NU * p.Qp;             // [NU][Ap]
   float* qtap = hcol + NU * Ap;                // [NU][ntap][R]
-  float* partial = qtap + (size_t)NU * ntap * R;  // [parts][NU][O]  (>= NU*max(1024, Omax))
+  float* partial = qtap + (size_t)NU * ntap * R + p.partial_pad;  // [parts][NU][O]  (>= NU*max(1024, Omax))
   __shared__ int s_n[NU];
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -342,14 +344,27 @@ __global__ void __launch_bounds__(kDecThreads) decode_kernel(const DecodeParams 
   }
 }
 
+// decode_kernel's shared-memory carve-up, in floats: the scalar regions xcat .. qtap, then `partial`.
+// gemv_partial stores float4 at partial + (part * NU + u) * O with O a multiple of 4, so partial must start at a
+// multiple of 4 floats (16 bytes) from the 16-byte aligned base.  R and S need not be multiples of 4 on this kernel,
+// so the scalar regions can end at 2 or 3 mod 4 floats (Q 256, Ap 32, R 6, S 8, ks 2, L 3 gives 378 at NU 1).
+// partial's offset is rounded up to 4 floats and the kernel skips the difference (DecodeParams::partial_pad); the
+// launcher sizes shared memory from the same offset.
+static size_t decode_scalar_floats(int NU, int R, int S, int Qp, int Ap, int ks, int L) {
+  const size_t K1 = (size_t)ks * R + Ap;
+  return (size_t)NU * (K1 + 2 * (size_t)R + 2 * (size_t)S + Qp + Ap + (size_t)(ks - 1) * L * R);
+}
+static size_t decode_partial_offset(int NU, int R, int S, int Qp, int Ap, int ks, int L) {
+  return (decode_scalar_floats(NU, R, S, Qp, Ap, ks, L) + 3) & ~(size_t)3;
+}
+
 static size_t decode_smem_floats(int NU, int R, int S, int Qp, int Ap, int ks, int L, int O1, int O2, int Sp) {
-  const int K1 = ks * R + Ap;
   size_t omax = (size_t)O1;
   if ((size_t)O2 > omax) omax = O2;
   if ((size_t)Sp > omax) omax = Sp;
   if ((size_t)Qp > omax) omax = Qp;
   if (omax < 1024) omax = 1024;
-  return (size_t)NU * (K1 + 2 * R + 2 * S + Qp + Ap + (size_t)(ks - 1) * L * R + omax);
+  return decode_partial_offset(NU, R, S, Qp, Ap, ks, L) + (size_t)NU * omax;
 }
 
 }  // namespace wnb
@@ -410,6 +425,8 @@ WNB_API int wnb_decode_at(int32_t* xs, const float* h, const float* up_w, const 
     NU >>= 1;
   }
   WNB_REQUIRE(smem <= 227 * 1024, "decode: configuration needs %zu bytes of shared memory per CTA", smem);
+  p.partial_pad =
+      (int)(decode_partial_offset(NU, R, S, p.Qp, Ap, ks, L) - decode_scalar_floats(NU, R, S, p.Qp, Ap, ks, L));
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = cdiv(B, NU);
 #define WNB_LAUNCH_DECODE(N)                                                                                  \

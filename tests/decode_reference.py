@@ -51,11 +51,13 @@ def _conv(W, x, d=1):
     return y
 
 
-def forward64(cfg, p, x, h, device="cpu"):
+def forward64(cfg, p, x, h, device="cpu", dtype=torch.float64):
     """``oracle.forward`` (no upsampling: h at sample rate) in float64 torch on ``device``: x (B, T) int, h (B, A, T)
-    -> logits (B, T, Q) as a float64 numpy array."""
+    -> logits (B, T, Q) as a float64 numpy array.  ``dtype=torch.float32`` runs the same forward in plain float32 (the
+    parameters and aux rounded to float32 first; on a GPU the caller keeps TF32 off), which calibrates what float32
+    evaluation order alone costs against float64."""
     def t(k):
-        return torch.as_tensor(np.asarray(p[k], np.float64), device=device)
+        return torch.as_tensor(np.asarray(p[k], np.float64), device=device).to(dtype)
 
     def b(k):
         return t(k)[None, :, None]
@@ -63,7 +65,7 @@ def forward64(cfg, p, x, h, device="cpu"):
     W = t("causal.conv.weight")
     R, Q, ks = W.shape
     x = torch.as_tensor(np.asarray(x, np.int64), device=device) % Q
-    h = torch.as_tensor(np.asarray(h, np.float64), device=device)
+    h = torch.as_tensor(np.asarray(h, np.float64), device=device).to(dtype)
     B, T = x.shape
     out = b("causal.conv.bias").expand(B, R, T).clone()
     for k in range(ks):
@@ -81,14 +83,16 @@ def forward64(cfg, p, x, h, device="cpu"):
         out = _conv(t("res_1x1.%d.weight" % l), z) + b("res_1x1.%d.bias" % l) + out
     r1 = torch.relu(_conv(t("conv_post_1.weight"), torch.relu(skip)) + b("conv_post_1.bias"))
     y = _conv(t("conv_post_2.weight"), r1) + b("conv_post_2.bias")
-    return y.transpose(1, 2).cpu().numpy()
+    return y.transpose(1, 2).cpu().to(torch.float64).numpy()
 
 
-def teacher_forced_logits(cfg, p64, x, h, samples, device=None, chunk=None):
+def teacher_forced_logits(cfg, p64, x, h, samples, device=None, chunk=None, dtype=torch.float64):
     """float64 logits (B, n, Q) the decoder should produce at steps 0..n-1, given the seed x (B, T0), the aux h as passed
     to the decoder and the samples (B, n) it produced.  Step i depends on samples[:, :i] only, so for an utterance that
     stopped at n_b < n whatever follows its n_b-th sample does not matter for steps < n_b.  ``device=None`` runs
-    ``oracle.forward`` (numpy), else ``forward64`` on that device, ``chunk`` utterances at a time."""
+    ``oracle.forward`` (numpy), else ``forward64`` on that device in ``dtype``, ``chunk`` utterances at a time.  The
+    config's dilations are used as they are, so a config whose ``dilations`` and ``receptive_field`` were replaced
+    gets the forward of those."""
     xp, hp = O._pad_inputs(cfg, p64, np.asarray(x, np.int64), np.asarray(h, np.float64))
     P = xp.shape[1]
     samples = np.asarray(samples, np.int64)
@@ -96,11 +100,13 @@ def teacher_forced_logits(cfg, p64, x, h, samples, device=None, chunk=None):
     seq = np.concatenate([xp, samples[:, :n - 1]], 1)
     hs = hp[:, :, :P - 1 + n]
     c0 = O.Config(*cfg.as_tuple()[:7] + (0,))
+    c0.dilations, c0.receptive_field = list(cfg.dilations), cfg.receptive_field
     if device is None:
+        assert dtype == torch.float64, "oracle.forward runs in float64 only"
         return O.forward(c0, p64, seq, hs)[:, P - 1:P - 1 + n]
     B = seq.shape[0]
     step = B if chunk is None else chunk
-    return np.concatenate([forward64(c0, p64, seq[i:i + step], hs[i:i + step], device)[:, P - 1:P - 1 + n]
+    return np.concatenate([forward64(c0, p64, seq[i:i + step], hs[i:i + step], device, dtype)[:, P - 1:P - 1 + n]
                            for i in range(0, B, step)], 0)
 
 

@@ -2,8 +2,10 @@
 """CPU tier: pins the decode references of tests/decode_reference.py.
 
 * teacher forcing: one whole-sequence forward reproduces the oracle's step-by-step fast generation (kernel size 2 and 3,
-  with and without upsampling, seeds of 1 sample, shorter and longer than the receptive field, ragged lengths), and the
-  float64 torch forward reproduces ``oracle.forward``;
+  with and without upsampling, seeds of 1 sample, shorter and longer than the receptive field, ragged lengths, and
+  dilations that are not powers of two set on the config), and the float64 torch forward reproduces ``oracle.forward``;
+* the same forward with ``dtype=torch.float32`` is a float32 evaluation: within float32 rounding of float64, not equal
+  to it, and returned as float64;
 * Philox4x32-10 against the Random123 known-answer vectors;
 * the lane-scan sampler: under the old rule, uniforms placed in the gaps between lanes return an inadmissible class
   (Q-1); under the fixed rule no uniform does, over 10^4 logit vectors;
@@ -54,6 +56,44 @@ def test_teacher_forced_logits_match_fast_generate(case):
         for b in range(B):
             err = np.abs(ref[b, :n_list[b]] - lg[b, :n_list[b]]).max()
             assert err <= 1e-12 * max(1.0, np.abs(lg).max()), (case, dev, b, err)
+
+
+def test_teacher_forced_logits_follow_custom_dilations():
+    """dilations replaced on the config (ks 4, 1 and one longer than the decode among them) reach both references"""
+    cfg = O.Config(256, 28, 16, 32, 3, 2, 4, 0)
+    cfg.dilations = [1, 3, 11, 2, 5, 6]
+    cfg.receptive_field = 3 * sum(cfg.dilations) + 1
+    p = {k: v.astype(np.float64) for k, v in O.make_params(cfg, 45).items()}
+    rng = np.random.RandomState(4)
+    n_list = [9, 4]
+    x = rng.randint(0, 256, size=(2, 3)).astype(np.int64)
+    h = rng.standard_normal((2, 28, 3 + 9))
+    outs, lg = O.batch_fast_generate(cfg, p, x, h, n_list, mode="argmax", return_logits=True)
+    gen = _batch_order(outs, n_list, 256)
+    for dev in (None, "cpu"):
+        ref = D.teacher_forced_logits(cfg, p, x, h, gen, device=dev)
+        for b in range(2):
+            assert np.abs(ref[b, :n_list[b]] - lg[b, :n_list[b]]).max() <= 1e-12 * max(1.0, np.abs(lg).max()), (dev, b)
+    default = O.Config(*cfg.as_tuple())        # the power-of-two dilations give other logits
+    assert np.abs(D.teacher_forced_logits(default, p, x, h, gen, device="cpu")[0, :9] - lg[0, :9]).max() > 1e-3
+
+
+def test_forward64_float32_is_a_float32_evaluation():
+    cfg = O.Config(256, 28, 16, 32, 4, 1, 3, 0)
+    p = {k: v.astype(np.float64) for k, v in O.make_params(cfg, 3).items()}
+    rng = np.random.RandomState(1)
+    x = rng.randint(0, 256, size=(2, 50))
+    h = rng.standard_normal((2, 28, 50))
+    y64 = D.forward64(cfg, p, x, h)
+    y32 = D.forward64(cfg, p, x, h, dtype=torch.float32)
+    assert y32.dtype == np.float64 and y32.shape == y64.shape
+    assert np.array_equal(y32, y32.astype(np.float32))          # every value is a float32
+    err = np.abs(y32 - y64).max()
+    assert 0 < err <= 64 * 2.0 ** -24 * max(1.0, np.abs(y64).max()), err
+    sd = D.teacher_forced_logits(cfg, p, x[:, :5], h, x[:, 5:20], device="cpu", dtype=torch.float32)
+    assert np.array_equal(sd, sd.astype(np.float32))
+    with pytest.raises(AssertionError):
+        D.teacher_forced_logits(cfg, p, x[:, :5], h, x[:, 5:20], dtype=torch.float32)
 
 
 def test_forward64_matches_oracle_forward():

@@ -24,16 +24,27 @@ def _r4(v):
     return (v + 3) & ~3
 
 
-def _supported(Q, Ap, R, S, ks, L):
-    """decode_stream.cu's stream_plan at NU = 1, restated"""
+def _stream_plan(Q, Ap, R, S, ks, L, NU=1):
+    """decode_stream.cu's stream_plan, restated: (NU, ring slots) for a launch that starts at ``NU`` utterances per CTA
+    (1 at B <= SMs, 2 at B <= 2 SMs, else 4), or None when the shape is not covered"""
     widths = [_r4(2 * R), _r4(R), _r4(S), _r4(S), _r4(Q)]
     if any(w // 4 > 256 or w * 4 > 32 * 1024 for w in widths):
-        return False
+        return None
     if L > 64 or R % 4 or S % 4 or Ap % 4:
-        return False
+        return None
     K1 = ks * R + Ap
-    work = 4 * (K1 + 2 * R + 2 * S + _r4(Q) + Ap + (ks - 1) * L * R + 1024)
-    return work + 2 * 32 * 1024 + 512 <= 227 * 1024
+    while True:
+        work = 4 * NU * (K1 + 2 * R + 2 * S + _r4(Q) + Ap + (ks - 1) * L * R + 1024)
+        nslot = 0 if work + 2 * 32 * 1024 + 512 > 227 * 1024 else min((227 * 1024 - 64 - work - 256) // (32 * 1024), 6)
+        if nslot >= 2 or NU == 1:
+            break
+        NU //= 2
+    return (NU, nslot) if nslot >= 2 else None
+
+
+def _supported(Q, Ap, R, S, ks, L):
+    """decode_stream.cu's coverage query: stream_plan at NU = 1"""
+    return _stream_plan(Q, Ap, R, S, ks, L) is not None
 
 
 def test_supported_matches_the_launch_rule():

@@ -86,21 +86,24 @@ def _inputs(cfg, B, T0, max_n, seed):
     return x, h, n_list
 
 
-def _decode(net, x, h, n_list, mode, kernel, uniforms=None, seed=None):
+def _decode(net, x, h, n_list, mode, kernel, uniforms=None, seed=None, expect=None):
+    """decode with ``kernel`` and check that ``expect`` (default: the kernel named) ran"""
     with torch.no_grad():
         gen, lg = net._decode(torch.from_numpy(x).cuda(), torch.from_numpy(h).cuda(), n_list, mode,
                               uniforms=None if uniforms is None else torch.from_numpy(uniforms),
                               return_logits=True, seed=seed, kernel=kernel)
-    assert net.last_decode_kernel == kernel
+    assert net.last_decode_kernel == (expect or kernel), (kernel, net.last_decode_kernel)
     return gen.cpu().numpy().astype(np.int64), lg.cpu().numpy()
 
 
-def _check(cfg, p64, x, h, n_list, gen, lg, mode, uni):
+def _check(cfg, p64, x, h, n_list, gen, lg, mode, uni, refs=None):
     """per-step logit errors vs the teacher-forced float64 forward and every pick; returns (errors (B, max_n) with NaN
-    past n_b, list of bad picks)"""
+    past n_b, list of bad picks).  A dict ``refs`` receives the float64 logits as ``refs["ref"]``."""
     B, max_n = len(n_list), max(n_list)
     Q = cfg.n_quantize
     ref = D.teacher_forced_logits(cfg, p64, x, h, gen[:, :max_n], device="cuda", chunk=8)
+    if refs is not None:
+        refs["ref"] = ref
     err = np.full((B, max_n), np.nan)
     bad = []
     for b in range(B):
@@ -118,8 +121,9 @@ def _check(cfg, p64, x, h, n_list, gen, lg, mode, uni):
     return err, bad
 
 
-def _run_modes(cfg, net, p64, x, h, n_list, kernel, seed):
-    """argmax, sampling with supplied uniforms and sampling with in-kernel Philox: worst logit error per mode"""
+def _run_modes(cfg, net, p64, x, h, n_list, kernel, seed, expect=None, on_mode=None):
+    """argmax, sampling with supplied uniforms and sampling with in-kernel Philox: worst logit error per mode.
+    ``on_mode(mode, gen, lg, ref)``, when given, returns a dict of further results for the mode's row."""
     rng = np.random.RandomState(seed)
     B, max_n = len(n_list), max(n_list)
     rows = {}
@@ -127,15 +131,18 @@ def _run_modes(cfg, net, p64, x, h, n_list, kernel, seed):
         uni = None
         if mode == "uniforms":
             uni = rng.uniform(size=(B, max_n)).astype(np.float32)
-            gen, lg = _decode(net, x, h, n_list, "sampling", kernel, uniforms=uni)
+            gen, lg = _decode(net, x, h, n_list, "sampling", kernel, uniforms=uni, expect=expect)
         elif mode == "philox":
-            gen, lg = _decode(net, x, h, n_list, "sampling", kernel, seed=seed)
+            gen, lg = _decode(net, x, h, n_list, "sampling", kernel, seed=seed, expect=expect)
             uni = D.philox_uniform(seed, np.arange(B)[:, None], np.arange(max_n)[None, :])
         else:
-            gen, lg = _decode(net, x, h, n_list, "argmax", kernel)
-        err, bad = _check(cfg, p64, x, h, n_list, gen, lg, "argmax" if mode == "argmax" else "sampling", uni)
+            gen, lg = _decode(net, x, h, n_list, "argmax", kernel, expect=expect)
+        refs = {}
+        err, bad = _check(cfg, p64, x, h, n_list, gen, lg, "argmax" if mode == "argmax" else "sampling", uni, refs)
         rows[mode] = {"max_err": float(np.nanmax(err)), "bad_picks": bad,
                       "max_abs_logit": float(np.abs(lg[0, :n_list[0]]).max())}
+        if on_mode is not None:
+            rows[mode].update(on_mode(mode, gen, lg, refs["ref"]))
     return rows
 
 
