@@ -664,6 +664,46 @@ WNB_API int wnb_decode_bf16_pool_unpark(const void* const* stores, void* queues,
 WNB_API int wnb_decode_pool_move(const void* const* src, void* const* dst, const int32_t* rotations, int n, int R,
                                  int ks, const int32_t* host_dilations, int L, void* stream_handle);
 
+/* ---- mel-cepstral distortion between reference and decoded mel-cepstra (csrc/distortion.cu, utils/distortion.py) -----
+ * Inputs are float32 frames of n_cols = D + 1 coefficients (c0 first), as wnb_mcep writes them, widened to float64 in
+ * the kernels; every operation is float64 with explicit rounding (__dadd_rn, __dmul_rn, __dsqrt_rn), never an FMA.
+ * Pair p is reference frames [ref_offsets[p], ref_offsets[p+1]) of `ref` and decoded frames [dec_offsets[p],
+ * dec_offsets[p+1]) of `dec` (n_pairs + 1 int64 each; they need not start at 0).  The offsets are passed twice: on the
+ * device for the kernel and on the host (the same values) for the launcher's checks.
+ * dist(a, b) = sqrt(sum_{d=1..D} (a_d - b_d)^2), the squares added in ascending d; c0 is left out.  A frame's MCD in dB
+ * is K dist with K = fl(10 / ln 10) fl(sqrt 2), applied by the caller: the kernels write sums of dist and counts.
+ *
+ * wnb_mcd_aligned: frames t < n = min(Tr, Td) compared index by index; sum[p] = their dists added as 32-frame chunks
+ * (each chunk an xor butterfly over its 32 lanes, o = 16, 8, 4, 2, 1, frames past n counting 0.0), the chunk sums added
+ * in ascending order from 0.0; count[p] = n.
+ *
+ * wnb_mcd_dtw: C(i, j) = dist(r_i, d_j) + min(C(i-1, j-1), C(i-1, j), C(i, j-1)), C(0, 0) = dist(r_0, d_0); row 0 and
+ * column 0 follow their one predecessor; ties go to (i-1, j-1), then (i-1, j), then (i, j-1).  The path runs from
+ * (0, 0) to (Tr-1, Td-1); count[p] = its length, sum[p] = C(Tr-1, Td-1), which equals the sum of dist along the path
+ * added in forward order.  With `path` (optional), pair p's steps (i, j) as int32 pairs fill the first count[p] entries of
+ * its slot of Tr + Td - 1 entries; slot p starts at entry (ref_offsets[p] - ref_offsets[0]) + (dec_offsets[p] -
+ * dec_offsets[0]) - p.  Pair p uses wnb_mcd_dtw_workspace(Tr, Td) bytes of `workspace` (16-byte aligned) starting at the
+ * sum of that size over the pairs before it: the step directions, one byte per cell laid out per strip of
+ * WNB_MCD_DTW_THREADS rows, and, when Td > WNB_MCD_DTW_SMEM_COLS, a row of Td doubles.  wnb_mcd_dtw_workspace returns 0
+ * for a length outside [1, WNB_MCD_MAX_FRAMES].  One CTA per pair, the grid strided over the pairs.
+ *
+ * Both: no allocation, no synchronisation, one launch.  WNB_ERR_UNSUPPORTED for D outside [1, WNB_MCD_MAX_DIM] (wnb_mcep's
+ * orders) or a side with no frames (or more than WNB_MCD_MAX_FRAMES); WNB_ERR_INVALID for a null pointer, a misaligned
+ * workspace or path, or a workspace smaller than the pairs need; all before any device work. */
+#define WNB_MCD_MAX_DIM 40
+#define WNB_MCD_MAX_FRAMES (1 << 24)
+#define WNB_MCD_DTW_THREADS 256
+#define WNB_MCD_DTW_SMEM_COLS 4096
+WNB_API int wnb_mcd_aligned(const float* ref, const float* dec, int n_cols, const long long* ref_offsets,
+                            const long long* dec_offsets, const long long* host_ref_offsets,
+                            const long long* host_dec_offsets, int n_pairs, double* sum, int64_t* count,
+                            void* stream);
+WNB_API size_t wnb_mcd_dtw_workspace(long long ref_frames, long long dec_frames);
+WNB_API int wnb_mcd_dtw(const float* ref, const float* dec, int n_cols, const long long* ref_offsets,
+                        const long long* dec_offsets, const long long* host_ref_offsets,
+                        const long long* host_dec_offsets, int n_pairs, void* workspace, size_t workspace_bytes,
+                        double* sum, int64_t* count, int32_t* path, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -97,6 +97,9 @@ SIGNATURES = {
                                                                                       _P, _P]),
     "wnb_mcep": (_I, [_P, _I, _P, _P, _I, _L, _I, _I, _I, _c.c_double] + [_P] * 5
                  + [_I, _I] + [_c.c_double] * 3 + [_P, _P, _P]),
+    "wnb_mcd_aligned": (_I, [_P, _P, _I] + [_P] * 4 + [_I, _P, _P, _P]),
+    "wnb_mcd_dtw_workspace": (_c.c_size_t, [_L, _L]),
+    "wnb_mcd_dtw": (_I, [_P, _P, _I] + [_P] * 4 + [_I, _P, _c.c_size_t, _P, _P, _P, _P]),
 }
 
 _lib = None

@@ -18,7 +18,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libwnb200.so")
-SOURCES = ["elementwise.cu", "resblock_simt.cu", "decode.cu", "decode_stream.cu", "decode_stream_prefill.cu", "wgrad_tc.cu", "decode_warp.cu", "decode_bf16.cu", "decode_prefill.cu", "decode_bf16_prefill.cu", "decode_bf16_pool.cu", "decode_bf16_park.cu", "decode_pool.cu", "gemm_nt_tc.cu", "resblock_z.cu", "stack.cu", "pack.cu", "loader.cu", "mlsa.cu", "melspc.cu", "melspc_stream.cu", "mcep.cu", "adam.cu", "score.cu"]
+SOURCES = ["elementwise.cu", "resblock_simt.cu", "decode.cu", "decode_stream.cu", "decode_stream_prefill.cu", "wgrad_tc.cu", "decode_warp.cu", "decode_bf16.cu", "decode_prefill.cu", "decode_bf16_prefill.cu", "decode_bf16_pool.cu", "decode_bf16_park.cu", "decode_pool.cu", "gemm_nt_tc.cu", "resblock_z.cu", "stack.cu", "pack.cu", "loader.cu", "mlsa.cu", "melspc.cu", "melspc_stream.cu", "mcep.cu", "adam.cu", "score.cu", "distortion.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--fmad=true", "-cudart", "static"]
 
