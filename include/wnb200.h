@@ -335,6 +335,11 @@ WNB_API int wnb_profile_read(int kind, double* total_ms, int* launches);
  * them), or WNB_ERR_INVALID (bad input, or more than max_pieces). */
 WNB_API int wnb_wgrad_partition(const int* stages, const int* nchunk, const double* cost, const int* lock, int nprob,
                                 int sms, int* cta_first, int* pieces, int max_pieces);
+/* How the consumer threads of the weight-gradient kernel transpose the nB (1..7) B sub-tiles of one tf32 stage (a host
+ * function; no device needed): one row of 10 ints per 4 x 4 unit, {thread, iteration, 4 load offsets from the first B
+ * sub-tile, 4 store offsets into the transposed tile}, in bytes; load i holds time row i of the unit's 4 channels, store
+ * j channel j of its 4 time rows.  map holds 640 nB ints.  Returns the number of units (64 nB) or WNB_ERR_INVALID. */
+WNB_API int wnb_wgrad_transpose_map(int nB, int* map);
 
 /* ---- residual stack in deferred-skip form (training path of WaveNet.forward, wavenet.py:229-236 over :525-536) ----
  * The skip sum over all L blocks is one GEMM over the concatenated gate outputs,

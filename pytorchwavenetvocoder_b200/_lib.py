@@ -43,6 +43,7 @@ SIGNATURES = {
     "wnb_profile_enable": (_I, [_I]),
     "wnb_profile_read": (_I, [_I, _P, _P]),
     "wnb_wgrad_partition": (_I, [_P, _P, _P, _P, _I, _I, _P, _P, _I]),
+    "wnb_wgrad_transpose_map": (_I, [_I, _P]),
     "wnb_stack_supported": (_I, [_I] * 6),
     "wnb_resblock_fwd_z": (_I, [_P] * 8 + [_I] * 8 + [_P]),
     "wnb_skip_gemm": (_I, [_P] * 4 + [_I] * 5 + [_P]),

@@ -214,7 +214,7 @@ __device__ __forceinline__ void named_bar(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 // byte offset of element (row r, column c < 32) in a [rows x 32 fp32] tile written by TMA with 128B swizzle
-__device__ __forceinline__ uint32_t sw128_off(int r, int c) {
+__host__ __device__ __forceinline__ uint32_t sw128_off(int r, int c) {
   return (uint32_t)(r * 128 + ((((c >> 2) ^ r) & 7) << 4) + ((c & 3) << 2));
 }
 

@@ -80,6 +80,27 @@ static_assert(sizeof(Params) <= 32000, "wgrad_tc: kernel parameters exceed the 3
 template <bool BF16>
 __host__ __device__ constexpr int bt_row_bytes() { return BF16 ? 64 : 128; }
 
+// The tf32 B transpose of one stage is cut into 64 nB units, each a 4 x 4 block of one B group: time rows 4 q .. 4 q + 3
+// of channel chunk c4 (four 16-byte loads from the swizzled [32 x 32] sub-tile) become channels 4 c4 .. 4 c4 + 3 of time
+// chunk q (four 16-byte stores into the K-major 128B-swizzled tile).  Unit u = 64 grp + 8 x + l has q = l, c4 = l ^ x:
+// the 8 lanes of each quarter warp then load from 8 distinct 16-byte bank groups and store to 8 distinct ones, so every
+// warp-wide load and store takes 4 shared-memory wavefronts for its 512 bytes.  (With c4 fixed per quarter warp the
+// stores would still fill whole rows, but the loads of a quarter warp would hit only 2 bank groups.)
+// Consumer thread t runs units t ^ 128, + 256, ...: warpgroup 1 takes the first ones, since in an M = 64 problem
+// warpgroup 0 alone also loads the A fragments and issues the MMAs.
+struct TrUnit { uint32_t src[4], dst[4]; };   // bytes from the first B sub-tile / from the transposed tile
+__host__ __device__ __forceinline__ int tr_first_unit(int t) { return t ^ 128; }
+__host__ __device__ __forceinline__ TrUnit tr_unit(int u) {
+  const int grp = u >> 6, q = u & 7, c4 = q ^ ((u >> 3) & 7), r = 4 * q;
+  TrUnit o;
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+    o.src[i] = grp * kSub + (r + i) * 128 + ((c4 ^ ((r + i) & 7)) << 4);   // time row r + i, channels 4 c4 ..
+    o.dst[i] = ptx::sw128_off(grp * 32 + 4 * c4 + i, r);                  // channel 4 c4 + i, time rows r ..
+  }
+  return o;
+}
+
 // One piece with N = 32 (nB + ones): the consumer loop of both warpgroups.  Ring position (s, ph) carries over from
 // piece to piece; the two transposed B tiles are free on entry (every wgmma of the previous piece has completed).
 template <int N, bool BF16, bool M64>
@@ -166,20 +187,21 @@ __device__ __forceinline__ void run_piece(const Params& p, const Prob& pr, const
     }
   } else {
     uint32_t a0[4][4], a1[4][4];
-    const int nvec = nB * 32 * 32 / 4;            // float4 pieces of the B sub-tiles
+    const int nunit = nB * 64;                    // 4 x 4 transpose units of the B sub-tiles (tr_unit)
     auto stage = [&](uint32_t (&a)[4][4], unsigned char* bTh, bool mine) {
       ptx::mbar_wait(&full[s], ph);
       const unsigned char* st = ring + (size_t)s * p.stage_bytes;
+      const unsigned char* sB = st + nA * kSub;
       ptx::named_bar(1, kConsumers);   // every consumer has waited for the MMAs of stage i - 2: bTh may be overwritten
-      for (int idx = threadIdx.x; idx < nvec; idx += kConsumers) {
-        const int grp = idx >> 8, r = (idx >> 3) & 31, c4 = idx & 7;   // B group, time row, 4-channel piece
-        const float4 v = *reinterpret_cast<const float4*>(st + (nA + grp) * kSub + r * 128 + ((c4 ^ (r & 7)) << 4));
-        const float vv[4] = {v.x, v.y, v.z, v.w};
+      for (int u = tr_first_unit(threadIdx.x); u < nunit; u += kConsumers) {
+        const TrUnit o = tr_unit(u);
+        float4 v[4];
 #pragma unroll
-        for (int j = 0; j < 4; j++) {
-          const int n = grp * 32 + c4 * 4 + j;
-          *reinterpret_cast<float*>(bTh + ptx::sw128_off(n, r)) = vv[j];
-        }
+        for (int i = 0; i < 4; i++) v[i] = *reinterpret_cast<const float4*>(sB + o.src[i]);
+        *reinterpret_cast<float4*>(bTh + o.dst[0]) = make_float4(v[0].x, v[1].x, v[2].x, v[3].x);
+        *reinterpret_cast<float4*>(bTh + o.dst[1]) = make_float4(v[0].y, v[1].y, v[2].y, v[3].y);
+        *reinterpret_cast<float4*>(bTh + o.dst[2]) = make_float4(v[0].z, v[1].z, v[2].z, v[3].z);
+        *reinterpret_cast<float4*>(bTh + o.dst[3]) = make_float4(v[0].w, v[1].w, v[2].w, v[3].w);
       }
       if (mine) {
 #pragma unroll
@@ -227,7 +249,9 @@ __device__ __forceinline__ void run_piece(const Params& p, const Prob& pr, const
 template <bool BF16>
 __global__ void __launch_bounds__(kThreadsW, 1) wgrad_tc_kernel(const __grid_constant__ Params p) {
   extern __shared__ unsigned char smem_raw[];
-  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  // aligned by pointer arithmetic on smem_raw (not through an integer), so that the compiler still knows every pointer
+  // derived from it is a shared-memory one and emits LDS / STS instead of generic loads and stores
+  unsigned char* smem = smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
   unsigned char* bT = smem;                                   // 2 x K-major [N x 32] B tile (+ the ones rows)
   unsigned char* ring = smem + 2 * p.bt_half;
   uint64_t* bars = reinterpret_cast<uint64_t*>(ring + (size_t)p.nstages * p.stage_bytes);
@@ -365,13 +389,15 @@ static cudaError_t launch(int grid, size_t smem, cudaStream_t st, const Params& 
 // Time of one stage on one SM (microseconds), from the problem's shape: the larger of streaming its HBM bytes through
 // the CTA's ring and the work of the consumer warpgroups (B transpose and A fragment loads per element, wgmma per
 // flop at the dense tf32 rate of one SM, 3.75 TFLOP/s).  The per-element and streaming constants are fitted to the
-// per-piece times of this kernel measured with %globaltimer on an H100 80GB HBM3 (700 W, 1980 MHz) at the bench shape:
-// dWskip 1.21 us per stage (N = 224, 6 transposed groups), dW1 1.03 (N = 192, 5 groups), both consumer-bound, and
-// dW2res 0.60 (16 KB per stage streamed, ~27 GB/s per SM with four ring stages in flight).
+// per-piece times of this kernel's tf32 path (the 4 x 4 register-block transpose) measured with %globaltimer on an
+// H100 80GB HBM3 (700 W power limit, SM clock 1980 MHz) at the bench shape: dWskip 0.89 us per stage (N = 224,
+// 6 transposed groups), dW1 0.85 (N = 192, 5 groups), 0.73 for N = 160 with 4 groups, all consumer-bound (the
+// B-element constant is their least-squares fit), and dW2res 0.50 (16 KB per stage streamed, ~33 GB/s per SM with four
+// ring stages in flight).
 static double stage_cost_us(int M, int N, int nB, double hbm_bytes, bool bf16) {
-  const double stream_us = hbm_bytes / 27.3e3;
+  const double stream_us = hbm_bytes / 32.8e3;
   const double flop_us = 2.0 * M * N * kTK / (bf16 ? 7.5e6 : 3.75e6);
-  const double elem_us = 1.07e-4 * nB * 32.0 * kTK + 1.6e-5 * (double)M * kTK;
+  const double elem_us = 6.4e-5 * nB * 32.0 * kTK + 1.6e-5 * (double)M * kTK;
   return fmax(stream_us, flop_us + elem_us);
 }
 
@@ -646,4 +672,21 @@ WNB_API int wnb_wgrad_partition(const int* stages, const int* nchunk, const doub
                                       reinterpret_cast<wnb::WgPiece*>(pieces), max_pieces);
   if (np < 0) wnb::set_error("wgrad_partition: bad arguments or more than %d pieces", max_pieces);
   return np < 0 ? WNB_ERR_INVALID : np;
+}
+
+WNB_API int wnb_wgrad_transpose_map(int nB, int* map) {
+  using namespace wnb::wg;
+  if (nB < 1 || nB > kMaxB - 1 || !map) {
+    wnb::set_error("wgrad_transpose_map: 1..7 B groups and a map");
+    return WNB_ERR_INVALID;
+  }
+  int k = 0;
+  for (int t = 0; t < kConsumers; t++)   // the consumer loop of run_piece, thread by thread
+    for (int u = tr_first_unit(t), it = 0; u < nB * 64; u += kConsumers, it++) {
+      const TrUnit o = tr_unit(u);
+      int* row = map + 10 * k++;
+      row[0] = t; row[1] = it;
+      for (int i = 0; i < 4; i++) { row[2 + i] = (int)o.src[i]; row[6 + i] = (int)o.dst[i]; }
+    }
+  return k;
 }
