@@ -145,7 +145,7 @@ def test_post_bwd_bf16_exact(S, B, T):
 # ------------------------------------------------------------------------------------------------------------------
 # 3. stage by stage against float64 (cv=to_bf16)
 # ------------------------------------------------------------------------------------------------------------------
-def _perblock_bf16(R_, S, Ap, ks, d, B, T, last, init, seed):
+def _perblock_bf16(R_, S, Ap, ks, d, B, T, last, init, seed, repeat_bwd=False):
     L_, lib = _lib()
     g = torch.Generator(device="cuda").manual_seed(seed)
     rn = lambda *sh: torch.randn(*sh, device="cuda", generator=g)   # noqa: E731
@@ -167,13 +167,22 @@ def _perblock_bf16(R_, S, Ap, ks, d, B, T, last, init, seed):
     dskip = rn(B, T, S)
     w1t, w2t = w1.t().contiguous(), w2.t().contiguous()
     ginit = dict(dh=rn(B, T, Ap), dw1=rn(2 * R_, K1), db1=rn(2 * R_), dw2=rn(R_ + S, R_), db2=rn(R_ + S))
-    gout = {k: G(tuple(v.shape), v) for k, v in ginit.items()}
-    dx = G((B, T, R_))
-    ws = G((lib.wnb_resblock_bwd_workspace(B, T, R_, S, Ap, ks) // 4,))
-    L_.check(lib.wnb_resblock_bwd(L_.ptr(xin), L_.ptr(haux), L_.ptr(dout), L_.ptr(dskip), L_.ptr(w1), L_.ptr(b1),
-                                  L_.ptr(w1t), L_.ptr(w2t), L_.ptr(dx), L_.ptr(gout["dh"]), L_.ptr(gout["dw1"]),
-                                  L_.ptr(gout["db1"]), L_.ptr(gout["dw2"]), L_.ptr(gout["db2"]), L_.ptr(ws),
-                                  B, T, R_, S, Ap, ks, d, L_.MATH_BF16, L_.stream()), "resblock_bwd")
+
+    def backward():
+        gout = {k: G(tuple(v.shape), v) for k, v in ginit.items()}
+        dx = G((B, T, R_))
+        ws = G((lib.wnb_resblock_bwd_workspace(B, T, R_, S, Ap, ks) // 4,))
+        L_.check(lib.wnb_resblock_bwd(L_.ptr(xin), L_.ptr(haux), L_.ptr(dout), L_.ptr(dskip), L_.ptr(w1), L_.ptr(b1),
+                                      L_.ptr(w1t), L_.ptr(w2t), L_.ptr(dx), L_.ptr(gout["dh"]), L_.ptr(gout["dw1"]),
+                                      L_.ptr(gout["db1"]), L_.ptr(gout["dw2"]), L_.ptr(gout["db2"]), L_.ptr(ws),
+                                      B, T, R_, S, Ap, ks, d, L_.MATH_BF16, L_.stream()), "resblock_bwd")
+        return gout, dx, ws
+    gout, dx, ws = backward()
+    if repeat_bwd:     # a second backward from the same inputs: bit-identical gradients (fixed summation order)
+        g2, dx2, _ = backward()
+        assert torch.equal(dx2, dx), "dx differs between two backward runs"
+        for k in gout:
+            assert torch.equal(g2[k], gout[k]), "%s differs between two backward runs" % k
     torch.cuda.synchronize()
     G.check()
     log = Log()
@@ -218,21 +227,22 @@ def test_composed_block_bf16_stages(R_, S, Ap, ks, d, T, last, init):
     _perblock_bf16(R_, S, Ap, ks, d, 2, T, last, init, seed=R_ + S + T + ks + 1)
 
 
-@pytest.mark.parametrize("S,B,T", [(512, 2, 1000), (256, 3, 65), (96, 1, 1)])
-def test_post_network_bf16_stages(S, B, T):
+def _post_stages(S, Q, B, T, math_mode, cv, rectified, seed, name):
+    """wnb_post_fwd / wnb_post_bwd stage by stage against float64 with the bounds for cv (to_tf32 or to_bf16).
+    rectified: 0 = the forward rectifies skip in place; 1 = skip is passed rectified (skip_rectified) and stays as is."""
     L_, lib = _lib()
-    Q = 256
-    cv = to_bf16
-    g = torch.Generator(device="cuda").manual_seed(S + B + T)
+    mm = {"tf32": L_.MATH_TF32, "bf16": L_.MATH_BF16}[math_mode]
+    g = torch.Generator(device="cuda").manual_seed(seed)
     rn = lambda *sh: torch.randn(*sh, device="cuda", generator=g)   # noqa: E731
     wp1, bp1 = rn(S, S) / math.sqrt(S), 0.1 * rn(S)
     wp2, bp2 = rn(Q, S) / math.sqrt(S), 0.1 * rn(Q)
     G = Guarded()
-    skip = G((B, T, S), rn(B, T, S))
-    sr = skip.clamp_min(0)
+    skip0 = rn(B, T, S)
+    skip = G((B, T, S), skip0.clamp_min(0) if rectified else skip0)
+    sr = skip0.clamp_min(0)
     r1, logits = G((B, T, S)), G((B, T, Q))
     L_.check(lib.wnb_post_fwd(L_.ptr(skip), L_.ptr(wp1), L_.ptr(bp1), L_.ptr(wp2), L_.ptr(bp2), L_.ptr(r1),
-                              L_.ptr(logits), B, T, S, Q, L_.MATH_BF16, 0, L_.stream()), "post_fwd")
+                              L_.ptr(logits), B, T, S, Q, mm, rectified, L_.stream()), "post_fwd")
     dlogits = rn(B, T, Q)
     init = dict(dwp1=rn(S, S), dbp1=rn(S), dwp2=rn(Q, S), dbp2=rn(Q))
     out = {k: G(tuple(v.shape), v) for k, v in init.items()}
@@ -240,11 +250,11 @@ def test_post_network_bf16_stages(S, B, T):
     wp1t, wp2t = wp1.t().contiguous(), wp2.t().contiguous()
     L_.check(lib.wnb_post_bwd(L_.ptr(skip), L_.ptr(r1), L_.ptr(dlogits), L_.ptr(wp1t), L_.ptr(wp2t), L_.ptr(dskip),
                               L_.ptr(out["dwp1"]), L_.ptr(out["dbp1"]), L_.ptr(out["dwp2"]), L_.ptr(out["dbp2"]),
-                              L_.ptr(ws), B, T, S, Q, L_.MATH_BF16, L_.stream()), "post_bwd")
+                              L_.ptr(ws), B, T, S, Q, mm, L_.stream()), "post_bwd")
     torch.cuda.synchronize()
     G.check()
     log = Log()
-    assert torch.equal(skip, sr)
+    assert torch.equal(skip, sr), "skip is not rectified in place"
     (h1, e1), logits_of = ref.post_fwd(sr, wp1, bp1, wp2, bp2, cv=cv)
     log("r1", r1, (h1, e1))
     log("logits", logits, logits_of(r1))
@@ -255,7 +265,12 @@ def test_post_network_bf16_stages(S, B, T):
         v, b = st[k]
         i = init[k].double()
         log(k, out[k], (v + i, b + ref.U * ((v + i).abs() + i.abs())))
-    _report("bf16_post_S%d_B%d_T%d" % (S, B, T), log.res)
+    _report(name, log.res)
+
+
+@pytest.mark.parametrize("S,B,T", [(512, 2, 1000), (256, 3, 65), (96, 1, 1)])
+def test_post_network_bf16_stages(S, B, T):
+    _post_stages(S, 256, B, T, "bf16", to_bf16, 0, S + B + T, "bf16_post_S%d_B%d_T%d" % (S, B, T))
 
 
 # ------------------------------------------------------------------------------------------------------------------

@@ -275,7 +275,7 @@ def test_block_z_and_skip_gemm(d, T, last):
 # ------------------------------------------------------------------------------------------------------------------
 # per-block tf32 entries: the fused kernel (R = 64) and the composed path
 # ------------------------------------------------------------------------------------------------------------------
-def _perblock(R_, S, Ap, ks, d, B, T, last, init, seed):
+def _perblock(R_, S, Ap, ks, d, B, T, last, init, seed, repeat_bwd=False):
     L_, lib = _lib()
     g = torch.Generator(device="cuda").manual_seed(seed)
     rn = lambda *sh: torch.randn(*sh, device="cuda", generator=g)   # noqa: E731
@@ -297,13 +297,22 @@ def _perblock(R_, S, Ap, ks, d, B, T, last, init, seed):
     dskip = rn(B, T, S)
     w1t, w2t = w1.t().contiguous(), w2.t().contiguous()
     ginit = dict(dh=rn(B, T, Ap), dw1=rn(2 * R_, K1), db1=rn(2 * R_), dw2=rn(R_ + S, R_), db2=rn(R_ + S))
-    gout = {k: G(tuple(v.shape), v) for k, v in ginit.items()}
-    dx = G((B, T, R_))
-    ws = G((lib.wnb_resblock_bwd_workspace(B, T, R_, S, Ap, ks) // 4,))
-    L_.check(lib.wnb_resblock_bwd(L_.ptr(xin), L_.ptr(haux), L_.ptr(dout), L_.ptr(dskip), L_.ptr(w1), L_.ptr(b1),
-                                  L_.ptr(w1t), L_.ptr(w2t), L_.ptr(dx), L_.ptr(gout["dh"]), L_.ptr(gout["dw1"]),
-                                  L_.ptr(gout["db1"]), L_.ptr(gout["dw2"]), L_.ptr(gout["db2"]), L_.ptr(ws),
-                                  B, T, R_, S, Ap, ks, d, L_.MATH_TF32, L_.stream()), "resblock_bwd")
+
+    def backward():
+        gout = {k: G(tuple(v.shape), v) for k, v in ginit.items()}
+        dx = G((B, T, R_))
+        ws = G((lib.wnb_resblock_bwd_workspace(B, T, R_, S, Ap, ks) // 4,))
+        L_.check(lib.wnb_resblock_bwd(L_.ptr(xin), L_.ptr(haux), L_.ptr(dout), L_.ptr(dskip), L_.ptr(w1), L_.ptr(b1),
+                                      L_.ptr(w1t), L_.ptr(w2t), L_.ptr(dx), L_.ptr(gout["dh"]), L_.ptr(gout["dw1"]),
+                                      L_.ptr(gout["db1"]), L_.ptr(gout["dw2"]), L_.ptr(gout["db2"]), L_.ptr(ws),
+                                      B, T, R_, S, Ap, ks, d, L_.MATH_TF32, L_.stream()), "resblock_bwd")
+        return gout, dx, ws
+    gout, dx, ws = backward()
+    if repeat_bwd:     # a second backward from the same inputs: bit-identical gradients (fixed summation order)
+        g2, dx2, _ = backward()
+        assert torch.equal(dx2, dx), "dx differs between two backward runs"
+        for k in gout:
+            assert torch.equal(g2[k], gout[k]), "%s differs between two backward runs" % k
     torch.cuda.synchronize()
     G.check()
     log = Log()
