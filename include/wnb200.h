@@ -128,6 +128,19 @@ WNB_API int wnb_make_train_batch(const float* wave, const void* feat, const int3
                                  int64_t* x, int64_t* t, float* h, int B, int T, int Tf, int D, int feat_f64, int mu,
                                  void* stream);
 
+/* ---- the same batch cut from a device-resident corpus (utils/corpus.py, utils/device_loader.DeviceCorpusGenerator) ---
+ * `wave` (int16) and `feat` (rows of D, layout and feat_f64 as above) hold every utterance once, trimmed to whole frames.
+ * The stream of concatenated utterances in epoch order is a table of the n_utts non-empty utterances it covers:
+ * starts[k] = stream position of the utterance's first sample (strictly increasing), offsets[k] = its first sample in
+ * `wave` (a multiple of U; its first frame is row offsets[k] / U).  Stream position p maps to the utterance k with the
+ * largest starts[k] <= p (binary search), sample offsets[k] + p - starts[k].  [table_begin, table_end) is the part of the
+ * stream the table covers; every window must lie in it.  x[b][i] = encode_mu_law(sample / 32768) of position
+ * s0 + b*hop + i, t the next sample, h[b][d][j] = the scaled row of stream frame (s0 + b*hop)/U + j (up-sampling layer). */
+WNB_API int wnb_make_train_batch_corpus(const int16_t* wave, const void* feat, const int64_t* starts, const int64_t* offsets,
+                                        int n_utts, int64_t table_begin, int64_t table_end, int64_t s0, int64_t hop, int U,
+                                        const double* mean, const double* scale, int64_t* x, int64_t* t, float* h, int B,
+                                        int T, int Tf, int D, int feat_f64, int mu, void* stream);
+
 /* ---- a12: the optimizer step (bin/train.py:457-460, :539 torch.optim.Adam) as one kernel over flat buffers ----------
  * p, g, m, v: parameters, gradients (the flat buffer wnb_pack_weights' backward direction fills), first and second moment
  * estimates, n floats each, 16-byte aligned, identical layout.  torch's (fused) Adam arithmetic in fp32: g += weight_decay*p;

@@ -87,6 +87,7 @@ SIGNATURES = {
     "wnb_pack_weights": (_I, [_P, _I, _P, _P, _P, _P]),
     "wnb_zero": (_I, [_P, _c.c_size_t, _P]),
     "wnb_make_train_batch": (_I, [_P, _P, _P, _L, _L, _I, _L, _L] + [_P] * 5 + [_I] * 6 + [_P]),
+    "wnb_make_train_batch_corpus": (_I, [_P] * 4 + [_I, _L, _L, _L, _L, _I] + [_P] * 5 + [_I] * 6 + [_P]),
     "wnb_adam_flat": (_I, [_P, _P, _P, _P, _L] + [_c.c_double] * 7 + [_P]),
     "wnb_mlsa_filter": (_I, [_P, _I, _P, _I, _P, _I, _c.c_double, _I, _c.c_double, _P, _I, _P]),
     "wnb_mlsa_state_doubles": (_c.c_size_t, [_I, _I]),

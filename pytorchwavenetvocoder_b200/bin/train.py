@@ -178,8 +178,10 @@ def get_parser():
     """Flags of reference train.py:337-394 (+ optional --math_mode)."""
     parser = argparse.ArgumentParser()
     parser.add_argument("--waveforms", required=True, type=str, help="directory or list of wav files")
-    parser.add_argument("--feats", required=True, type=str, help="directory or list of aux feat files")
-    parser.add_argument("--stats", required=True, type=str, help="hdf5 file including statistics")
+    parser.add_argument("--feats", default=None, type=str,
+                        help="directory or list of aux feat files (required unless --extract_features true)")
+    parser.add_argument("--stats", default=None, type=str,
+                        help="hdf5 file including statistics (required unless --extract_features true)")
     parser.add_argument("--expdir", required=True, type=str, help="directory to save the model")
     parser.add_argument("--feature_type", default="world", choices=["world", "melspc"], type=str,
                         help="feature type")
@@ -218,6 +220,28 @@ def get_parser():
                              "(0: off)")
     parser.add_argument("--dev_batch_samples", default=1 << 19, type=int,
                         help="samples per held-out scoring batch (rows x longest row)")
+    # (H100 build) the *-melspc recipes' stages 1-3 on the device, the corpus resident in HBM (utils/corpus.py); the
+    # extraction flags are feature_extract.py's and noise_shaping.py's, with their defaults
+    from pytorchwavenetvocoder_b200.bin.feature_extract import _optional_int
+    parser.add_argument("--extract_features", default=False, type=_strtobool,
+                        help="(H100 build) compute the melspc features, statistics (<expdir>/stats.h5) and optional "
+                             "noise shaping from the raw wavs of --waveforms on the GPU and train from the resident "
+                             "corpus, instead of reading --feats / --stats")
+    parser.add_argument("--fs", default=16000, type=int, help="sampling frequency (--extract_features)")
+    parser.add_argument("--shiftms", default=5, type=float, help="frame shift in msec (--extract_features)")
+    parser.add_argument("--fftl", default=1024, type=int, help="FFT length (--extract_features)")
+    parser.add_argument("--mspc_dim", default=80, type=int, help="dimension of mel spectrogram (--extract_features)")
+    parser.add_argument("--fmin", default=None, nargs="?", type=_optional_int,
+                        help="minimum frequency for melspc (empty: not given; --extract_features)")
+    parser.add_argument("--fmax", default=None, nargs="?", type=_optional_int,
+                        help="maximum frequency for melspc (empty: not given; --extract_features)")
+    parser.add_argument("--highpass_cutoff", default=70, type=int,
+                        help="cut off frequency of the low-cut filter, 0: none (--extract_features)")
+    parser.add_argument("--noise_shaping", default=False, type=_strtobool,
+                        help="train on noise-shaped wavs (noise_shaping.py --inv true; --extract_features)")
+    parser.add_argument("--mcep_dim", default=24, type=int, help="dimension of mel cepstrum (--noise_shaping)")
+    parser.add_argument("--mcep_alpha", default=0.41, type=float, help="alpha of mel cepstrum (--noise_shaping)")
+    parser.add_argument("--mag", default=0.5, type=float, help="magnification of noise shaping (--noise_shaping)")
     return parser
 
 
@@ -232,6 +256,126 @@ def check_dev_args(args):
     if args.dev_batch_samples <= 0:
         return "--dev_batch_samples should be positive, got %d" % args.dev_batch_samples
     return None
+
+
+def extract_wav_list(waveforms):
+    """The wav files of --waveforms in the order train.py reads them: sorted from a directory, or the list's order."""
+    if os.path.isdir(waveforms):
+        return [waveforms + "/" + f for f in sorted(find_files(waveforms, "*.wav", use_dir_name=False))]
+    if os.path.isfile(waveforms):
+        return read_txt(waveforms)
+    return None
+
+
+def check_extract_args(args, parser):
+    """Refusals of --extract_features, before any work: an error message, or None.  Reads the wav headers only."""
+    from pytorchwavenetvocoder_b200.utils.corpus import wav_refusals
+    from pytorchwavenetvocoder_b200.utils.melspc import shift_length
+    if not args.extract_features:
+        return None
+    if args.feats is not None or args.stats is not None:
+        return "--extract_features true computes the features and statistics: do not give --feats or --stats"
+    if args.feature_type != "melspc":
+        return "--extract_features true extracts melspc features: use --feature_type melspc"
+    if args.mspc_dim != args.n_aux:
+        return "--mspc_dim %d should equal --n_aux %d" % (args.mspc_dim, args.n_aux)
+    if not args.use_upsampling_layer:
+        return "--extract_features true trains with the up-sampling layer: --use_upsampling_layer false is not covered"
+    hop = shift_length(args.shiftms, args.fs)
+    if args.upsampling_factor != hop:
+        return "--upsampling_factor %d should be the frame shift in samples, %d (--shiftms %g at --fs %d)" % (
+            args.upsampling_factor, hop, args.shiftms, args.fs)
+    if args.use_speaker_code:
+        return "--extract_features true does not cover --use_speaker_code"
+    if args.batch_length <= 0:
+        return "--extract_features true covers the mini-batch mode: --batch_length 0 is not covered"
+    if args.host_loader:
+        return "--extract_features true trains from the device-resident corpus: --host_loader is not covered"
+    for name in ("dev_waveforms", "dev_feats", "dev_interval", "dev_batch_samples"):
+        if getattr(args, name) != parser.get_default(name):
+            return "--extract_features true does not cover the held-out loss: do not give --%s" % name
+    wav_list = extract_wav_list(args.waveforms)
+    if wav_list is None:
+        return "--waveforms should be directory or list."
+    if len(wav_list) == 0:
+        return "--waveforms names no wav files"
+    bad = wav_refusals(wav_list, args.fs, args.fftl)
+    if bad:
+        return "; ".join(bad)
+    return None
+
+
+def file_generator(args, model, local):
+    """The training generator over --waveforms / --feats with the --stats scaler: (generator, scaler)."""
+    scaler = StandardScaler()
+    scaler.mean_ = read_hdf5(args.stats, "/" + args.feature_type + "/mean")
+    scaler.scale_ = read_hdf5(args.stats, "/" + args.feature_type + "/scale")
+    wav_transform = lambda x: encode_mu_law(x, args.n_quantize)  # noqa: E731
+    feat_transform = lambda x: scaler.transform(x)  # noqa: E731
+
+    if os.path.isdir(args.waveforms):
+        filenames = sorted(find_files(args.waveforms, "*.wav", use_dir_name=False))
+        wav_list = [args.waveforms + "/" + filename for filename in filenames]
+        feat_list = [args.feats + "/" + filename.replace(".wav", ".h5") for filename in filenames]
+    elif os.path.isfile(args.waveforms):
+        wav_list = read_txt(args.waveforms)
+        feat_list = read_txt(args.feats)
+    else:
+        logging.error("--waveforms should be directory or list.")
+        sys.exit(1)
+    assert len(wav_list) == len(feat_list)
+    logging.info("number of training data = %d." % len(wav_list))
+    if args.batch_length > 0 and not args.host_loader:
+        # mini-batch modes: windowing + mu-law + scaler on the device, utterances uploaded once (utils/device_loader.py);
+        # same batches as train_generator below (tests/test_gpu_loader.py)
+        from pytorchwavenetvocoder_b200.utils.device_loader import DeviceTrainGenerator
+        generator = DeviceTrainGenerator(
+            wav_list, feat_list, model.receptive_field, args.batch_length, args.batch_size,
+            feature_type=args.feature_type, n_quantize=args.n_quantize, mean=scaler.mean_, scale=scaler.scale_,
+            shuffle=True, upsampling_factor=args.upsampling_factor, use_upsampling_layer=args.use_upsampling_layer,
+            use_speaker_code=args.use_speaker_code, device=local)
+    else:
+        generator = train_generator(
+            wav_list, feat_list,
+            receptive_field=model.receptive_field,
+            batch_length=args.batch_length if args.batch_length > 0 else None,
+            batch_size=args.batch_size,
+            feature_type=args.feature_type,
+            wav_transform=wav_transform,
+            feat_transform=feat_transform,
+            shuffle=True,
+            upsampling_factor=args.upsampling_factor,
+            use_upsampling_layer=args.use_upsampling_layer,
+            use_speaker_code=args.use_speaker_code,
+            device=local)
+    return generator, scaler
+
+
+def corpus_generator(args, model, rank, local):
+    """--extract_features: the *-melspc recipes' stages 1-3 on this rank's GPU into a resident corpus, <expdir>/stats
+    written by rank 0, and the generator over the corpus.  Every rank prepares the same corpus (the same bits)."""
+    from pytorchwavenetvocoder_b200.bin.feature_extract import _feature_ext
+    from pytorchwavenetvocoder_b200.utils.corpus import CorpusTooLarge, prepare_corpus
+    from pytorchwavenetvocoder_b200.utils.device_loader import DeviceCorpusGenerator
+    wav_list = extract_wav_list(args.waveforms)
+    logging.info("number of training data = %d." % len(wav_list))
+    try:
+        corpus = prepare_corpus(wav_list, fs=args.fs, shiftms=args.shiftms, fftl=args.fftl, mspc_dim=args.mspc_dim,
+                                fmin=args.fmin, fmax=args.fmax, highpass_cutoff=args.highpass_cutoff,
+                                noise_shaping=args.noise_shaping, mcep_dim=args.mcep_dim,
+                                mcep_alpha=args.mcep_alpha, mag=args.mag, device=local)
+    except CorpusTooLarge as e:
+        logging.error(str(e))
+        sys.exit(1)
+    if rank == 0:
+        stats_file = args.expdir + "/stats" + _feature_ext()
+        if os.path.exists(stats_file):
+            os.remove(stats_file)                  # this run's statistics only
+        corpus.write_stats(stats_file)
+        logging.info("statistics written to %s." % stats_file)
+    return DeviceCorpusGenerator(corpus, model.receptive_field, args.batch_length, args.batch_size,
+                                 n_quantize=args.n_quantize, mean=corpus.mean, scale=corpus.scale, shuffle=True,
+                                 device=local)
 
 
 def dev_loss(model, utts, batch_samples):
@@ -255,7 +399,11 @@ def _strtobool(v):
 
 def main():
     """RUN TRAINING."""
-    args = get_parser().parse_args()
+    parser = get_parser()
+    args = parser.parse_args()
+    if not args.extract_features and (args.feats is None or args.stats is None):
+        parser.error("the following arguments are required: %s" % ", ".join(
+            f for f, v in (("--feats", args.feats), ("--stats", args.stats)) if v is None))
     fmt = '%(asctime)s (%(module)s:%(lineno)d) %(levelname)s: %(message)s'
     level = logging.INFO if args.verbose == 1 else (logging.DEBUG if args.verbose > 1 else logging.WARNING)
     logging.basicConfig(level=level, format=fmt, datefmt='%m/%d/%Y %I:%M:%S')
@@ -263,6 +411,11 @@ def main():
         logging.warning("logging is disabled.")
     for key, value in vars(args).items():
         logging.info("%s = %s" % (key, str(value)))
+
+    refusal = check_extract_args(args, parser)
+    if refusal is not None:
+        logging.error(refusal)
+        sys.exit(1)
 
     # one process per GPU (torchrun sets RANK / WORLD_SIZE / LOCAL_RANK)
     rank = int(os.environ.get("RANK", 0))
@@ -342,47 +495,10 @@ def main():
     from pytorchwavenetvocoder_b200.optim import Adam
     optimizer = Adam(model.parameters(), lr=args.lr, weight_decay=args.weight_decay, module=model)
 
-    scaler = StandardScaler()
-    scaler.mean_ = read_hdf5(args.stats, "/" + args.feature_type + "/mean")
-    scaler.scale_ = read_hdf5(args.stats, "/" + args.feature_type + "/scale")
-    wav_transform = lambda x: encode_mu_law(x, args.n_quantize)  # noqa: E731
-    feat_transform = lambda x: scaler.transform(x)  # noqa: E731
-
-    if os.path.isdir(args.waveforms):
-        filenames = sorted(find_files(args.waveforms, "*.wav", use_dir_name=False))
-        wav_list = [args.waveforms + "/" + filename for filename in filenames]
-        feat_list = [args.feats + "/" + filename.replace(".wav", ".h5") for filename in filenames]
-    elif os.path.isfile(args.waveforms):
-        wav_list = read_txt(args.waveforms)
-        feat_list = read_txt(args.feats)
+    if args.extract_features:
+        generator, scaler = corpus_generator(args, model, rank, local), None
     else:
-        logging.error("--waveforms should be directory or list.")
-        sys.exit(1)
-    assert len(wav_list) == len(feat_list)
-    logging.info("number of training data = %d." % len(wav_list))
-    if args.batch_length > 0 and not args.host_loader:
-        # mini-batch modes: windowing + mu-law + scaler on the device, utterances uploaded once (utils/device_loader.py);
-        # same batches as train_generator below (tests/test_gpu_loader.py)
-        from pytorchwavenetvocoder_b200.utils.device_loader import DeviceTrainGenerator
-        generator = DeviceTrainGenerator(
-            wav_list, feat_list, model.receptive_field, args.batch_length, args.batch_size,
-            feature_type=args.feature_type, n_quantize=args.n_quantize, mean=scaler.mean_, scale=scaler.scale_,
-            shuffle=True, upsampling_factor=args.upsampling_factor, use_upsampling_layer=args.use_upsampling_layer,
-            use_speaker_code=args.use_speaker_code, device=local)
-    else:
-        generator = train_generator(
-            wav_list, feat_list,
-            receptive_field=model.receptive_field,
-            batch_length=args.batch_length if args.batch_length > 0 else None,
-            batch_size=args.batch_size,
-            feature_type=args.feature_type,
-            wav_transform=wav_transform,
-            feat_transform=feat_transform,
-            shuffle=True,
-            upsampling_factor=args.upsampling_factor,
-            use_upsampling_layer=args.use_upsampling_layer,
-            use_speaker_code=args.use_speaker_code,
-            device=local)
+        generator, scaler = file_generator(args, model, local)
 
     if args.resume is not None and len(args.resume) != 0:
         checkpoint = torch.load(args.resume, map_location=lambda storage, loc: storage, weights_only=False)

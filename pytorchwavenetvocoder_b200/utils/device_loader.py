@@ -12,6 +12,8 @@ times (milliseconds) that thread is the wall.  Here
   the reference's hop arithmetic, mu-law (bit exact), scaler, (frames, D) -> (D, frames) layout, next-sample targets.
 
 Same batches, bit for bit, as ``bin.train.train_generator`` on the same file lists (tests/test_gpu_loader.py).
+``DeviceCorpusGenerator`` yields the same batches from a corpus prepared and kept on the device (utils/corpus.py,
+``wnb_make_train_batch_corpus``), with no files, threads or rings.
 """
 import logging
 import threading
@@ -306,6 +308,114 @@ class DeviceTrainGenerator(object):
                 break
             self._append(*item)
         self.stats["launch_s"] = self.stats.get("launch_s", 0.0) + time.time() - t1
+        return (x, h), t
+
+    __next__ = next
+
+    def __iter__(self):
+        return self
+
+
+def corpus_table(orders, first_epoch, lengths, offsets):
+    """The epoch table ``wnb_make_train_batch_corpus`` searches, for epochs ``first_epoch .. first_epoch + len(orders)
+    - 1`` of the stream (``orders[i]``: the utterance indices of that epoch in stream order): (starts, corpus offsets,
+    table_begin, table_end).  Epoch e starts at stream position e * (sum of lengths); empty utterances take no stream
+    position and are left out, so the starts increase strictly."""
+    L = int(np.sum(lengths))
+    starts, offs = [], []
+    for i, order in enumerate(orders):
+        n = lengths[order]
+        st = (first_epoch + i) * L + np.concatenate([[0], np.cumsum(n)[:-1]])
+        keep = n > 0
+        starts.append(st[keep])
+        offs.append(offsets[order][keep])
+    return (np.concatenate(starts).astype(np.int64), np.concatenate(offs).astype(np.int64), first_epoch * L,
+            (first_epoch + len(orders)) * L)
+
+
+def corpus_index(starts, offsets, p):
+    """Corpus sample of stream positions ``p``: numpy restatement of csrc/loader.cu ``corpus_index`` (the utterance with
+    the largest start <= p)."""
+    k = np.searchsorted(starts, p, side="right") - 1
+    return offsets[k] + (p - starts[k])
+
+
+class DeviceCorpusGenerator(object):
+    """Drop-in for ``DeviceTrainGenerator`` in the up-sampling mini-batch mode, fed by a ``corpus.ResidentCorpus``
+    instead of files: the same ``WindowPlanner`` bookkeeping over the same per-epoch ``np.random.permutation`` draws from
+    the global numpy RNG gives the same sequence of batches, each cut by one ``wnb_make_train_batch_corpus`` launch
+    straight from the resident int16 waveform and float32 frames.  No threads, rings or host copies per batch: the epoch
+    table (stream start and corpus offset of every utterance) is uploaded when a batch reaches past the one on the
+    device, about once per epoch."""
+
+    def __init__(self, corpus, receptive_field, batch_length, batch_size=1, n_quantize=256, mean=None, scale=None,
+                 shuffle=True, device=None):
+        if batch_length is None or batch_length <= 0:
+            raise ValueError("DeviceCorpusGenerator covers the mini-batch mode (batch_length > 0)")
+        self.lib = _lib.load()
+        self.dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
+        self.corpus, self.shuffle, self.B, self.mu = corpus, shuffle, batch_size, n_quantize
+        U = self.U = corpus.U
+        batch_mod = (receptive_field + batch_length) % U             # train.py:99-103, 202-205
+        logging.warning("batch length is decreased due to upsampling (%d -> %d)" % (
+            batch_length, batch_length - batch_mod))
+        batch_length -= batch_mod
+        self.Tf = (receptive_field + batch_length) // U
+        self.T = self.Tf * U
+        self.hop = (batch_length // U) * U
+        self.lengths = np.asarray(corpus.lengths, dtype=np.int64)
+        self.offsets = np.asarray(corpus.offsets, dtype=np.int64)
+        if self.lengths.sum() == 0:
+            raise ValueError("DeviceCorpusGenerator: the corpus has no samples")
+        self.D = corpus.feat.size(1)
+        self.feat_f64 = _f32_scaler_mode()
+        self.mean = None if mean is None else torch.as_tensor(np.asarray(mean, np.float64)).to(self.dev)
+        self.scale = None if scale is None else torch.as_tensor(np.asarray(scale, np.float64)).to(self.dev)
+        self.plan = WindowPlanner(self.B, self.hop, (self.Tf + 1) * U)
+        self._orders = []                                # utterance indices of every epoch drawn so far
+        self._order = np.arange(len(self.lengths))
+        self._fed = 0                                    # utterances handed to the planner
+        self.table = None
+        self.table_span = (0, 0)
+        self.stats = {"batches": 0, "tables": 0}
+
+    def _epoch(self, e):
+        """utterance order of epoch e (reference train.py:95-98, 308-312: a permutation of the current order per epoch)"""
+        while len(self._orders) <= e:
+            if self.shuffle:
+                self._order = self._order[np.random.permutation(len(self._order))]
+            self._orders.append(self._order)
+        return self._orders[e]
+
+    def _upload(self, s0, end):
+        L = int(self.lengths.sum())
+        e0, e1 = s0 // L, (end - 1) // L
+        starts, offs, begin, stop = corpus_table([self._epoch(e) for e in range(e0, e1 + 1)], e0, self.lengths,
+                                                 self.offsets)
+        self.table = torch.from_numpy(np.stack([starts, offs])).to(self.dev)
+        self.table_span = (begin, stop)
+        self.stats["tables"] += 1
+
+    def next(self):
+        N = len(self.lengths)
+        while not self.plan.ready:
+            e, i = divmod(self._fed, N)
+            self.plan.append(int(self.lengths[self._epoch(e)[i]]), i + 1 == N)
+            self._fed += 1
+        s0 = self.plan.ready.pop(0)
+        end = s0 + (self.B - 1) * self.hop + self.T + 1
+        if not (self.table_span[0] <= s0 and end <= self.table_span[1]):
+            self._upload(s0, end)
+        x = torch.empty(self.B, self.T, dtype=torch.int64, device=self.dev)
+        t = torch.empty(self.B, self.T, dtype=torch.int64, device=self.dev)
+        h = torch.empty(self.B, self.D, self.Tf, dtype=torch.float32, device=self.dev)
+        P = _lib.ptr
+        _lib.check(self.lib.wnb_make_train_batch_corpus(
+            P(self.corpus.wave), P(self.corpus.feat), P(self.table[0]), P(self.table[1]), self.table.size(1),
+            self.table_span[0], self.table_span[1], s0, self.hop, self.U, P(self.mean), P(self.scale), P(x), P(t), P(h),
+            self.B, self.T, self.Tf, self.D, self.feat_f64, self.mu, torch.cuda.current_stream(self.dev).cuda_stream),
+            "make_train_batch_corpus")
+        self.stats["batches"] += 1
         return (x, h), t
 
     __next__ = next

@@ -183,6 +183,26 @@ def melspc_batch(signals, fs, fftl, hop, n_mels, fmin=None, fmax=None, highpass_
     kernels do not cover (powers of two from 64 to 4096) raises ``WnbError``."""
     if len(signals) == 0:
         return ([], []) if filtered_int16 else []
+    out, y16, off, foff = melspc_batch_device(signals, fs, fftl, hop, n_mels, fmin=fmin, fmax=fmax,
+                                              highpass_cutoff=highpass_cutoff, filtered_int16=filtered_int16,
+                                              device=device)
+    with torch.cuda.device(out.device):
+        feats = out.cpu().numpy()
+        wavs = y16.cpu().numpy() if y16 is not None else None
+    feats = [feats[foff[i]:foff[i + 1]] for i in range(len(signals))]
+    if filtered_int16:
+        return feats, [wavs[off[i]:off[i + 1]] for i in range(len(signals))]
+    return feats
+
+
+def melspc_batch_device(signals, fs, fftl, hop, n_mels, fmin=None, fmax=None, highpass_cutoff=0, filtered_int16=False,
+                        device=None):
+    """``melspc_batch`` with its results left on the device: (frames, filtered int16 wavs or None, sample offsets,
+    frame offsets).  frames is one float32 CUDA tensor (total frames, n_mels) and the filtered wavs one int16 CUDA
+    tensor (total samples,); utterance i owns rows ``frame_offsets[i]:frame_offsets[i + 1]`` and samples
+    ``offsets[i]:offsets[i + 1]`` (host int64 arrays).  The work is queued on the current stream, not synchronised."""
+    if len(signals) == 0:
+        raise ValueError("melspc: no signals")
     if filtered_int16 and not highpass_cutoff:
         raise ValueError("melspc: filtered wavs need a highpass cutoff (the reference saves them only then)")
     if hop <= 0:
@@ -210,12 +230,7 @@ def melspc_batch(signals, fs, fftl, hop, n_mels, fmin=None, fmax=None, highpass_
         check(load().wnb_melspc(ptr(x), 1 if is_i16 else 0, ptr(offsets), ptr(frame_offsets), len(signals),
                                 int(foff[-1]), int(fftl), int(hop), ptr(window), ptr(tw), ptr(mel), ptr(mlo), ptr(mhi),
                                 int(n_mels), ptr(out), stream()), "melspc")
-        feats = out.cpu().numpy()
-        wavs = y16.cpu().numpy() if y16 is not None else None
-    feats = [feats[foff[i]:foff[i + 1]] for i in range(len(signals))]
-    if filtered_int16:
-        return feats, [wavs[off[i]:off[i + 1]] for i in range(len(signals))]
-    return feats
+    return out, y16, off, foff
 
 
 # ---- streaming (DESIGN.md §6 row f7) --------------------------------------------------------------------------------

@@ -47,7 +47,6 @@ def mlsa_filter_batch(signals, coef, alpha, pd=4, out_int16=None, device=None):
     if len(signals) == 0:
         return []
     dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-    coef = np.ascontiguousarray(coef, dtype=np.float64)
     is_i16 = all(np.asarray(s).dtype == np.int16 for s in signals)
     if out_int16 is None:
         out_int16 = is_i16
@@ -59,15 +58,28 @@ def mlsa_filter_batch(signals, coef, alpha, pd=4, out_int16=None, device=None):
     if off[-1] == 0:
         return [np.zeros(0, dtype=np.int16 if out_int16 else np.float64) for _ in signals]
     with torch.cuda.device(dev):
-        x = torch.from_numpy(flat).to(dev)
-        offsets = torch.from_numpy(off).to(dev)
-        b = torch.from_numpy(coef).to(dev)
-        y = torch.empty(int(off[-1]), dtype=torch.int16 if out_int16 else torch.float64, device=dev)
-        check(load().wnb_mlsa_filter(ptr(x), 1 if is_i16 else 0, ptr(offsets), len(signals), ptr(b), len(coef) - 1,
-                                     float(alpha), int(pd), float(np.exp(coef[0])), ptr(y), 1 if out_int16 else 0, stream()),
-              "mlsa_filter")
+        y = mlsa_filter_device(torch.from_numpy(flat).to(dev), off, coef, alpha, pd=pd, out_int16=out_int16)
         yh = y.cpu().numpy()
     return [yh[off[i]:off[i + 1]] for i in range(len(signals))]
+
+
+def mlsa_filter_device(x, offsets, coef, alpha, pd=4, out_int16=False):
+    """``mlsa_filter_batch`` of signals already on the device: x is one int16 or float64 CUDA tensor holding the signals
+    back to back, signal i at ``offsets[i]:offsets[i + 1]`` (host int64 array, offsets[-1] == x.numel() > 0).  Returns
+    the filtered CUDA tensor of the same length (int16 with ``out_int16``, float64 otherwise), queued on the current
+    stream."""
+    coef = np.ascontiguousarray(coef, dtype=np.float64)
+    off = np.ascontiguousarray(offsets, dtype=np.int64)
+    if x.dtype not in (torch.int16, torch.float64) or x.dim() != 1 or off[-1] != x.numel() or x.numel() == 0:
+        raise ValueError("MLSA filter: x should be a non-empty 1-D int16 or float64 tensor of offsets[-1] samples")
+    with torch.cuda.device(x.device):
+        d_off = torch.from_numpy(off).to(x.device)
+        b = torch.from_numpy(coef).to(x.device)
+        y = torch.empty(x.numel(), dtype=torch.int16 if out_int16 else torch.float64, device=x.device)
+        check(load().wnb_mlsa_filter(ptr(x), 1 if x.dtype == torch.int16 else 0, ptr(d_off), len(off) - 1, ptr(b),
+                                     len(coef) - 1, float(alpha), int(pd), float(np.exp(coef[0])), ptr(y),
+                                     1 if out_int16 else 0, stream()), "mlsa_filter")
+    return y
 
 
 class MlsaStreamFilter(object):
