@@ -330,8 +330,8 @@ WNB_API int wnb_zero(void* p, size_t bytes, void* stream);
 #define WNB_PROF_FWD_BLOCK 0   /* resblock_fwd_z: one residual block, deferred-skip form */
 #define WNB_PROF_SKIP_GEMM 1   /* skip = Z_all Wskip^T */
 #define WNB_PROF_DZALL_GEMM 2  /* dZ_all = dskip Wskip */
-#define WNB_PROF_GATE_BWD 3    /* gate recompute + dz + dpre */
-#define WNB_PROF_DX_GEMM 4     /* dx (+ dhaux) */
+#define WNB_PROF_GATE_BWD 3    /* the stack backward's block chain: last gate backward, dx_l + gate backward of block l-1, dx_0 */
+#define WNB_PROF_DX_GEMM 4     /* dx (+ dhaux) (no longer launched on its own: part of WNB_PROF_GATE_BWD) */
 #define WNB_PROF_DW1 5         /* dW1, db1 (no longer launched on its own: part of WNB_PROF_WGRAD) */
 #define WNB_PROF_DW2RES 6      /* dW2res, db2res (part of WNB_PROF_WGRAD) */
 #define WNB_PROF_DWSKIP 7      /* dWskip, dbskip (part of WNB_PROF_WGRAD) */

@@ -9,7 +9,8 @@
 //   forward    z_l -> Z_all[:, :, l*R:(l+1)*R]     (resblock_z.cu writes the slice)
 //              skip  = Z_all Wskip^T + bskip        one NT GEMM, K = L*R          (Wskip[s][l*R+c] = W2_l[R+s][c])
 //   backward   dZ_all = dskip Wskip                  one NT GEMM, N = L*R in column blocks (A tile shared via L2)
-//              per block: gate recompute + dz_l = dZ_all[l] + dout W2res_l + gate backward (one GEMM) ; dx
+//              per block: gate recompute + dz_l = dZ_all[l] + dout W2res_l + gate backward (one GEMM) ; dx, which is
+//              the dout of the block below: dx_l and block l-1's gate backward run as one launch (stack_bwd_chain.cu)
 //              dW1_l, dW2res_l of ALL blocks: one segmented weight-gradient launch each (dpre_l, dx_l are kept)
 //              dWskip = dskip^T Z_all                one weight-gradient GEMM, column groups of Z_all across CTAs
 //
@@ -30,8 +31,9 @@ static int pick_block(int total, const int* cands, int n) {
 }
 
 // Consecutive kernels of the block chain walk the time tiles in opposite directions (forward: odd blocks backwards;
-// backward: gate backward front to back, dX back to front), so each starts on the rows its producer wrote last -- still
-// in the 50 MB L2 -- instead of on the ones written a tensor ago.  WNB_ALT_DIR=0: every kernel front to back.
+// backward: the chain launches alternately front to back and back to front), so each starts on the rows its producer
+// wrote last -- still in the 50 MB L2 -- instead of on the ones written a tensor ago.  WNB_ALT_DIR=0: every kernel front
+// to back.
 static int alternate_dir() {
   static const int on = [] { const char* e = getenv("WNB_ALT_DIR"); return (e && e[0] == '0') ? 0 : 1; }();
   return on;
@@ -156,46 +158,56 @@ WNB_API int wnb_stack_bwd(const float* xs, const float* haux, const float* zall,
       return rc;
   }
 
-  const float* dout = nullptr;   // gradient w.r.t. the block's residual output (none for the last block)
-  for (int l = L - 1; l >= 0; l--) {
-    const int d = dilations[l];
+  // The block chain in L + 1 launches: the gate backward of the last block alone, then one stack_bwd_chain launch per
+  // block boundary l = L-1 .. 1 (dx_l, fed from shared memory straight into the gate backward of block l-1 as its dout),
+  // then dx_0 alone.  Launch k walks the time tiles in direction k & 1.
+  auto dpre_of = [&](int l) { return dpre_all + (size_t)l * bt * 2 * R; };
+  auto dx_of = [&](int l) { return l == 0 ? dx0 : dx_all + (size_t)l * xsz; };
+  auto wgate_of = [&](int l) { return wgate + (size_t)l * 3 * R * (K1 + R); };
+  auto rev = [&](int launch) { return alternate_dir() ? (launch & 1) : 0; };
+  {  // gate recompute (pre = W1 [x(t-d) | x(t) | aux]) and dz = dZ_all[L-1] -> dpre_{L-1}.  With a dout (the chain
+     // kernel) the GEMM runs over the block matrix wgate_l = [[W1, 0], [0, W2res^T]] (3R x (K1+R)): accumulator
+     // columns 2R..3R-1 are then the residual part of dz, dout W2res_l.
+    const int l = L - 1, d = dilations[l];
     const float* xin = xs + (size_t)l * xsz;
-    const float* w1tl = w1t + (size_t)l * K1 * 2 * R;
-    float* dzl = dzall + (size_t)l * R;          // (B,T,R) view with row pitch ldz
-    float* dxin = (l == 0) ? dx0 : dx_all + (size_t)l * xsz;
-    float* dpre = dpre_all + (size_t)l * bt * 2 * R;
-    {  // gate recompute (pre = W1 [x(t-d) | x(t) | aux]) and dz_l = dZ_all[l] + dout W2res_l in ONE GEMM over the block
-       // matrix wgate_l = [[W1, 0], [0, W2res^T]] (3R x (K1+R)): accumulator columns 0..2R-1 are the gate
-       // pre-activations, columns 2R..3R-1 the residual part of dz; the epilogue turns both into dpre.
-      const float* wg = wgate + (size_t)l * 3 * R * (K1 + R);
-      const NtTcSeg sg[4] = {{xin, R, -d, R, wg, 3 * R, K1 + R, 0, 0}, {xin, R, 0, R, wg, 3 * R, K1 + R, R, 0},
-                             {haux, Ap, 0, Ap, wg, 3 * R, K1 + R, 2 * R, 0}, {dout, R, 0, R, wg, 3 * R, K1 + R, K1, 0}};
-      const NtTcOpts o{1, ldz, 1, dout ? 1 : 0};
-      ProfScope ps(WNB_PROF_GATE_BWD, st);
-      if ((rc = gemm_nt_tc(sg, dout ? 4 : 3, dout ? 3 * R : 2 * R, dxin /* z output suppressed */, R,
-                           b1 + (size_t)l * 2 * R, nullptr, 0, nullptr, 0, 0, 0, B, T, st, dzl, dpre, nullptr, 0, 0,
-                           nullptr, &o)) != WNB_OK)
-        return rc;
-    }
-    // dxin = dout + dpre(t+d) W1[:, tap0] + dpre(t) W1[:, tap1]   and   dhaux += dpre(t) W1[:, aux]
+    const float* wg = wgate_of(l);
+    const NtTcSeg sg[3] = {{xin, R, -d, R, wg, 3 * R, K1 + R, 0, 0}, {xin, R, 0, R, wg, 3 * R, K1 + R, R, 0},
+                           {haux, Ap, 0, Ap, wg, 3 * R, K1 + R, 2 * R, 0}};
+    const NtTcOpts o{1, ldz, 1, 0, rev(0)};
+    ProfScope ps(WNB_PROF_GATE_BWD, st);
+    if ((rc = gemm_nt_tc(sg, 3, 2 * R, dx_of(l) /* z output suppressed */, R, b1 + (size_t)l * 2 * R, nullptr, 0,
+                         nullptr, 0, 0, 0, B, T, st, dzall + (size_t)l * R, dpre_of(l), nullptr, 0, 0, nullptr, &o)) !=
+        WNB_OK)
+      return rc;
+  }
+  // dx_l = dx_{l+1} + dpre_l(t+d) W1_l[:, tap0] + dpre_l(t) W1_l[:, tap1]   and   dhaux += dpre_l(t) W1_l[:, aux]
+  for (int l = L - 1; l >= 1; l--) {
+    ProfScope ps(WNB_PROF_GATE_BWD, st);
+    if ((rc = stack_bwd_chain(dpre_of(l), w1t + (size_t)l * K1 * 2 * R, l + 1 < L ? dx_of(l + 1) : nullptr, dx_of(l),
+                              dhaux, xs + (size_t)(l - 1) * xsz, haux, wgate_of(l - 1), b1 + (size_t)(l - 1) * 2 * R,
+                              dzall + (size_t)(l - 1) * R, ldz, dpre_of(l - 1), B, T, dilations[l], dilations[l - 1],
+                              rev(L - l), st)) != WNB_OK)
+      return rc;
+  }
+  {  // dx_0 (the same products and K order as the chain kernel's dX)
+    const int d = dilations[0];
+    const float* dpre = dpre_of(0);
+    const float* dout = L > 1 ? dx_of(1) : nullptr;
+    const NtTcOpts ox{1, 0, 0, 0, rev(L)};
+    ProfScope ps(WNB_PROF_GATE_BWD, st);
     if (dhaux) {
-      ProfScope ps(WNB_PROF_DX_GEMM, st);
       // (the shifted segment sees w1t as an R-row matrix: its rows R.. are TMA zero fill, only the unshifted tap feeds the
       //  aux columns)
-      const NtTcSeg sx[2] = {{dpre, 2 * R, 0, 2 * R, w1tl, K1, 2 * R, 0, R}, {dpre, 2 * R, d, 2 * R, w1tl, R, 2 * R, 0, 0}};
-      const NtTcOpts ox{1, 0, 0, 0, alternate_dir()};
-      if ((rc = gemm_nt_tc(sx, 2, R + Ap, dxin, R, nullptr, nullptr, 0, dout, R, 0, 0, B, T, st, nullptr, nullptr, dhaux,
+      const NtTcSeg sx[2] = {{dpre, 2 * R, 0, 2 * R, w1t, K1, 2 * R, 0, R}, {dpre, 2 * R, d, 2 * R, w1t, R, 2 * R, 0, 0}};
+      if ((rc = gemm_nt_tc(sx, 2, R + Ap, dx0, R, nullptr, nullptr, 0, dout, R, 0, 0, B, T, st, nullptr, nullptr, dhaux,
                            Ap, R, nullptr, &ox)) != WNB_OK)
         return rc;
     } else {
-      ProfScope ps(WNB_PROF_DX_GEMM, st);
-      const NtTcSeg sx[2] = {{dpre, 2 * R, d, 2 * R, w1tl, K1, 2 * R, 0, 0}, {dpre, 2 * R, 0, 2 * R, w1tl, K1, 2 * R, 0, R}};
-      const NtTcOpts ox{1, 0, 0, 0, alternate_dir()};
-      if ((rc = gemm_nt_tc(sx, 2, R, dxin, R, nullptr, nullptr, 0, dout, R, 0, 0, B, T, st, nullptr, nullptr, nullptr, 0, 0,
+      const NtTcSeg sx[2] = {{dpre, 2 * R, d, 2 * R, w1t, K1, 2 * R, 0, 0}, {dpre, 2 * R, 0, 2 * R, w1t, K1, 2 * R, 0, R}};
+      if ((rc = gemm_nt_tc(sx, 2, R, dx0, R, nullptr, nullptr, 0, dout, R, 0, 0, B, T, st, nullptr, nullptr, nullptr, 0, 0,
                            nullptr, &ox)) != WNB_OK)
         return rc;
     }
-    dout = dxin;
   }
 
   // The three weight gradients only read tensors that exist by now and do not depend on each other: ONE problem list,

@@ -62,6 +62,15 @@ int gemm_nt_tc(const NtTcSeg* segs, int nseg, int N, float* out, int ld_out, con
                const float* gate_dz = nullptr, float* gate_dpre = nullptr, float* out2 = nullptr, int ld_out2 = 0,
                int out2_col0 = 0, const NtTcGate* gate = nullptr, const NtTcOpts* opts = nullptr);
 
+// ---- one block boundary of the stack backward (stack_bwd_chain.cu; R = 64, Ap = 32, ks = 2) ----------------------
+// dx = dx_next + dpre(t) W1[:, tap1] + dpre(t+d) W1[:, tap0] (dx_next null: no residual), dhaux += dpre(t) W1[:, aux]
+// (dhaux null: not computed), then the gate backward of the block below with dout = dx: gate recompute from
+// [xprev(t-d_prev) | xprev(t) | haux] and dz = dz_prev (row pitch ldz) + dx W2res through wgate_prev, dpre_prev out.
+// Bit-identical to gemm_nt_tc's dX launch followed by its N = 192 gate-backward launch.
+int stack_bwd_chain(const float* dpre, const float* w1t, const float* dx_next, float* dx, float* dhaux, const float* xprev,
+                    const float* haux, const float* wgate_prev, const float* b1_prev, const float* dz_prev, int ldz,
+                    float* dpre_prev, int B, int T, int d, int d_prev, int reverse, cudaStream_t st);
+
 // ---- fused residual block, deferred-skip form (resblock_z.cu) --------------------------------------------------
 bool resblock_fwd_z_supported(int R, int Ap, int ks);
 int resblock_fwd_z(const float* xin, const float* haux, const float* w1, const float* b1, const float* w2res,
