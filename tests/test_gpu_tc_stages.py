@@ -33,6 +33,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests import stack_shapes as SS
 from tests import tc_reference as ref
 
 pytestmark = pytest.mark.gpu
@@ -135,31 +136,29 @@ def _empty_range_T(L, S, B, sms):
 
 
 def _case(name):
-    bench = [2 ** i for i in range(10)] * 3
-    if name == "a":
-        return 1, 32, 1, 1, [1]
-    if name == "b":
-        return 3, 96, 2, 95, [1, 64, 200]
-    if name == "c":
-        return 5, 512, 3, 1040, [1, 2, 4, 8, 16]
-    if name == "d":
-        L, S, B = 22, 256, 1
-        return L, S, B, _empty_range_T(L, S, B, _sms()), [2 ** (i % 10) for i in range(L)]
-    if name == "e":
-        return 30, 512, 2, 8300, bench
-    if name == "f":
-        return 64, 128, 1, 200, [(37 * i) % 300 + 1 for i in range(64)]
-    raise KeyError(name)
+    """the case's row of tests/stack_shapes.py; case d's T is the smallest that gives a weight-gradient CTA of each
+    launch an empty time range on this device"""
+    row = SS.STACK_ROWS["case_" + name]
+    L, S, B, T = row["L"], row["S"], row["B"], row["T"]
+    return L, S, B, (T if T is not None else _empty_range_T(L, S, B, _sms())), row["dilations"]
 
 
 @pytest.mark.parametrize("relu", [0, 1])
 @pytest.mark.parametrize("case", ["a", "b", "c", "d", "e", "f"])
 def test_stack_stages(case, relu):
-    L_, lib = _lib()
     L, S, B, T, dil = _case(case)
+    _stack_stages(L, S, B, T, dil, relu, True, 1000 + ord(case) + relu,
+                  "stack_%s_relu%d_L%d_S%d_B%d_T%d" % (case, relu, L, S, B, T))
+
+
+def _stack_stages(L, S, B, T, dil, relu, aux, seed, name, repeat_bwd=False, check=True):
+    """``wnb_stack_fwd`` + ``wnb_stack_bwd`` on random operands, every stage checked against float64 (check=False: run
+    only).  aux=False: dhaux is NULL (a model without an up-sampling layer) and not checked.  repeat_bwd: a second
+    backward from the same inputs must give bit-identical gradients and workspace.  Returns every output."""
+    L_, lib = _lib()
     assert lib.wnb_stack_supported(R, S, AP, KS, L, L_.MATH_TF32)
     K1 = KS * R + AP
-    g = torch.Generator(device="cuda").manual_seed(1000 + ord(case) + relu)
+    g = torch.Generator(device="cuda").manual_seed(seed)
     rn = lambda *sh: torch.randn(*sh, device="cuda", generator=g)   # noqa: E731
     w1 = rn(L, 2 * R, K1) / math.sqrt(K1)
     b1 = 0.2 * rn(L, 2 * R)
@@ -185,16 +184,31 @@ def test_stack_stages(case, relu):
     wskt = wskip.t().contiguous()
     init = dict(dhaux=rn(B, T, AP), dw1=rn(L, 2 * R, K1), db1=rn(L, 2 * R), dw2res=rn(L, R, R), db2res=rn(L, R),
                 dwskip=rn(S, L * R), dbskip=rn(S))
-    out = {k: G(tuple(v.shape), v) for k, v in init.items()}
-    dx0 = G((B, T, R))
-    ws = G((lib.wnb_stack_bwd_workspace(L, B, T, R, S, AP, KS) // 4,))
-    L_.check(lib.wnb_stack_bwd(L_.ptr(xs), L_.ptr(haux), L_.ptr(zall), L_.ptr(dskip), L_.ptr(w1), L_.ptr(b1),
-                               L_.ptr(w1t), L_.ptr(wgate), L_.ptr(wskt), L_.ptr(dx0), L_.ptr(out["dhaux"]),
-                               L_.ptr(out["dw1"]), L_.ptr(out["db1"]), L_.ptr(out["dw2res"]), L_.ptr(out["db2res"]),
-                               L_.ptr(out["dwskip"]), L_.ptr(out["dbskip"]), L_.ptr(ws), dils, L, B, T, R, S, AP, KS,
-                               L_.stream()), "stack_bwd")
+    if not aux:
+        del init["dhaux"]
+
+    def backward():
+        out = {k: G(tuple(v.shape), v) for k, v in init.items()}
+        dx0 = G((B, T, R))
+        ws = G((lib.wnb_stack_bwd_workspace(L, B, T, R, S, AP, KS) // 4,))
+        L_.check(lib.wnb_stack_bwd(L_.ptr(xs), L_.ptr(haux), L_.ptr(zall), L_.ptr(dskip), L_.ptr(w1), L_.ptr(b1),
+                                   L_.ptr(w1t), L_.ptr(wgate), L_.ptr(wskt), L_.ptr(dx0), L_.ptr(out.get("dhaux")),
+                                   L_.ptr(out["dw1"]), L_.ptr(out["db1"]), L_.ptr(out["dw2res"]), L_.ptr(out["db2res"]),
+                                   L_.ptr(out["dwskip"]), L_.ptr(out["dbskip"]), L_.ptr(ws), dils, L, B, T, R, S, AP, KS,
+                                   L_.stream()), "stack_bwd")
+        return out, dx0, ws
+    out, dx0, ws = backward()
+    if repeat_bwd:     # a second backward from the same inputs: bit-identical (fixed summation order)
+        out2, dx02, ws2 = backward()
+        assert torch.equal(dx02, dx0), "dx0 differs between two backward runs"
+        assert torch.equal(ws2.nan_to_num(SENTINEL), ws.nan_to_num(SENTINEL)), "workspace differs between two runs"
+        for k in out:
+            assert torch.equal(out2[k], out[k]), "%s differs between two backward runs" % k
     torch.cuda.synchronize()
     G.check()
+    result = dict(xs=xs, zall=zall, skip=skip, dx0=dx0, ws=ws, **out)
+    if not check:
+        return result
     W = stack_bwd_workspace_views(ws, L, B, T, R)
     log = Log()
 
@@ -225,13 +239,15 @@ def test_stack_stages(case, relu):
                                            init["db2res"][l])
             log("dW2res[block %d]" % l, out["dw2res"][l], (dw, bw))
             log("db2res[block %d]" % l, out["db2res"][l], (db, bb))
-    log("dhaux", out["dhaux"], ref.accumulate(init["dhaux"], dh_parts))
+    if aux:
+        log("dhaux", out["dhaux"], ref.accumulate(init["dhaux"], dh_parts))
     assert torch.equal(out["dw2res"][L - 1], init["dw2res"][L - 1]) and torch.equal(out["db2res"][L - 1],
                                                                                       init["db2res"][L - 1])
     (dw, bw), (db, bb) = ref.wgrad(dskip, [zall], init["dwskip"], init["dbskip"])
     log("dWskip", out["dwskip"], (dw, bw))
     log("dbskip", out["dbskip"], (db, bb))
-    _report("stack_%s_relu%d_L%d_S%d_B%d_T%d" % (case, relu, L, S, B, T), log.res)
+    _report(name, log.res)
+    return result
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -275,7 +291,7 @@ def test_block_z_and_skip_gemm(d, T, last):
 # ------------------------------------------------------------------------------------------------------------------
 # per-block tf32 entries: the fused kernel (R = 64) and the composed path
 # ------------------------------------------------------------------------------------------------------------------
-def _perblock(R_, S, Ap, ks, d, B, T, last, init, seed, repeat_bwd=False):
+def _perblock(R_, S, Ap, ks, d, B, T, last, init, seed, repeat_bwd=False, dhaux=True):
     L_, lib = _lib()
     g = torch.Generator(device="cuda").manual_seed(seed)
     rn = lambda *sh: torch.randn(*sh, device="cuda", generator=g)   # noqa: E731
@@ -297,13 +313,15 @@ def _perblock(R_, S, Ap, ks, d, B, T, last, init, seed, repeat_bwd=False):
     dskip = rn(B, T, S)
     w1t, w2t = w1.t().contiguous(), w2.t().contiguous()
     ginit = dict(dh=rn(B, T, Ap), dw1=rn(2 * R_, K1), db1=rn(2 * R_), dw2=rn(R_ + S, R_), db2=rn(R_ + S))
+    if not dhaux:      # dhaux NULL: the backward computes no aux gradient
+        del ginit["dh"]
 
     def backward():
         gout = {k: G(tuple(v.shape), v) for k, v in ginit.items()}
         dx = G((B, T, R_))
         ws = G((lib.wnb_resblock_bwd_workspace(B, T, R_, S, Ap, ks) // 4,))
         L_.check(lib.wnb_resblock_bwd(L_.ptr(xin), L_.ptr(haux), L_.ptr(dout), L_.ptr(dskip), L_.ptr(w1), L_.ptr(b1),
-                                      L_.ptr(w1t), L_.ptr(w2t), L_.ptr(dx), L_.ptr(gout["dh"]), L_.ptr(gout["dw1"]),
+                                      L_.ptr(w1t), L_.ptr(w2t), L_.ptr(dx), L_.ptr(gout.get("dh")), L_.ptr(gout["dw1"]),
                                       L_.ptr(gout["db1"]), L_.ptr(gout["dw2"]), L_.ptr(gout["db2"]), L_.ptr(ws),
                                       B, T, R_, S, Ap, ks, d, L_.MATH_TF32, L_.stream()), "resblock_bwd")
         return gout, dx, ws
@@ -332,7 +350,8 @@ def _perblock(R_, S, Ap, ks, d, B, T, last, init, seed, repeat_bwd=False):
     dz, e_dz = ref.dz_perblock(dout, dskip, w2)
     log("dpre", dpre, ref.gate_bwd(xin, haux, w1, b1, d, ks, dz, e_dz))
     log("dx", dx, ref.dx_stage(dpre, w1, d, ks, dout))
-    log("dhaux", gout["dh"], ref.accumulate(ginit["dh"], [ref.dhaux_stage(dpre, w1, ks)]))
+    if dhaux:
+        log("dhaux", gout["dh"], ref.accumulate(ginit["dh"], [ref.dhaux_stage(dpre, w1, ks)]))
     (dw, bw), (db, bb) = ref.wgrad(dpre, ref.taps(xin, ks, d) + [haux], ginit["dw1"], ginit["db1"])
     log("dW1", gout["dw1"], (dw, bw))
     log("db1", gout["db1"], (db, bb))
@@ -343,8 +362,9 @@ def _perblock(R_, S, Ap, ks, d, B, T, last, init, seed, repeat_bwd=False):
     log("db2", gout["db2"][r0:], (db, bb))
     if last:
         assert torch.equal(gout["dw2"][:R_], ginit["dw2"][:R_]) and torch.equal(gout["db2"][:R_], ginit["db2"][:R_])
-    _report("perblock_R%d_S%d_Ap%d_ks%d_d%d_B%d_T%d%s%s" % (R_, S, Ap, ks, d, B, T, "_last" if last else "",
-                                                             "_init" if init else ""), log.res)
+    _report("perblock_R%d_S%d_Ap%d_ks%d_d%d_B%d_T%d%s%s%s" % (R_, S, Ap, ks, d, B, T, "_last" if last else "",
+                                                               "_init" if init else "", "" if dhaux else "_nodhaux"),
+            log.res)
     return kind
 
 
